@@ -1,6 +1,6 @@
-# Build the sm_100a CUDA library (C-ABI) and the CPU oracle.  nvcc cross-compiles without a GPU.
+# Build the sm_90a CUDA library (C-ABI) and the CPU oracle.  nvcc cross-compiles without a GPU.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function --expt-relaxed-constexpr -Iinclude -Icrazyara_b200/csrc
 CSRC      := crazyara_b200/csrc
 CU_SRCS   := $(wildcard $(CSRC)/*.cu)

@@ -2,7 +2,7 @@
 """bench.py -- headline benchmark: MCTS simulations/sec (NPS), crazyhouse start position, Batch_Size 64.
 
 One "step" = one complete search (`go`) of --sims simulations with a fresh tree: root evaluation, then mini-batch
-iterations of select -> RISE conv stack (tcgen05) -> scatter / backup, all device-resident.  NPS is computed exactly like
+iterations of select -> RISE conv stack (wgmma) -> scatter / backup, all device-resident.  NPS is computed exactly like
 the reference: (root.visitSum - root.freeVisits) / elapsed (engine/src/evalinfo.cpp:73-85, node.cpp:1303-1306).
 
   --threads 2 (default): the reference's UCI default `Threads 2` (uci/optionsuci.cpp:182) -- two logical search threads
@@ -328,7 +328,7 @@ def selfplay_config_main(args, rank, local_rank, world):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
         conv_tf = tot[2] / world * net_flops_per_position(arch) / 1e12  # per GPU: evaluated nodes/s x FLOP per position
         print(json.dumps({
             "metric": metric, "value": tot[0], "unit": "games/h", "n_gpus": world, "steps": 1, "warmup": 1,
@@ -344,6 +344,20 @@ def selfplay_config_main(args, rank, local_rank, world):
                          "achieved_from": "searched nodes per second x FLOP per position (per GPU, over the wall time of the arena)"}}))
     if dist is not None:
         dist.destroy_process_group()
+
+
+def dump_search_result(r, out_dir):
+    """What a caller of the timed path receives from its last search (EvalInfo of the root): per-move arrays in the
+    root's move order, and the scalar results.  The inputs are fixed (start position, seeded weights, deterministic search
+    schedule), so two builds can be compared file by file."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"visits": np.asarray(r["visits"], np.float64), "q": np.asarray(r["q"], np.float32),
+              "prior": np.asarray(r["prior"], np.float32), "policy": np.asarray(r["policy"], np.float64),
+              "scalars": np.array([r["root_value"], r["best_move_q"], r["visit_sum"], r["free_visits"], r["nodes"],
+                                   r["best_idx"], r["evals"]], np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def search_leg(agent, net, steps, flush):
@@ -380,7 +394,11 @@ def main():
     ap.add_argument("--trees", type=int, default=32, help="extra leg: concurrent searches per GPU (0 = skip)")
     ap.add_argument("--selfplay-seconds", type=float, default=8.0, help="extra leg: self-play arena window (0 = skip)")
     ap.add_argument("--selfplay-games", type=int, default=64)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed search returned as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -438,7 +456,7 @@ def main():
     settings = default_settings(mode, batch_size=batch, simulations=sims, threads=args.threads, input_version=version)
     agent = MCTSAgent(net, settings, local_rank, 1)
     agent._bench_variant = vid
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > the 50 MB L2
 
     search_leg(agent, net, args.warmup, flush)
     launches0 = agent.launch_count() + net.launch_count()
@@ -449,6 +467,8 @@ def main():
     torch.cuda.synchronize()
     nodes, dev_ms, wall_s, last = search_leg(agent, net, args.steps, flush)
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_search_result(last, args.dump_outputs)
     if dist is not None:
         dist.barrier()
     sampler.stop_flag = True
@@ -508,20 +528,11 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback 1.4 PFLOP/s sustained"
+        peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+        peak_src = ("measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else
+                    "H100 SXM data sheet, 989 TFLOP/s dense fp16 / bf16 (not a measured rate)")
         # achieved = the FLOPs of the leaves the search evaluated (not of the padded rows of its forwards) / forward time
         conv_tflops = evals * flops_pos / (net_ms * 1e-3) / 1e12 if net_ms > 0 else 0.0
-        traffic = None  # DRAM bytes per launch of the dominant tensor kernel, from the committed `ncu --set full` capture
-        for prof_file in ("r02_ncu_trunk_pair.json", "r02_ncu_trunk.json", "r01_ncu_rise_trunk_kernel.json"):
-            try:
-                k = json.load(open(os.path.join(ROOT, "profiles", prof_file)))["kernels"][0]
-                scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-                traffic = (k["dram__bytes_read.sum"] * scale[k["dram__bytes_read.sum unit"]] +
-                           k["dram__bytes_write.sum"] * scale[k["dram__bytes_write.sum unit"]])
-                break
-            except Exception:
-                pass
         value = total_nodes / (max_dev_ms * 1e-3)
         e2e_value = total_nodes / max_wall
         out = {
@@ -539,12 +550,10 @@ def main():
             "gpu_launches": int(launches),
             "clocks": sampler.summary(),
             "roofline": {"bound": "tensor", "achieved": conv_tflops, "peak": peak_tf, "unit": "TFLOP/s",
-                         "frac": conv_tflops / peak_tf if peak_tf else None, "traffic": traffic,
-                         "traffic_note": "rise_trunk_c_kernel, one launch of 64 positions, dram__bytes_read+write "
-                                         "(profiles/r02_ncu_trunk_pair.json; cold L2: the weights + the input tile)",
-                         "kernel": f"{net_name} conv stack per forward of {batch} positions: rise_trunk_c_kernel (all bottleneck "
-                                   "blocks on CTA pairs, tcgen05 SS MMAs with the channels in M, one launch) + stem/policy "
-                                   "conv_gemm_kernel + head kernels",
+                         "frac": conv_tflops / peak_tf if peak_tf else None, "traffic": None,
+                         "kernel": f"{net_name} conv stack per forward of {batch} positions: rise_trunk_kernel (all bottleneck "
+                                   "blocks, one warpgroup per board, wgmma, one launch) + stem/policy conv_gemm_kernel + "
+                                   "head kernels",
                          "achieved_from": "evaluated leaves x FLOP per position / device time of the forwards",
                          "flop_per_position": flops_pos, "peak_source": peak_src},
         }
@@ -553,13 +562,13 @@ def main():
             # (Q, n, P, vl) at every tree level -- a dependent pointer chase, so far below the HBM peak by nature
             if args.threads == 1:
                 sel_bytes = 32.0 * float(last.get("sum_depth", 0)) + 13.0 * float(last.get("sum_select_k", 0))
-                hbm_peak = float(peaks.get("hbm_gbs", 6500.0))
+                hbm_peak = float(peaks.get("hbm_gbs", 3350.0))  # H100 SXM data sheet when not measured
                 sel_gbs = sel_bytes / (sel_ms * 1e-3) / 1e9 if sel_ms > 0 else 0.0
                 out["roofline_select"] = {"bound": "hbm", "achieved": sel_gbs, "peak": hbm_peak, "unit": "GB/s",
                                           "frac": sel_gbs / hbm_peak if hbm_peak else None,
                                           "algorithmic_bytes_per_search": sel_bytes,
                                           "note": "select_kernel: one warp per tree, one dependent L2/HBM round trip per tree "
-                                                  "level; latency-bound (profiles/r01_ncu_select_kernel.json)"}
+                                                  "level; latency-bound"}
         except Exception:
             pass
         if world == 1 and not args.no_cpu_baseline:

@@ -1,4 +1,4 @@
-"""crazyara_b200: B200-native (sm_100a) MCTS + neural-network leaf evaluation engine.
+"""crazyara_b200: H100-native (sm_90a) MCTS + neural-network leaf evaluation engine.
 
 Hot path of QueensGambit/CrazyAra rebuilt as hand-written CUDA behind a C-ABI (include/ara_b200.h).
 """

@@ -1,4 +1,4 @@
-"""ctypes loader for the sm_100a C-ABI library (include/ara_b200.h).
+"""ctypes loader for the sm_90a C-ABI library (include/ara_b200.h).
 
 There is deliberately no CPU fallback: if the CUDA library is missing the import of any product
 entry point raises (the oracle under oracle/ is test infrastructure and is never used from here).

@@ -1,4 +1,4 @@
-// Convolution-as-GEMM on the 5th-gen tensor cores (tcgen05.mma, TMEM accumulators, TMA operand feeds).
+// Convolution-as-GEMM on the Hopper tensor cores (wgmma, register accumulators, TMA operand feeds).
 //
 // Computes, for a batch of 8x8 boards stored NHWC in fp16,
 //     out[m, n] = epi( sum_{tap, c} act[board(m), sq(m)+tap, c] * w[n, tap*cw + c] + bias[n] )
@@ -10,15 +10,16 @@
 // is ONE 4-D TMA box {64 ch, 8 files, 8 ranks, 2 boards} fetched at coordinates (c0, dx, dy, 2*m_tile):
 // the halo of the 3x3 taps falls outside the tensor and is zero-filled by the TMA unit, so the 3x3
 // convolutions are implicit GEMMs with no im2col buffer.  Both operands land K-major with the 128-byte
-// swizzle; the MMA is issued by one elected thread; four epilogue warps drain TMEM (one row per thread).
+// swizzle; two consumer warpgroups (one board = 64 rows each) run wgmma M=64 N=BN on the staged tiles and apply the
+// epilogue straight from their accumulator registers, one producer warp keeps the TMA ring full.
 //
 // Precision float32 (the reference's `Precision float32`, uci/optionsuci.cpp:144, nn/tensorrtapi.cpp:334-360) runs on
 // the SAME kernel: an fp32 value x is carried as the fp16 pair hi = fp16(x), lo = fp16(x - hi), activations are stored
 // with their channels tripled [hi | hi | lo] and weights per tap as [hi | lo | hi], so that ONE GEMM over 3*Cin
-// "channels" accumulates  a_hi*w_hi + a_hi*w_lo + a_lo*w_hi  in the fp32 TMEM accumulator (the dropped a_lo*w_lo term
+// "channels" accumulates  a_hi*w_hi + a_hi*w_lo + a_lo*w_hi  in the fp32 accumulator (the dropped a_lo*w_lo term
 // is 2^-22 relative); the epilogue adds an fp32 residual and writes fp32 and / or the split form for the next layer.
 #pragma once
-#include "sm100_prims.cuh"
+#include "wgmma.cuh"
 
 namespace ara {
 
@@ -44,7 +45,8 @@ struct ConvGemmArgs {
     int split_cs;             // channel pitch of one part (multiple of 64)
 };
 
-constexpr int kGemmThreads = 192;  // warp0: TMA producer, warp1: MMA issuer (+TMEM alloc), warps2-5: epilogue
+constexpr int kGemmConsumers = 2;                        // warpgroups, one board (64 rows) each
+constexpr int kGemmThreads = kGemmConsumers * 128 + 32;  // + warp 8: TMA producer
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 
@@ -57,11 +59,11 @@ struct ConvGemmCfg {
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-template <int BN, int FMT>
+template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                  const ConvGemmArgs args) {
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000)
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 900)
     using Cfg = ConvGemmCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     // 1 KB alignment by offset arithmetic on the shared array itself: a pointer -> integer -> pointer round trip would
@@ -69,8 +71,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + Cfg::kStages;
-    uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -80,28 +80,21 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     const int taps = args.ksize * args.ksize;
     const int num_kb = taps * args.c_chunks;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm_a);
         tma_prefetch_desc(&tm_b);
         for (int i = 0; i < Cfg::kStages; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
+            mbar_init(&empty_bar[i], kGemmConsumers * 4);  // lane 0 of every consumer warp
         }
-        mbar_init(tmem_full_bar, 1);
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc<BN>(tmem_slot);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // PDL: everything above overlapped the tail of the previous kernel; its outputs are only touched below
     pdl_wait();
     pdl_launch_dependents();
 
-    if (warp == 0) {
+    if (warp == kGemmConsumers * 4) {
         if (lane == 0) {
             const int half_k = args.ksize >> 1;
             for (int kb = 0; kb < num_kb; ++kb) {
@@ -119,131 +112,68 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
                 tma_load_2d(sb, &tm_b, &full_bar[s], tap * args.cw + cc * kBlockK, n_tile * BN);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = umma_idesc_f16(kBlockM, BN, FMT);
-        for (int kb = 0; kb < num_kb; ++kb) {
-            const int s = kb % Cfg::kStages;
-            const uint32_t ph = (kb / Cfg::kStages) & 1;
-            mbar_wait(&full_bar[s], ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes);
-                const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    const uint64_t da = umma_desc_k_sw128(sa + k * 32, 1024);
-                    const uint64_t db = umma_desc_k_sw128(sb + k * 32, 1024);
-                    umma_f16_ss(tmem_base, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[s]);  // frees the smem stage once these MMAs retire
-            }
-            __syncwarp();
-        }
-        if (lane == 0) umma_commit(tmem_full_bar);
-        __syncwarp();
-    } else {
-        // Epilogue: warp w may only touch TMEM lanes [32*(w%4), 32*(w%4)+32).
-        const int lane_grp = warp & 3;
-        const int row = lane_grp * 32 + lane;
-        const int m = m_tile * kBlockM + row;
-        const bool row_ok = m < args.M;
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            const int n0 = n_tile * BN + c0;
-            if (n0 >= args.ldo) break;  // warp-uniform
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(lane_grp * 32) << 16) + c0, v);
-            tmem_ld_wait();
-            float f[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-            if (args.bias != nullptr) {
-                const float4* bp = reinterpret_cast<const float4*>(args.bias + n0);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 b = __ldg(bp + j);
-                    f[4 * j + 0] += b.x;
-                    f[4 * j + 1] += b.y;
-                    f[4 * j + 2] += b.z;
-                    f[4 * j + 3] += b.w;
-                }
-            }
-            if (args.relu) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.0f);
-            }
-            if (row_ok) {
-                if (args.residual != nullptr) {
-                    const uint4* rp = reinterpret_cast<const uint4*>(args.residual + static_cast<size_t>(m) * args.ldr + n0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint4 r = __ldg(rp + j);
-                        const __half2* h = reinterpret_cast<const __half2*>(&r);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            const float2 x = __half22float2(h[q]);
-                            f[8 * j + 2 * q] += x.x;
-                            f[8 * j + 2 * q + 1] += x.y;
-                        }
-                    }
-                }
-                if (args.residual_f != nullptr) {
-                    const float4* rp = reinterpret_cast<const float4*>(args.residual_f + static_cast<size_t>(m) * args.ldr + n0);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 r = __ldg(rp + j);
-                        f[4 * j + 0] += r.x;
-                        f[4 * j + 1] += r.y;
-                        f[4 * j + 2] += r.z;
-                        f[4 * j + 3] += r.w;
-                    }
-                }
-                if (args.out_split != nullptr && n0 < args.split_cs) {
-                    __half* base = args.out_split + static_cast<size_t>(m) * (3 * args.split_cs) + n0;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        uint4 oh, ol;
-                        __half2* hh = reinterpret_cast<__half2*>(&oh);
-                        __half2* hl = reinterpret_cast<__half2*>(&ol);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            const float a = f[8 * j + 2 * q], b = f[8 * j + 2 * q + 1];
-                            const __half2 hi = __floats2half2_rn(a, b);
-                            const float2 hf = __half22float2(hi);
-                            hh[q] = hi;
-                            hl[q] = __floats2half2_rn(a - hf.x, b - hf.y);
-                        }
-                        reinterpret_cast<uint4*>(base)[j] = oh;
-                        reinterpret_cast<uint4*>(base + args.split_cs)[j] = oh;
-                        reinterpret_cast<uint4*>(base + 2 * args.split_cs)[j] = ol;
-                    }
-                }
-                if (args.out_h != nullptr) {
-                    uint4* op = reinterpret_cast<uint4*>(args.out_h + static_cast<size_t>(m) * args.ldo + n0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        uint4 o;
-                        __half2* h = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) h[q] = __floats2half2_rn(f[8 * j + 2 * q], f[8 * j + 2 * q + 1]);
-                        op[j] = o;
-                    }
-                }
-                if (args.out_f != nullptr) {
-                    float4* op = reinterpret_cast<float4*>(args.out_f + static_cast<size_t>(m) * args.ldo + n0);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) op[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<BN>(tmem_base);
+    // ---- consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of the tile (board 2 m_tile + wg)
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+    for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % Cfg::kStages;
+        mbar_wait(&full_bar[s], (kb / Cfg::kStages) & 1);
+        const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes) + Cfg::kABytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k)
+            wgmma_f16<BN>(acc, wgmma_desc_k_sw128(sa + k * 32, 1024), wgmma_desc_k_sw128(sb + k * 32, 1024),
+                          (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        // the stage before this one is free once its wgmma group has retired (one group stays in flight)
+        wgmma_wait<1>();
+        wgmma_fence_regs(acc);
+        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(kb - 1) % Cfg::kStages]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+
+    // ---- epilogue from the accumulator fragments: rows r0, r0 + 8; columns 8 j + 2 (lane % 4) (+ 1)
+    const int r0 = m_tile * kBlockM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int g0 = n_tile * BN + 8 * j;
+        if (g0 >= args.ldo) break;  // uniform
+        const int n = g0 + 2 * (lane & 3);
+        float2 b = make_float2(0.0f, 0.0f);
+        if (args.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(args.bias + n));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = r0 + 8 * h;
+            float f0 = acc[4 * j + 2 * h] + b.x, f1 = acc[4 * j + 2 * h + 1] + b.y;
+            if (args.relu) f0 = fmaxf(f0, 0.0f), f1 = fmaxf(f1, 0.0f);
+            if (m >= args.M) continue;
+            if (args.residual != nullptr) {
+                const float2 x = __half22float2(*reinterpret_cast<const __half2*>(args.residual + static_cast<size_t>(m) * args.ldr + n));
+                f0 += x.x, f1 += x.y;
+            }
+            if (args.residual_f != nullptr) {
+                const float2 x = __ldg(reinterpret_cast<const float2*>(args.residual_f + static_cast<size_t>(m) * args.ldr + n));
+                f0 += x.x, f1 += x.y;
+            }
+            if (args.out_split != nullptr && g0 < args.split_cs) {
+                __half* base = args.out_split + static_cast<size_t>(m) * (3 * args.split_cs) + n;
+                const __half2 hi = __floats2half2_rn(f0, f1);
+                const float2 hf = __half22float2(hi);
+                *reinterpret_cast<__half2*>(base) = hi;
+                *reinterpret_cast<__half2*>(base + args.split_cs) = hi;
+                *reinterpret_cast<__half2*>(base + 2 * args.split_cs) = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+            }
+            if (args.out_h != nullptr)
+                *reinterpret_cast<__half2*>(args.out_h + static_cast<size_t>(m) * args.ldo + n) = __floats2half2_rn(f0, f1);
+            if (args.out_f != nullptr)
+                *reinterpret_cast<float2*>(args.out_f + static_cast<size_t>(m) * args.ldo + n) = make_float2(f0, f1);
+        }
     }
 #endif
 }

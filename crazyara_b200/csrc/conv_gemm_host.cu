@@ -1,4 +1,4 @@
-// Host side of the tcgen05 convolution GEMM: TMA tensor-map construction and launch.
+// Host side of the wgmma convolution GEMM: TMA tensor-map construction and launch.
 #include "conv_gemm_host.h"
 
 #include <cstdlib>
@@ -134,11 +134,11 @@ static int launch_bn(const ConvLayer* L, const ConvGemmArgs& a, dim3 grid, cudaS
     using Cfg = ConvGemmCfg<BN>;
     static bool attr_done = false;
     if (!attr_done) {
-        ARA_CUDA_OK(cudaFuncSetAttribute(conv_gemm_kernel<BN, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        ARA_CUDA_OK(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes));
         attr_done = true;
     }
-    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN, 0>, grid, dim3(kGemmThreads), Cfg::kSmemBytes, stream, L->tm_a, L->tm_b, a));
+    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN>, grid, dim3(kGemmThreads), Cfg::kSmemBytes, stream, L->tm_a, L->tm_b, a));
     return 0;
 }
 

@@ -1,4 +1,4 @@
-// Host-side handle for one tcgen05 convolution layer (tensor maps + epilogue arguments).
+// Host-side handle for one wgmma convolution layer (tensor maps + epilogue arguments).
 #pragma once
 #include "abi_common.h"
 #include "conv_gemm.cuh"

@@ -1,4 +1,4 @@
-// RISE network: blob loader, weight re-layout for the tcgen05 GEMMs, forward launch sequence, C-ABI.
+// RISE network: blob loader, weight re-layout for the wgmma GEMMs, forward launch sequence, C-ABI.
 #include "net.h"
 
 #include <cstdio>
@@ -205,7 +205,7 @@ int Net::upload_value_head(const HostWeights& hw) {
     return 0;
 }
 
-// Precision float16: stem (tcgen05 implicit GEMM) -> persistent tower kernel -> heads
+// Precision float16: stem (wgmma implicit GEMM) -> persistent tower kernel -> heads
 int Net::build_half(const HostWeights& hw) {
     const int C = hdr.channels;
     const size_t rows = static_cast<size_t>(batch_cap) * 64;
@@ -256,7 +256,7 @@ int Net::build_half(const HostWeights& hw) {
     return 0;
 }
 
-// Precision float32: every layer a launch; GEMMs on tcgen05 with fp16 hi + lo operand splitting (3x the K extent),
+// Precision float32: every layer a launch; GEMMs on wgmma with fp16 hi + lo operand splitting (3x the K extent),
 // fp32 activations in HBM between the layers, CUDA-core stages in fp32
 int Net::build_precise(const HostWeights& hw) {
     const int C = hdr.channels;
@@ -337,8 +337,8 @@ int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
     {
         cudaDeviceProp prop;
         ARA_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-        if (prop.major < 10)
-            return set_error("ara_net_create: device %d is sm_%d%d; this library only runs on sm_100a (B200)", device,
+        if (prop.major != 9 || prop.minor != 0)
+            return set_error("ara_net_create: device %d is sm_%d%d; this library only runs on sm_90a (H100)", device,
                              prop.major, prop.minor);
     }
     ARA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));

@@ -1,4 +1,4 @@
-// CUDA-core kernels of the RISE forward pass that surround the tcgen05 GEMMs: layout conversion, value head, policy
+// CUDA-core kernels of the RISE forward pass that surround the wgmma GEMMs: layout conversion, value head, policy
 // softmax; for Precision float32 also depthwise convolution and squeeze-excitation (in Precision float16 those live
 // inside the persistent tower kernel, rise_trunk.cuh).  Activations are NHWC ([board*64+sq, C]).
 // Reference semantics: DeepCrazyhouse/src/domain/neural_net/architectures/pytorch/builder_util.py
@@ -10,7 +10,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "sm100_prims.cuh"
+#include "sm90_prims.cuh"
 
 namespace ara {
 
@@ -36,7 +36,7 @@ __global__ void nchw_f32_to_nhwc_f16_kernel(const float* __restrict__ in, __half
 
 // =============================================================================================
 // Precision float32 (the reference's `Precision float32`): fp32 activations between the layers; every tensor that feeds
-// a tcgen05 GEMM is ALSO stored split as fp16 [hi | hi | lo] with the channel pitch cs (conv_gemm.cuh).  The CUDA-core
+// a wgmma GEMM is ALSO stored split as fp16 [hi | hi | lo] with the channel pitch cs (conv_gemm.cuh).  The CUDA-core
 // stages below read / write fp32.
 __device__ __forceinline__ void store_split(__half* row3, int cs, int c, float v) {
     const __half hi = __float2half_rn(v);

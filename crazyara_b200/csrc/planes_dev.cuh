@@ -8,7 +8,7 @@
 // plane, so the encoder walks the layout once and hands each channel to a sink as (mask in OUTPUT coordinates, v):
 //   * NCHW fp32 sink (the reference's [C,8,8] float tensor, State::get_state_planes): lanes write 2 squares each,
 //     coalesced 256 B per plane;
-//   * NHWC fp16 sink (the tcgen05 stem convolution's A operand): lane l keeps the descriptors of channels l, l+32,
+//   * NHWC fp16 sink (the wgmma stem convolution's A operand): lane l keeps the descriptors of channels l, l+32,
 //     l+64 and then writes row after row, 64 contiguous bytes per warp store.
 // The reference fills plane after plane with a bit-serial loop (set_bits_from_bitmap :33-46).
 #pragma once

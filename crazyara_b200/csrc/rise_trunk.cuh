@@ -1,42 +1,31 @@
 // The whole RISE residual tower as ONE persistent kernel (builder_util.py:437-475 _BottlekneckResidualBlock, repeated
 // for every block of rise_mobile_v2 / v3; the squeeze-excitation of a block acts on its input, in place).
-//
-// One CTA owns two boards (128 rows) from the stem output to the tower output: nothing a board needs lives in another
-// CTA (1x1 convolutions are row-local, the depthwise convolution and the SE pooling are board-local), so the
-// 256-channel activation tile X never leaves the SM between blocks: it lives in TENSOR MEMORY (fp16, 128 columns),
-// where the tensor core reads it directly as the A operand and the compute warps read / rewrite it with
-// tcgen05.ld / tcgen05.st.  Only the weights stream through shared memory, as pre-tiled images (the host lays every
-// 64-channel chunk out exactly as its shared-memory bytes, rise_trunk_host.cu) so that a chunk is TWO 1-D bulk copies:
-// the per-SM copy engine handles one operation at a time with ~270 cycles of fixed cost (tools/micro/tma_bw.cu), so
-// few large operations are what reaches its ~30 B/clk.
-// Per block, the operating channels are processed in chunks of 64:
-//     MMA1  D1[128x64]  = X[128x256] . W1_chunk^T        tcgen05, A from TMEM, B from the W1 ring
-//     epi1  relu(D1 + b1) -> H1 (smem, fp16, channel-group major)          16 compute warps, tcgen05.ld
-//     dw    depthwise kxk, + bd, relu -> H2 (smem, 128B-swizzled K-major)  CUDA cores: two warps per 8-channel group
-//           (one per board), one lane per (row pair, column): 2 squares x 8 channels in registers, activations and
-//           weights stay packed fp16 and feed the mixed-precision FMA (FHFMA: fp16 x fp16 + fp32)
-//     MMA2  D2[128x256] += H2[128x64] . W2_chunk^T        tcgen05 N=256, accumulator stays in TMEM for the whole block
-// then   X <- D2 + b2 + X   (TMEM -> registers -> TMEM; also to global after the last block).
-// Warp roles: 0 = producer of the W1 ring (weights + per-chunk vectors), 1 = MMA issuer + TMEM owner, 2..17 = compute,
-// 18 = producer of the W2 ring.  TMEM columns: X 0..127, D1 128..255 (2 x 64), D2 256..511.
+// One consumer warpgroup owns one board (64 rows) from the stem output to the tower output; its activation tile X stays
+// in shared memory, 128B-swizzled K-major (wgmma's A operand).  Per 64-channel chunk of a block:
+//     MMA1  D1[64x64] = X . W1^T (wgmma m64n64) -> relu(D1 + b1) -> H1 -> depthwise kxk, + bd, relu -> H2
+//     MMA2  D2[64x256] += H2 . W2^T (wgmma m64n256, accumulator in registers for the whole block)
+// then X <- (D2 + b2) + X.  Pre-tiled weight images (rise_trunk_host.cu) stream through one bulk-copy ring per CTA.
+// Every board runs the same instructions whatever NB is: its outputs do not depend on the batch.
 #pragma once
 #include "rise_trunk_args.h"
-#include "sm100_prims.cuh"
+#include "wgmma.cuh"
 
 namespace ara {
 
-constexpr int kRtComputeWarps = 16;
-constexpr int kRtComputeThreads = kRtComputeWarps * 32;
-constexpr int kRtThreads = (kRtComputeWarps + 3) * 32;
-constexpr int kRtW1Ring = 2, kRtW2Ring = 3;
-constexpr int kRtOffW2 = kRtW1Ring * kTrunkW1Image;
-constexpr int kRtOffH2 = kRtOffW2 + kRtW2Ring * kTrunkW2Image;
-constexpr int kRtOffH1 = kRtOffH2 + 2 * 16384;
-constexpr int kRtOffB2 = kRtOffH1 + 16384;
-constexpr int kRtOffBar = kRtOffB2 + 2 * 1024;  // b2 is double-buffered by block parity
-constexpr int kRtSmemBytes = kRtOffBar + 512 + 1024;
-static_assert(kRtSmemBytes <= 232448, "trunk kernel shared memory exceeds the sm_100 limit");
-constexpr uint32_t kRtColX = 0, kRtColD1 = 128, kRtColD2 = 256;
+// ring of weight units: unit 2 c = W1 image of chunk c (tile + vectors), unit 2 c + 1 = its W2 image
+constexpr int kRtSlot = kTrunkW1Image;
+template <int NB>
+struct RtCfg {
+    static constexpr int kRing = NB == 1 ? 4 : 3;
+    // + the producer: a warp, or with two boards a warpgroup (setmaxnreg hands registers over per warpgroup)
+    static constexpr int kThreads = NB * 128 + (NB == 1 ? 32 : 128);
+    static constexpr int kOffBoard = kRing * kRtSlot;
+    // per board: X [4 K panels][64 rows][128 B] | H2 [64 rows][128 B] | H1 [8 groups][64 squares][16 B] | SE scratch
+    static constexpr int kBoardBytes = 32768 + 8192 + 8192 + 2048;
+    static constexpr int kOffBar = kOffBoard + NB * kBoardBytes;
+    static constexpr int kSmemBytes = kOffBar + 256 + 1024 /*align slack*/;
+    static_assert(kSmemBytes <= 232448, "trunk kernel shared memory exceeds the sm_90 limit of 227 KB per block");
+};
 
 // -DARA_TRUNK_PROF: per-role cycle counters of CTA 0 (args.prof[role * 16 + slot]); see tools/prof_trunk.py
 #if defined(ARA_TRUNK_PROF)
@@ -58,10 +47,6 @@ constexpr uint32_t kRtColX = 0, kRtColD1 = 128, kRtColD2 = 256;
 #define RT_PROF_FLUSH(role) do { } while (0)
 #endif
 
-__device__ __forceinline__ void rt_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void rt_bar_sync(int id) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(kRtComputeThreads) : "memory");
-}
 __device__ __forceinline__ float rt_hard_sigmoid(float x) { return fminf(fmaxf(x * (1.0f / 6.0f) + 0.5f, 0.0f), 1.0f); }
 __device__ __forceinline__ float2 rt_unpack(uint32_t v) { return __half22float2(*reinterpret_cast<const __half2*>(&v)); }
 __device__ __forceinline__ uint32_t rt_pack(float a, float b) {
@@ -69,57 +54,8 @@ __device__ __forceinline__ uint32_t rt_pack(float a, float b) {
     return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// depthwise k x k for 2 vertically adjacent squares (rows y0, y0+1, column x of board db) and the 8 channels of group g.
-// aux: b1[64] f32 | bd[64] f32 | wd[k*k][64] f16
-template <int K>
-__device__ __forceinline__ void rt_depthwise(const uint8_t* sH1, const uint8_t* aux, int g, int db, int y0, int x,
-                                             uint4 (&out)[2]) {
-    constexpr int R = K / 2, NR = 2 + 2 * R;
-    const float* bd = reinterpret_cast<const float*>(aux + 256) + g * 8;
-    const uint8_t* wd = aux + 512 + g * 16;
-    float acc[2][8];
-    {
-        const float4 b0 = *reinterpret_cast<const float4*>(bd), b1 = *reinterpret_cast<const float4*>(bd + 4);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            acc[j][0] = b0.x, acc[j][1] = b0.y, acc[j][2] = b0.z, acc[j][3] = b0.w;
-            acc[j][4] = b1.x, acc[j][5] = b1.y, acc[j][6] = b1.z, acc[j][7] = b1.w;
-        }
-    }
-    const uint8_t* base = sH1 + g * 2048 + db * 1024;
-#pragma unroll
-    for (int dxi = 0; dxi < K; ++dxi) {
-        const int xx = x + dxi - R;
-        if (xx < 0 || xx > 7) continue;
-        uint4 in[NR];
-#pragma unroll
-        for (int i = 0; i < NR; ++i) {
-            const int yy = y0 - R + i;
-            in[i] = make_uint4(0u, 0u, 0u, 0u);
-            if (yy >= 0 && yy <= 7) in[i] = *reinterpret_cast<const uint4*>(base + ((yy * 8 + xx) << 4));
-        }
-#pragma unroll
-        for (int dyi = 0; dyi < K; ++dyi) {
-            const uint4 w = *reinterpret_cast<const uint4*>(wd + (dyi * K + dxi) * 128);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                fhfma2(acc[j][0], acc[j][1], in[j + dyi].x, w.x);
-                fhfma2(acc[j][2], acc[j][3], in[j + dyi].y, w.y);
-                fhfma2(acc[j][4], acc[j][5], in[j + dyi].z, w.z);
-                fhfma2(acc[j][6], acc[j][7], in[j + dyi].w, w.w);
-            }
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        out[j].x = rt_pack(fmaxf(acc[j][0], 0.0f), fmaxf(acc[j][1], 0.0f));
-        out[j].y = rt_pack(fmaxf(acc[j][2], 0.0f), fmaxf(acc[j][3], 0.0f));
-        out[j].z = rt_pack(fmaxf(acc[j][4], 0.0f), fmaxf(acc[j][5], 0.0f));
-        out[j].w = rt_pack(fmaxf(acc[j][6], 0.0f), fmaxf(acc[j][7], 0.0f));
-    }
-}
-
-// the same for the 4 channels `sub` of group g (one-board variant: the work of a chunk is spread over all 16 warps)
+// depthwise k x k for 2 vertically adjacent squares (rows y0, y0+1, column x) and the 4 channels `sub` of the 8-channel
+// group g.  sH1: [8 groups][64 squares][8 channels] fp16; aux: b1[64] f32 | bd[64] f32 | wd[k*k][64] f16
 template <int K>
 __device__ __forceinline__ void rt_depthwise4(const uint8_t* sH1, const uint8_t* aux, int g, int sub, int y0, int x,
                                               uint2 (&out)[2]) {
@@ -158,548 +94,239 @@ __device__ __forceinline__ void rt_depthwise4(const uint8_t* sH1, const uint8_t*
     }
 }
 
-// kRows = 128: a CTA owns two boards (UMMA M = 128, all 128 TMEM lanes).  kRows = 64: one board per CTA (UMMA M = 64,
-// whose rows live in lanes 0..15 of each 32-lane quadrant: row r <-> lane 32 (r / 16) + r % 16), used while the batch
-// has fewer boards than the GPU has SMs -- twice as many SMs work on the same batch, each CTA's CUDA-core stages
-// handle half the rows.
-//
-// kSplit = 2 (one-board variant only, launched as clusters of two CTAs): the two CTAs of a cluster hold the same board
-// and take alternate chunks of every block, so that a batch of 64 boards occupies 128 SMs.  Each ends a block with a
-// partial accumulator; they exchange halves through distributed shared memory (the CTA that owns a column half adds
-// the partner's partial sums, finishes X for those columns and sends the fp16 result back), synchronised by
-// cluster-scope mbarriers.  The SE of a block is computed redundantly by both.
-template <int kRows, int kSplit = 1>
-__global__ void __launch_bounds__(kRtThreads, 1) rise_trunk_kernel(const __grid_constant__ TrunkArgs args) {
-    constexpr bool kHalf = kRows == 64;
-    static_assert(kSplit == 1 || (kSplit == 2 && kHalf), "the chunk split exists for the one-board variant only");
-    constexpr int kW2Ring = kSplit == 2 ? 2 : kRtW2Ring;  // the third W2 slot holds the exchange buffer when splitting
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000)
+
+__device__ __forceinline__ void rt_wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+// byte offset of the fp16 element (row, channel) in the swizzled X tile
+__device__ __forceinline__ uint32_t rt_x_off(int row, int ch) {
+    return static_cast<uint32_t>((ch >> 6) * 8192 + row * 128 + ((((ch & 63) >> 3) ^ (row & 7)) << 4) + (ch & 7) * 2);
+}
+
+template <int NB>
+// A consumer needs ~230 registers (accumulators: 160).  Two boards = 12 warps, 3 per 16 K-register SM sub-partition:
+// 168 each at launch, then the producer warpgroup drops to 40 and the consumers grow to 232 (2 x 232 + 40 = 504).
+__global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(const __grid_constant__ TrunkArgs args) {
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 900)
+    using Cfg = RtCfg<NB>;
+    constexpr int R = Cfg::kRing;
     extern __shared__ uint8_t smem_raw[];
     // 1 KB alignment by offset arithmetic on the shared array itself: a pointer -> integer -> pointer round trip would
     // make every access below a GENERIC load/store (LD.E / ST.E) instead of LDS / STS
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* sW1 = smem;
-    uint8_t* sW2 = smem + kRtOffW2;
-    uint8_t* sH2 = smem + kRtOffH2;
-    uint8_t* sH1 = smem + kRtOffH1;
-    float* sB2all = reinterpret_cast<float*>(smem + kRtOffB2);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kRtOffBar);
-    uint64_t* x_ready = bars + 0;
-    uint64_t* w1_full = bars + 1;    // [2]
-    uint64_t* w1_empty = bars + 3;   // [2]  tensor core done with the tile AND compute warps done with the vectors
-    uint64_t* w2_full = bars + 5;    // [3]
-    uint64_t* w2_empty = bars + 8;   // [3]
-    uint64_t* d1_full = bars + 11;   // [2]
-    uint64_t* d1_empty = bars + 13;  // [2]
-    uint64_t* h2_full = bars + 15;   // [2]
-    uint64_t* h2_empty = bars + 17;  // [2]
-    uint64_t* d2_full = bars + 19;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-    uint64_t* ex1_full = bars + 21;  // split: the partner's partial sums for my columns have arrived
-    uint64_t* ex2_full = bars + 22;  // split: the partner's finished X columns have arrived
-    float* sEx = reinterpret_cast<float*>(sW2 + 2 * kTrunkW2Image);  // split: [64 rows][128 cols] fp32 partials
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kOffBar);
+    uint64_t* empty = full + R;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int crank = kSplit == 2 ? static_cast<int>(blockIdx.x & 1) : 0;  // rank inside the CTA pair
-    const int m_tile = kSplit == 2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
     const int n_blocks = args.n_blocks;
-    // device-side batch size: a CTA (pair) whose boards hold no input leaves before it allocates anything
-    if (args.boards_dev != nullptr && m_tile * (kRows / 64) >= *args.boards_dev) return;
+    // device-side batch size: a CTA whose boards hold no input leaves before it touches anything
+    if (args.boards_dev != nullptr && static_cast<int>(blockIdx.x) * NB >= *args.boards_dev) return;
 
-    if (warp == 0 && lane == 0) {
-        mbar_init(x_ready, kRtComputeWarps);
-        for (int i = 0; i < kRtW1Ring; ++i) {
-            mbar_init(&w1_full[i], 1);
-            mbar_init(&w1_empty[i], 1 + kRtComputeWarps);
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < R; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], NB);  // one arrival per warpgroup
         }
-        for (int i = 0; i < kW2Ring; ++i) {
-            mbar_init(&w2_full[i], 1);
-            mbar_init(&w2_empty[i], 1);
-        }
-        mbar_init(ex1_full, kRtComputeWarps / 2);
-        mbar_init(ex2_full, kRtComputeWarps / 2);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&d1_full[i], 1);
-            mbar_init(&d1_empty[i], kRtComputeWarps);
-            mbar_init(&h2_full[i], kRtComputeWarps);
-            mbar_init(&h2_empty[i], 1);
-        }
-        mbar_init(d2_full, 1);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    if (kSplit == 2) cluster_sync_all();  // the partner's barriers exist before anything arrives on them
     pdl_wait();
     pdl_launch_dependents();
 
-    if (warp == 0) {
-        // ---------------------------------------------------------------- producer: W1 images (tile + chunk vectors)
-        if (lane == 0) {
-            uint32_t gc = 0;
-            for (int b = 0; b < n_blocks; ++b) {
-                const TrunkBlock& B = args.blk[b];
-                for (int j = crank; j < B.n_chunks; j += kSplit, ++gc) {
-                    const uint32_t s = gc % kRtW1Ring;
-                    mbar_wait_relaxed(&w1_empty[s], ((gc / kRtW1Ring) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&w1_full[s], kTrunkW1Image);
-                    bulk_load_1d(sW1 + s * kTrunkW1Image, args.w1_img + static_cast<size_t>(B.chunk0 + j) * kTrunkW1Image,
-                                 kTrunkW1Image, &w1_full[s]);
-                }
+    if (warp >= NB * 4) {
+        if (NB > 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        // ---------------------------------------------------------------- producer: the weight stream
+        if (warp == NB * 4 && lane == 0) {
+            const TrunkBlock& L = args.blk[n_blocks - 1];
+            const int n_units = 2 * (L.chunk0 + L.n_chunks);
+            for (int u = 0; u < n_units; ++u) {
+                const int s = u % R;
+                mbar_wait_relaxed(&empty[s], ((u / R) & 1) ^ 1);
+                const size_t c = static_cast<size_t>(u >> 1);
+                const uint32_t bytes = (u & 1) ? kTrunkW2Image : kTrunkW1Image;
+                const uint8_t* src = (u & 1) ? args.w2_img + c * kTrunkW2Image : args.w1_img + c * kTrunkW1Image;
+                mbar_arrive_expect_tx(&full[s], bytes);
+                bulk_load_1d(smem + s * kRtSlot, src, bytes, &full[s]);
             }
         }
-    } else if (warp == kRtComputeWarps + 2) {
-        // ---------------------------------------------------------------- producer: W2 images
-        if (lane == 0) {
-            uint32_t gc = 0;
-            for (int b = 0; b < n_blocks; ++b) {
-                const TrunkBlock& B = args.blk[b];
-                for (int j = crank; j < B.n_chunks; j += kSplit, ++gc) {
-                    const uint32_t s = gc % kW2Ring;
-                    mbar_wait_relaxed(&w2_empty[s], ((gc / kW2Ring) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&w2_full[s], kTrunkW2Image);
-                    bulk_load_1d(sW2 + s * kTrunkW2Image, args.w2_img + static_cast<size_t>(B.chunk0 + j) * kTrunkW2Image,
-                                 kTrunkW2Image, &w2_full[s]);
-                }
-            }
+        return;
+    }
+
+    // -------------------------------------------------------------------- consumer warpgroup wg: one board
+    if (NB > 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;
+    const int w = t >> 5;
+    const int board = static_cast<int>(blockIdx.x) * NB + wg;
+    const bool board_ok = board * 64 < args.M;
+    uint8_t* sX = smem + Cfg::kOffBoard + wg * Cfg::kBoardBytes;
+    uint8_t* sH2 = sX + 32768;
+    uint8_t* sH1 = sH2 + 8192;
+    float* sPool = reinterpret_cast<float*>(sH1 + 8192);  // [256]
+    float* sHid = sPool + 256;                             // [256]
+    const uint32_t aX = smem_u32(sX), aH2 = smem_u32(sH2);
+    // accumulator fragment of this thread: rows fr, fr + 8; columns 8 j + fc, 8 j + fc + 1
+    const int fr = w * 16 + (lane >> 2), fc = 2 * (lane & 3);
+    RT_PROF_DECL();
+
+    {   // stem output -> the X tile (16-byte pieces into the swizzled layout); rows of a board without input: zeros
+        const uint4* src = reinterpret_cast<const uint4*>(args.x_in + static_cast<size_t>(board) * 64 * 256);
+#pragma unroll 4
+        for (int i = 0; i < 16; ++i) {
+            const int p = t + i * 128, r = p >> 5, c16 = p & 31;
+            const uint4 v = board_ok ? __ldg(src + p) : make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(sX + (c16 >> 3) * 8192 + r * 128 + (((c16 & 7) ^ (r & 7)) << 4)) = v;
         }
-    } else if (warp == 1) {
-        // ---------------------------------------------------------------- MMA issuer
-        constexpr uint32_t idesc1 = umma_idesc_f16(kRows, 64, 0);
-        constexpr uint32_t idesc2 = umma_idesc_f16(kRows, 256, 0);
-        const uint32_t aW1 = smem_u32(sW1), aW2 = smem_u32(sW2), aH2 = smem_u32(sH2);
-        uint32_t gc = 0;
-        RT_PROF_DECL();
-        auto mma2 = [&](uint32_t g, bool first) {
-            const uint32_t s = g & 1, slot = g % kW2Ring;
-            RT_PROF(0);
-            mbar_wait(&h2_full[s], (g >> 1) & 1);
-            RT_PROF(1);  // wait for H2 (compute warps)
-            mbar_wait(&w2_full[slot], (g / kW2Ring) & 1);
-            RT_PROF(2);  // wait for W2 ring
-            tc_fence_after();
-            if (lane == 0) {
+        fence_proxy_async();
+        rt_wg_sync(wg);
+    }
+    RT_PROF(0);  // X load
+
+    float acc2[128];
+    int u = 0;  // position in the weight stream
+    for (int b = 0; b < n_blocks; ++b) {
+        const TrunkBlock& B = args.blk[b];
+        const int nch = B.n_chunks;
+        if (B.se_type != 0) {
+            // squeeze-excitation on the block input, in place: thread t owns channels 2t, 2t+1
+            float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll 8
+            for (int r = 0; r < 64; ++r) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(sX + rt_x_off(r, 2 * t)));
+                s0 += f.x, s1 += f.y;
+            }
+            sPool[2 * t] = s0 * (1.0f / 64.0f);
+            sPool[2 * t + 1] = s1 * (1.0f / 64.0f);
+            rt_wg_sync(wg);
+            float sc0, sc1;
+            if (B.se_type == 1) {  // fc1 256 -> 128 (relu), fc2 128 -> 256 (hard sigmoid)
+                float a = 0.0f;
+#pragma unroll 16
+                for (int k = 0; k < 256; ++k) a = fmaf(__half2float(B.se_w1t[k * 128 + t]), sPool[k], a);
+                sHid[t] = fmaxf(a, 0.0f);
+                rt_wg_sync(wg);
+                float a0 = 0.0f, a1 = 0.0f;
+                const __half2* w2 = reinterpret_cast<const __half2*>(B.se_w2t) + t;
+#pragma unroll 16
+                for (int j = 0; j < 128; ++j) {
+                    const float2 wf = __half22float2(__ldg(w2 + j * 128));
+                    a0 = fmaf(wf.x, sHid[j], a0);
+                    a1 = fmaf(wf.y, sHid[j], a1);
+                }
+                sc0 = rt_hard_sigmoid(a0), sc1 = rt_hard_sigmoid(a1);
+            } else {  // 256 -> 256 + bias (hard sigmoid)
+                float a0 = 0.0f, a1 = 0.0f;
+                const __half2* w1 = reinterpret_cast<const __half2*>(B.se_w1t) + t;
+#pragma unroll 16
+                for (int k = 0; k < 256; ++k) {
+                    const float2 wf = __half22float2(__ldg(w1 + k * 128));
+                    a0 = fmaf(wf.x, sPool[k], a0);
+                    a1 = fmaf(wf.y, sPool[k], a1);
+                }
+                sc0 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t) + a0), sc1 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t + 1) + a1);
+            }
+#pragma unroll 8
+            for (int r = 0; r < 64; ++r) {
+                __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, 2 * t));
+                const float2 f = __half22float2(*x);
+                *x = __floats2half2_rn(f.x * sc0, f.y * sc1);
+            }
+            fence_proxy_async();
+            rt_wg_sync(wg);
+        }
+        RT_PROF(1);  // squeeze-excitation
+
+        for (int j = 0; j < nch; ++j) {
+            // ---- MMA1: D1 = X . W1^T (4 K panels of 64)
+            const int s1 = u % R;
+            mbar_wait(&full[s1], (u / R) & 1);
+            RT_PROF(2);  // wait for the W1 image
+            const uint8_t* w1 = smem + s1 * kRtSlot;
+            const uint32_t aW1 = smem_u32(w1);
+            float acc1[32];
+            wgmma_fence();
+#pragma unroll
+            for (int p = 0; p < 4; ++p)
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    umma_f16_ss(tmem_base + kRtColD2, umma_desc_k_sw128(aH2 + s * 16384 + k * 32, 1024),
-                                umma_desc_k_sw128(aW2 + slot * kTrunkW2Image + k * 32, 1024), idesc2,
-                                (first && k == 0) ? 0u : 1u);
-                umma_commit(&w2_empty[slot]);
-                umma_commit(&h2_empty[s]);
+                    wgmma_f16<64>(acc1, wgmma_desc_k_sw128(aX + p * 8192 + k * 32, 1024),
+                                  wgmma_desc_k_sw128(aW1 + p * 8192 + k * 32, 1024), (p > 0 || k > 0) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc1);
+            RT_PROF(3);  // MMA1
+            // ---- epilogue 1: relu(D1 + b1) -> H1
+            const uint8_t* aux = w1 + kTrunkW1Tile;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                const float2 b1 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux) + 8 * jj + fc);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    *reinterpret_cast<__half2*>(sH1 + jj * 1024 + (fr + 8 * h) * 16 + fc * 2) =
+                        __floats2half2_rn(fmaxf(acc1[4 * jj + 2 * h] + b1.x, 0.0f), fmaxf(acc1[4 * jj + 2 * h + 1] + b1.y, 0.0f));
             }
-            __syncwarp();
-        };
-        for (int b = 0; b < n_blocks; ++b) {
-            const int nch = args.blk[b].n_chunks;
-            RT_PROF(0);
-            mbar_wait(x_ready, b & 1);
-            RT_PROF(3);  // wait for the X tile (block boundary)
-            int own = 0;  // index among this CTA's chunks of the block
-            for (int j = crank; j < nch; j += kSplit, ++gc, ++own) {
-                const uint32_t s = gc & 1, slot = gc % kRtW1Ring;
-                mbar_wait(&d1_empty[s], ((gc >> 1) & 1) ^ 1);
-                RT_PROF(4);  // wait for a free D1 buffer
-                mbar_wait(&w1_full[slot], (gc / kRtW1Ring) & 1);
-                RT_PROF(5);  // wait for W1 ring
-                tc_fence_after();
-                if (lane == 0) {
+            rt_wg_sync(wg);  // H1 complete (and MMA2 of the previous chunk, waited by every thread, is done with H2)
+            RT_PROF(4);  // epilogue 1
+            // ---- depthwise k x k -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout
 #pragma unroll
-                    for (int p = 0; p < 4; ++p)
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_f16_ts(tmem_base + kRtColD1 + s * 64, tmem_base + kRtColX + p * 32 + k * 8,
-                                        umma_desc_k_sw128(aW1 + slot * kTrunkW1Image + p * 8192 + k * 32, 1024), idesc1,
-                                        (p > 0 || k > 0) ? 1u : 0u);
-                    umma_commit(&w1_empty[slot]);
-                    umma_commit(&d1_full[s]);
-                }
-                __syncwarp();
-                if (own >= 1) mma2(gc - 1, own == 1);
-            }
-            mma2(gc - 1, own == 1);
-            if (lane == 0) umma_commit(d2_full);
-            __syncwarp();
-        }
-        RT_PROF(0);
-        RT_PROF_FLUSH(0);
-    } else {
-        // ---------------------------------------------------------------- compute warps
-        const int cw = warp - 2;        // 0..15
-        const int grp = warp & 3;       // TMEM lane group this warp may access
-        const int cq = cw >> 2;         // column quarter (64 channels) handled by this thread in the TMEM accesses
-        // row of the tile held by this thread's TMEM lane (one-board variant: only lanes 0..15 of a quadrant hold rows)
-        const bool valid = !kHalf || lane < 16;
-        const int r = kHalf ? grp * 16 + (lane & 15) : grp * 32 + lane;
-        const int tid = cw * 32 + lane; // 0..511
-        const uint32_t lane_addr = static_cast<uint32_t>(grp * 32) << 16;
-        const uint32_t x_addr = tmem_base + lane_addr + kRtColX + cq * 32;
-        // depthwise role: two warps per 8-channel group (one per board), lane = (row pair, column)
-        // (one-board variant: two warps per 8-channel group, 4 channels each)
-        const int dg = cw >> 1, db = cw & 1, dy0 = (lane >> 3) * 2, dx = lane & 7;
-        const int m = m_tile * kRows + r;
-        uint32_t gc = 0;
-        RT_PROF_DECL();
-        {   // stem output -> tensor memory (fp16 pairs are already in the packed order the tensor core expects)
-            uint32_t xv[32];
-            if (valid && m < args.M) {
-                const uint4* src = reinterpret_cast<const uint4*>(args.x_in + static_cast<size_t>(m) * 256 + cq * 64);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const uint4 t = __ldg(src + i);
-                    xv[i * 4 + 0] = t.x, xv[i * 4 + 1] = t.y, xv[i * 4 + 2] = t.z, xv[i * 4 + 3] = t.w;
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) xv[i] = 0u;
-            }
-            tmem_st_32x32b_x32(x_addr, xv);
-            tmem_st_wait();
-        }
-        RT_PROF(0);  // X load
-        for (int b = 0; b < n_blocks; ++b) {
-            const TrunkBlock& B = args.blk[b];
-            const int nch = B.n_chunks;
-            const bool last = b == n_blocks - 1;
-            float* sB2 = sB2all + (b & 1) * 256;  // read in this block's epilogue, behind the chunk loop's barriers
-            if (tid < 256) sB2[tid] = __ldg(B.b2 + tid);
-            if (B.se_type != 0) {
-                // squeeze-excitation on the block input, in place (arithmetic of se_kernel, net_kernels.cuh)
-                // Pooling order (identical in both kernel variants, so that a position's outputs do not depend on which
-                // one evaluates it): 16-row sums by a lane butterfly inside each half warp, then ((s0+s1)+(s2+s3)) over
-                // the four 16-row groups of a board.
-                float* sPoolPart = reinterpret_cast<float*>(sH1);  // [8 groups of 16 rows][256]; dead once sPool exists
-                float* sPart = sPoolPart;                           // partial sums: [4][2][128] or [2][2][256]
-                float* sPool = sPoolPart + 2048;                    // [2][256]
-                float* sHid = sPool + 512;                          // [2][128]
-                float* sScale = sHid + 256;                         // [2][256]
-                const int bb = tid >> 8, c = tid & 255;
-                uint32_t xv[32];
-                tmem_ld_32x32b_x32(x_addr, xv);
-                tmem_ld_wait();
-                rt_bar_sync(1);  // H1 (aliased by the scratch above) is no longer read by the previous block
-                {
-                    // tile rows of this half warp: two-board variant 32 grp + 16 (lane / 16) .., one-board 16 grp ..
-                    const int q16 = kHalf ? grp : 2 * grp + (lane >> 4);
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        float vals[32];
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            const float2 f = rt_unpack(xv[hh * 16 + i]);
-                            vals[2 * i] = valid ? f.x : 0.0f, vals[2 * i + 1] = valid ? f.y : 0.0f;
-                        }
-                        // butterfly over the 16 lanes of the half warp: the value count halves at every step, lane l
-                        // ends up with the sums of channels 2 (l % 16) and 2 (l % 16) + 1
-#pragma unroll
-                        for (int off = 8, n = 16; off >= 1; off >>= 1, n >>= 1) {
-                            const bool upper = (lane & off) != 0;
-#pragma unroll
-                            for (int i = 0; i < n; ++i) {
-                                const float send = upper ? vals[i] : vals[i + n];
-                                const float keep = upper ? vals[i + n] : vals[i];
-                                vals[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                            }
-                        }
-                        if (valid) {
-                            // channel bits 4..1 come from lane bits 3..0 (bit 3 decided first), bit 0 is the value index
-                            const int l = lane & 15;
-                            const int ch = ((l >> 3) & 1) * 16 + ((l >> 2) & 1) * 8 + ((l >> 1) & 1) * 4 + (l & 1) * 2;
-                            float* dst = sPoolPart + q16 * 256 + cq * 64 + hh * 32 + ch;
-                            dst[0] = vals[0];
-                            dst[1] = vals[1];
-                        }
-                    }
-                }
-                rt_bar_sync(2);
-                {
-                    const float* pp = sPoolPart + (kHalf ? 0 : bb * 1024) + c;
-                    const float sum = (pp[0] + pp[256]) + (pp[512] + pp[768]);
-                    const float pooled = (kHalf && bb) ? 0.0f : sum * (1.0f / 64.0f);  // one-board variant: board 1 is idle
-                    rt_bar_sync(1);  // sPart (the FC scratch) aliases sPoolPart
-                    sPool[bb * 256 + c] = pooled;
-                }
-                rt_bar_sync(1);
-                // every weight is loaded once (fp16) and used for both boards; K is split over the thread groups and
-                // the partial sums meet in shared memory
-                // (half2 loads: two adjacent outputs per thread, 128 contiguous bytes per warp request)
-                if (B.se_type == 1) {
-                    {   // fc1 (256 -> 128): 8 K-groups of 32 x 64 output pairs
-                        const int kg = tid >> 6, jp = tid & 63;
-                        const __half2* w = reinterpret_cast<const __half2*>(B.se_w1t + (kg * 32) * 128) + jp;
-                        const float* p0 = sPool + kg * 32;
-                        const float* p1 = sPool + 256 + kg * 32;
-                        float a0 = 0.0f, a1 = 0.0f, c0 = 0.0f, c1 = 0.0f;  // (output 2jp, 2jp+1) x (board 0, 1)
-#pragma unroll 32
-                        for (int k = 0; k < 32; ++k) {
-                            const float2 wf = __half22float2(__ldg(w + k * 64));
-                            a0 = fmaf(wf.x, p0[k], a0);
-                            a1 = fmaf(wf.x, p1[k], a1);
-                            c0 = fmaf(wf.y, p0[k], c0);
-                            c1 = fmaf(wf.y, p1[k], c1);
-                        }
-                        sPart[(kg * 2 + 0) * 128 + 2 * jp] = a0;
-                        sPart[(kg * 2 + 1) * 128 + 2 * jp] = a1;
-                        sPart[(kg * 2 + 0) * 128 + 2 * jp + 1] = c0;
-                        sPart[(kg * 2 + 1) * 128 + 2 * jp + 1] = c1;
-                    }
-                    rt_bar_sync(2);
-                    if (tid < 256) {
-                        const float* q = sPart + (tid >> 7) * 128 + (tid & 127);
-                        sHid[tid] = fmaxf(((q[0] + q[256]) + (q[512] + q[768])) + ((q[1024] + q[1280]) + (q[1536] + q[1792])), 0.0f);
-                    }
-                    rt_bar_sync(1);
-                    {   // fc2 (128 -> 256): 4 K-groups of 32 x 128 output pairs
-                        const int kg = tid >> 7, cp = tid & 127;
-                        const __half2* w = reinterpret_cast<const __half2*>(B.se_w2t + (kg * 32) * 256) + cp;
-                        const float* h0 = sHid + kg * 32;
-                        const float* h1 = sHid + 128 + kg * 32;
-                        float a0 = 0.0f, a1 = 0.0f, c0 = 0.0f, c1 = 0.0f;
-#pragma unroll 32
-                        for (int j = 0; j < 32; ++j) {
-                            const float2 wf = __half22float2(__ldg(w + j * 128));
-                            a0 = fmaf(wf.x, h0[j], a0);
-                            a1 = fmaf(wf.x, h1[j], a1);
-                            c0 = fmaf(wf.y, h0[j], c0);
-                            c1 = fmaf(wf.y, h1[j], c1);
-                        }
-                        sPart[(kg * 2 + 0) * 256 + 2 * cp] = a0;
-                        sPart[(kg * 2 + 1) * 256 + 2 * cp] = a1;
-                        sPart[(kg * 2 + 0) * 256 + 2 * cp + 1] = c0;
-                        sPart[(kg * 2 + 1) * 256 + 2 * cp + 1] = c1;
-                    }
-                    rt_bar_sync(2);
-                    {
-                        const float* q = sPart + bb * 256 + c;
-                        sScale[bb * 256 + c] = rt_hard_sigmoid((q[0] + q[512]) + (q[1024] + q[1536]));
-                    }
-                } else {
-                    {   // 256 -> 256: 4 K-groups of 64 x 128 output pairs
-                        const int kg = tid >> 7, cp = tid & 127;
-                        const __half2* w = reinterpret_cast<const __half2*>(B.se_w1t + (kg * 64) * 256) + cp;
-                        const float* p0 = sPool + kg * 64;
-                        const float* p1 = sPool + 256 + kg * 64;
-                        float a0 = 0.0f, a1 = 0.0f, c0 = 0.0f, c1 = 0.0f;
-#pragma unroll 32
-                        for (int k = 0; k < 64; ++k) {
-                            const float2 wf = __half22float2(__ldg(w + k * 128));
-                            a0 = fmaf(wf.x, p0[k], a0);
-                            a1 = fmaf(wf.x, p1[k], a1);
-                            c0 = fmaf(wf.y, p0[k], c0);
-                            c1 = fmaf(wf.y, p1[k], c1);
-                        }
-                        sPart[(kg * 2 + 0) * 256 + 2 * cp] = a0;
-                        sPart[(kg * 2 + 1) * 256 + 2 * cp] = a1;
-                        sPart[(kg * 2 + 0) * 256 + 2 * cp + 1] = c0;
-                        sPart[(kg * 2 + 1) * 256 + 2 * cp + 1] = c1;
-                    }
-                    rt_bar_sync(2);
-                    {
-                        const float* q = sPart + bb * 256 + c;
-                        sScale[bb * 256 + c] = rt_hard_sigmoid(__ldg(B.se_b + c) + ((q[0] + q[512]) + (q[1024] + q[1536])));
-                    }
-                }
-                rt_bar_sync(1);
-                {
-                    const float* sc = sScale + (kHalf ? 0 : (r >> 6) * 256) + cq * 64;
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const float2 f = rt_unpack(xv[i]);
-                        xv[i] = rt_pack(f.x * sc[2 * i], f.y * sc[2 * i + 1]);
-                    }
-                    tmem_st_32x32b_x32(x_addr, xv);
-                    tmem_st_wait();
-                }
-            }
-            // the tile (just loaded, rewritten by the previous epilogue, or rescaled above) becomes the A operand
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(x_ready);
-            RT_PROF(1);  // squeeze-excitation + hand-over of the tile
-
-            for (int j = crank; j < nch; j += kSplit, ++gc) {
-                const uint32_t s = gc & 1, slot = gc % kRtW1Ring;
-                // ---- epilogue 1: D1 -> relu(+b1) -> H1
-                mbar_wait(&d1_full[s], (gc >> 1) & 1);
-                RT_PROF(2);  // wait for D1 (tensor core); the W1 image (and its vectors) arrived before the MMA ran
-                tc_fence_after();
-                uint32_t v[16];
-                tmem_ld_32x32b_x16(tmem_base + lane_addr + kRtColD1 + s * 64 + cq * 16, v);
-                tmem_ld_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&d1_empty[s]);
-                RT_PROF(3);  // TMEM read-out
-                mbar_wait(&w1_full[slot], (gc / kRtW1Ring) & 1);  // already complete: makes the copied vectors visible here
-                const uint8_t* aux = sW1 + slot * kTrunkW1Image + kTrunkW1Tile;
-                rt_bar_sync(1);  // every thread is done reading the previous chunk's H1
-                RT_PROF(5);
-#pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const float* bp = reinterpret_cast<const float*>(aux) + cq * 16 + q * 8;
-                    const float4 ba = *reinterpret_cast<const float4*>(bp);
-                    const float4 bb = *reinterpret_cast<const float4*>(bp + 4);
-                    uint4 o;
-                    o.x = rt_pack(fmaxf(__uint_as_float(v[q * 8 + 0]) + ba.x, 0.0f), fmaxf(__uint_as_float(v[q * 8 + 1]) + ba.y, 0.0f));
-                    o.y = rt_pack(fmaxf(__uint_as_float(v[q * 8 + 2]) + ba.z, 0.0f), fmaxf(__uint_as_float(v[q * 8 + 3]) + ba.w, 0.0f));
-                    o.z = rt_pack(fmaxf(__uint_as_float(v[q * 8 + 4]) + bb.x, 0.0f), fmaxf(__uint_as_float(v[q * 8 + 5]) + bb.y, 0.0f));
-                    o.w = rt_pack(fmaxf(__uint_as_float(v[q * 8 + 6]) + bb.z, 0.0f), fmaxf(__uint_as_float(v[q * 8 + 7]) + bb.w, 0.0f));
-                    if (valid) *reinterpret_cast<uint4*>(sH1 + (cq * 2 + q) * (kRows * 16) + r * 16) = o;
-                }
-                RT_PROF(6);  // H1 write
-                rt_bar_sync(2);  // H1 complete
-                RT_PROF(7);
-                // ---- depthwise k x k
-                uint4 o2[2];
-                uint2 o2h[2];
-                if (kHalf) {
-                    if (B.ksize == 3)
-                        rt_depthwise4<3>(sH1, aux, dg, db, dy0, dx, o2h);
-                    else
-                        rt_depthwise4<5>(sH1, aux, dg, db, dy0, dx, o2h);
-                } else {
-                    if (B.ksize == 3)
-                        rt_depthwise<3>(sH1, aux, dg, db, dy0, dx, o2);
-                    else
-                        rt_depthwise<5>(sH1, aux, dg, db, dy0, dx, o2);
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&w1_empty[slot]);  // this warp is done with the chunk vectors
-                RT_PROF(8);  // depthwise
-                // ---- H2 (A operand of MMA2) in the 128B-swizzled K-major layout
-                mbar_wait(&h2_empty[s], ((gc >> 1) & 1) ^ 1);
-                RT_PROF(9);  // wait for a free H2 buffer
+            for (int i = 0; i < 4; ++i) {
+                const int item = t + i * 128;
+                const int g = item >> 6, sub = (item >> 5) & 1, y0 = ((item >> 3) & 3) * 2, x = item & 7;
+                uint2 o[2];
+                if (B.ksize == 3)
+                    rt_depthwise4<3>(sH1, aux, g, sub, y0, x, o);
+                else
+                    rt_depthwise4<5>(sH1, aux, g, sub, y0, x, o);
 #pragma unroll
                 for (int jj = 0; jj < 2; ++jj) {
-                    if (kHalf) {
-                        const int rr = (dy0 + jj) * 8 + dx;
-                        *reinterpret_cast<uint2*>(sH2 + s * 16384 + rr * 128 + ((dg ^ (rr & 7)) << 4) + db * 8) = o2h[jj];
-                    } else {
-                        const int rr = db * 64 + (dy0 + jj) * 8 + dx;
-                        *reinterpret_cast<uint4*>(sH2 + s * 16384 + rr * 128 + ((dg ^ (rr & 7)) << 4)) = o2[jj];
-                    }
-                }
-                rt_fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&h2_full[s]);
-                RT_PROF(10);  // H2 write
-            }
-            // ---- block epilogue: X <- D2 + b2 + X (tensor memory in place; also to global after the last block)
-            mbar_wait(d2_full, b & 1);
-            RT_PROF(11);  // wait for D2
-            tc_fence_after();
-            if (kSplit == 2) {
-                // This CTA's D2 holds the sum over ITS chunks only.  Column half `crank` is finished here: the partner
-                // sends its partial sums for those columns, this CTA adds them, applies bias + residual, keeps the new
-                // X columns and sends them back; for the other half the roles are swapped.
-                const bool mine = (cq >> 1) == crank;
-                const uint32_t partner = static_cast<uint32_t>(crank ^ 1);
-                uint32_t* sXh = reinterpret_cast<uint32_t*>(sH2 + (cq & 1) * 16384 + 8192);  // [64 rows][32] packed fp16 pairs
-                if (!mine) {
-                    const uint32_t rex = cluster_map(sEx + r * 128 + (cq & 1) * 64, partner);
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) {
-                        uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + lane_addr + kRtColD2 + cq * 64 + cc * 32, v);
-                        tmem_ld_wait();
-                        if (valid) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i)
-                                st_cluster_v4(rex + (cc * 32 + i * 4) * 4, v[i * 4], v[i * 4 + 1], v[i * 4 + 2], v[i * 4 + 3]);
-                        }
-                    }
-                    asm volatile("fence.acq_rel.cluster;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(cluster_map(ex1_full, partner));
-                    if (!last) {  // the finished X columns come back from the partner
-                        mbar_wait_cluster(ex2_full, b & 1);
-                        uint32_t xv[32];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const uint4 t = *reinterpret_cast<const uint4*>(sXh + r * 32 + i * 4);
-                            xv[i * 4] = t.x, xv[i * 4 + 1] = t.y, xv[i * 4 + 2] = t.z, xv[i * 4 + 3] = t.w;
-                        }
-                        tmem_st_32x32b_x32(x_addr, xv);
-                        tmem_st_wait();
-                    }
-                } else {
-                    mbar_wait_cluster(ex1_full, b & 1);
-                    uint32_t xv[32];
-                    tmem_ld_32x32b_x32(x_addr, xv);
-#pragma unroll
-                    for (int cc = 0; cc < 2; ++cc) {
-                        uint32_t v[32];
-                        tmem_ld_32x32b_x32(tmem_base + lane_addr + kRtColD2 + cq * 64 + cc * 32, v);
-                        tmem_ld_wait();
-                        const float* b2p = sB2 + cq * 64 + cc * 32;
-                        const float* pp = sEx + r * 128 + (cq & 1) * 64 + cc * 32;
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            const float2 xr = rt_unpack(xv[cc * 16 + i]);
-                            const float2 pr = valid ? *reinterpret_cast<const float2*>(pp + 2 * i) : make_float2(0.0f, 0.0f);
-                            // chunk order of the unsplit kernel is even, odd, even, ...: rank 0's partial first
-                            const float s0 = crank == 0 ? __uint_as_float(v[2 * i]) + pr.x : pr.x + __uint_as_float(v[2 * i]);
-                            const float s1 = crank == 0 ? __uint_as_float(v[2 * i + 1]) + pr.y : pr.y + __uint_as_float(v[2 * i + 1]);
-                            xv[cc * 16 + i] = rt_pack(s0 + b2p[2 * i] + xr.x, s1 + b2p[2 * i + 1] + xr.y);
-                        }
-                    }
-                    if (!last) {
-                        tmem_st_32x32b_x32(x_addr, xv);
-                        if (valid) {
-                            const uint32_t rxh = cluster_map(sXh + r * 32, partner);
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) st_cluster_v4(rxh + i * 16, xv[i * 4], xv[i * 4 + 1], xv[i * 4 + 2], xv[i * 4 + 3]);
-                        }
-                        tmem_st_wait();
-                        asm volatile("fence.acq_rel.cluster;" ::: "memory");
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(cluster_map(ex2_full, partner));
-                    } else if (valid && m < args.M) {
-                        uint4* dst = reinterpret_cast<uint4*>(args.out + static_cast<size_t>(m) * 256 + cq * 64);
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) dst[i] = make_uint4(xv[i * 4], xv[i * 4 + 1], xv[i * 4 + 2], xv[i * 4 + 3]);
-                    }
-                }
-            } else {
-                uint32_t xv[32];
-                tmem_ld_32x32b_x32(x_addr, xv);
-#pragma unroll
-                for (int cc = 0; cc < 2; ++cc) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tmem_base + lane_addr + kRtColD2 + cq * 64 + cc * 32, v);
-                    tmem_ld_wait();
-                    const float* b2p = sB2 + cq * 64 + cc * 32;
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const float2 xr = rt_unpack(xv[cc * 16 + i]);
-                        xv[cc * 16 + i] = rt_pack(__uint_as_float(v[2 * i]) + b2p[2 * i] + xr.x,
-                                                  __uint_as_float(v[2 * i + 1]) + b2p[2 * i + 1] + xr.y);
-                    }
-                }
-                if (!last) {
-                    tmem_st_32x32b_x32(x_addr, xv);
-                    tmem_st_wait();
-                } else if (valid && m < args.M) {
-                    uint4* dst = reinterpret_cast<uint4*>(args.out + static_cast<size_t>(m) * 256 + cq * 64);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) dst[i] = make_uint4(xv[i * 4], xv[i * 4 + 1], xv[i * 4 + 2], xv[i * 4 + 3]);
+                    const int rr = (y0 + jj) * 8 + x;
+                    *reinterpret_cast<uint2*>(sH2 + rr * 128 + ((g ^ (rr & 7)) << 4) + sub * 8) = o[jj];
                 }
             }
-            tc_fence_before();
-            RT_PROF(12);  // block epilogue
+            fence_proxy_async();
+            rt_wg_sync(wg);
+            if (t == 0) mbar_arrive(&empty[s1]);  // the W1 image (tile and vectors) is no longer read
+            ++u;
+            RT_PROF(5);  // depthwise
+            // ---- MMA2: D2 += H2 . W2^T
+            const int s2 = u % R;
+            mbar_wait(&full[s2], (u / R) & 1);
+            RT_PROF(6);  // wait for the W2 image
+            const uint32_t aW2 = smem_u32(smem + s2 * kRtSlot);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_f16<256>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
+                               (j > 0 || k > 0) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc2);
+            if (t == 0) mbar_arrive(&empty[s2]);
+            ++u;
+            RT_PROF(7);  // MMA2
         }
-        if (warp == 2) RT_PROF_FLUSH(1);
+        // ---- block epilogue: X <- (D2 + b2) + X (the last block: to global memory)
+        const bool last = b == n_blocks - 1;
+#pragma unroll
+        for (int jj = 0; jj < 32; ++jj) {
+            const int c = 8 * jj + fc;
+            const float2 b2 = __ldg(reinterpret_cast<const float2*>(B.b2 + c));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = fr + 8 * h;
+                __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, c));
+                const float2 xr = __half22float2(*x);
+                const __half2 y = __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
+                if (!last)
+                    *x = y;
+                else if (board_ok)
+                    *reinterpret_cast<__half2*>(args.out + (static_cast<size_t>(board) * 64 + r) * 256 + c) = y;
+            }
+        }
+        fence_proxy_async();
+        rt_wg_sync(wg);
+        RT_PROF(8);  // block epilogue
     }
-    tc_fence_before();
-    __syncthreads();
-    if (kSplit == 2) cluster_sync_all();  // no CTA leaves while its partner may still write into its shared memory
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
-    }
+    if (t == 0 && wg == 0) RT_PROF_FLUSH(1);
 #endif
 }
 

@@ -15,25 +15,8 @@ constexpr int kTrunkAuxBytes = 3712;   // 64 f32 + 64 f32 + 25 * 64 f16
 constexpr int kTrunkW1Image = 36864;   // tile + aux, padded to 1 KB
 constexpr int kTrunkW2Image = 32768;
 
-// rise_trunk_t.cuh (one board per CTA, channels in M) streams the same weights as PAIRS of chunks, four 32 KB units per
-// pair: W1 rows (the pair's 128 operating channels) x K panels {0,1} | {2,3}, then W2 output-channel halves {0..127} |
-// {128..255} x the pair's 128 K.  Every unit is two 128-row K-major panels of 16 KB.  Per pair also a vector record:
-//   b1[128] f32 | bd[128] f32 | wd[k*k][128] f16
-// The fp16 squeeze-excitation matrices of a block travel in the same stream, as four units ahead of the block's pairs
-// (ca_se: [256][128] then [128][256]; eca_se: [256][256]), so that no load competes with the copy engine for the SM's port.
-constexpr int kTrunkTUnit = 32768;
-constexpr int kTrunkTAux = 7680;  // 512 + 512 + 25 * 256, padded to 256 B
-constexpr int kTrunkTLag = 2;     // MMA2 of a pair is issued this many pairs behind its MMA1 (the stream follows that order)
-#if !defined(ARA_TRUNK_CLAG)
-#define ARA_TRUNK_CLAG 3
-#endif
-constexpr int kTrunkCLag = ARA_TRUNK_CLAG;  // the same for rise_trunk_c.cuh (an H2 buffer crosses the cluster first)
-
 struct TrunkBlock {
     int n_chunks;     // ceil(Cop / 64)
-    int pair0;        // index of the block's first chunk pair (rise_trunk_t.cuh)
-    int se_seq0;      // rise_trunk_t.cuh: position in the unit stream of the block's four squeeze-excitation units
-    int se_seq0c[2];  // rise_trunk_c.cuh: the same in the stream of cluster rank 0 / 1
     int ksize;        // depthwise kernel: 3 or 5
     int se_type;      // 0 none, 1 ca_se, 2 eca_se (applied to the block input, in place)
     int chunk0;       // index of the block's first chunk in the image arrays
@@ -51,12 +34,6 @@ struct TrunkArgs {
     const __half* x_in;     // [M, 256] stem output
     __half* out;            // [M, 256]
     const int* boards_dev;     // device-side count of the boards in use (or nullptr): CTAs beyond it leave at once
-    const uint8_t* t_img;      // rise_trunk_t.cuh: [pairs][4][kTrunkTUnit]
-    const uint8_t* t_aux;      // [pairs][kTrunkTAux]
-    const int* t_seq;          // unit index (into t_img) of every unit of the stream, in consumption order
-    int t_units;
-    const int* c_seq[2];       // rise_trunk_c.cuh: the unit streams of cluster rank 0 / 1 (half the weights each)
-    int c_units[2];
     unsigned long long* prof;  // profiling builds (-DARA_TRUNK_PROF): [2][16] cycle counters of CTA 0, else unused
     TrunkBlock blk[kTrunkMaxBlocks];
 };

@@ -4,15 +4,13 @@
 #include <cstring>
 
 #include "rise_trunk.cuh"
-#include "rise_trunk_t.cuh"
-#include "rise_trunk_c.cuh"
 
 namespace ara {
 
 namespace {
 
 // byte offset of element (row, k) inside a K-major tile with 128-byte rows and the 128B swizzle (16-byte chunks XORed
-// with the row index modulo 8): the layout TMA's SWIZZLE_128B produces and the UMMA shared-memory descriptor reads
+// with the row index modulo 8): the layout TMA's SWIZZLE_128B produces and the wgmma shared-memory descriptor reads
 inline size_t sw128_offset(int row, int k) { return static_cast<size_t>(row) * 128 + ((((k >> 3) ^ (row & 7)) << 4)) + (k & 7) * 2; }
 
 }  // namespace
@@ -87,108 +85,11 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
     ARA_CUDA_OK(cudaMemcpy(T->d_w2, w2.data(), w2.size(), cudaMemcpyHostToDevice));
     T->args.w1_img = static_cast<const uint8_t*>(T->d_w1);
     T->args.w2_img = static_cast<const uint8_t*>(T->d_w2);
-    // the same weights for rise_trunk_t.cuh: chunk PAIRS (channels in M), four 32 KB units per pair, and the unit order
-    // of the stream (MMA2 of a pair follows kTrunkTLag pairs behind its MMA1; mirrored by the kernel's MMA issuer)
-    {
-        int pairs = 0;
-        for (int i = 0; i < nb; ++i) {
-            T->args.blk[i].pair0 = pairs;
-            pairs += (T->args.blk[i].n_chunks + 1) / 2;
-        }
-        int n_se = 0;
-        for (int i = 0; i < nb; ++i) n_se += blocks[i].se_type != 0 ? 1 : 0;
-        std::vector<uint8_t> img(static_cast<size_t>(pairs + n_se) * 4 * kTrunkTUnit, 0);
-        int se_idx = 0;
-        std::vector<uint8_t> aux(static_cast<size_t>(pairs) * kTrunkTAux, 0);
-        std::vector<int> seq;
-        std::vector<int> cseq[2];  // rise_trunk_c.cuh: rank r streams W1 of its own pairs and its half of every W2
-        for (int i = 0; i < nb; ++i) {
-            const TrunkBlockHost& h = blocks[i];
-            const TrunkBlock& B = T->args.blk[i];
-            const int kk = h.ksize * h.ksize, P = (B.n_chunks + 1) / 2;
-            for (int p = 0; p < P; ++p) {
-                uint8_t* unit = img.data() + static_cast<size_t>(B.pair0 + p) * 4 * kTrunkTUnit;
-                uint8_t* ax = aux.data() + static_cast<size_t>(B.pair0 + p) * kTrunkTAux;
-                float* ax_b1 = reinterpret_cast<float*>(ax);
-                float* ax_bd = reinterpret_cast<float*>(ax + 512);
-                __half* ax_wd = reinterpret_cast<__half*>(ax + 1024);
-                for (int r = 0; r < 128; ++r) {
-                    const int c = p * 128 + r;  // operating channel
-                    if (c >= h.c_op) break;
-                    // W1: row = operating channel of the pair, K = the 256 trunk channels in 4 panels (2 per unit)
-                    for (int k = 0; k < 256; ++k)
-                        *reinterpret_cast<__half*>(unit + (k >> 7) * kTrunkTUnit + ((k >> 6) & 1) * 16384 + sw128_offset(r, k & 63)) =
-                            __float2half_rn(h.w1[static_cast<size_t>(c) * 256 + k]);
-                    // W2: row = trunk channel (two halves of 128 = two units), K = the pair's operating channels in 2 panels
-                    for (int n = 0; n < 256; ++n)
-                        *reinterpret_cast<__half*>(unit + (2 + (n >> 7)) * kTrunkTUnit + (r >> 6) * 16384 + sw128_offset(n & 127, r & 63)) =
-                            __float2half_rn(h.w2[static_cast<size_t>(n) * h.c_op + c]);
-                    ax_b1[r] = h.b1[c];
-                    ax_bd[r] = h.bd[c];
-                    for (int q = 0; q < kk; ++q) ax_wd[q * 128 + r] = __float2half_rn(h.wd[static_cast<size_t>(c) * kk + q]);
-                }
-            }
-            if (h.se_type != 0) {  // the block's squeeze-excitation matrices (fp16, as the kernel's FC loops index them): 128 KB
-                const size_t n1 = h.se_type == 1 ? 256 * 128 : 256 * 256, n2 = h.se_type == 1 ? 128 * 256 : 0;
-                std::vector<float> f(n1 + n2);
-                ARA_CUDA_OK(cudaMemcpy(f.data(), h.se_w1t, n1 * 4, cudaMemcpyDeviceToHost));
-                if (n2) ARA_CUDA_OK(cudaMemcpy(f.data() + n1, h.se_w2t, n2 * 4, cudaMemcpyDeviceToHost));
-                __half* dst = reinterpret_cast<__half*>(img.data() + static_cast<size_t>(pairs + se_idx) * 4 * kTrunkTUnit);
-                for (size_t k = 0; k < n1 + n2; ++k) dst[k] = __float2half_rn(f[k]);
-                T->args.blk[i].se_seq0 = static_cast<int>(seq.size());
-                for (int u = 0; u < 4; ++u) seq.push_back((pairs + se_idx) * 4 + u);
-                for (int r = 0; r < 2; ++r) {
-                    T->args.blk[i].se_seq0c[r] = static_cast<int>(cseq[r].size());
-                    for (int u = 0; u < 4; ++u) cseq[r].push_back((pairs + se_idx) * 4 + u);
-                }
-                ++se_idx;
-            }
-            auto w2_units = [&](int p) {
-                seq.push_back((B.pair0 + p) * 4 + 2);
-                seq.push_back((B.pair0 + p) * 4 + 3);
-            };
-            for (int p = 0; p < P; ++p) {
-                seq.push_back((B.pair0 + p) * 4 + 0);
-                seq.push_back((B.pair0 + p) * 4 + 1);
-                if (p >= kTrunkTLag) w2_units(p - kTrunkTLag);
-            }
-            for (int p = P > kTrunkTLag ? P - kTrunkTLag : 0; p < P; ++p) w2_units(p);
-            for (int r = 0; r < 2; ++r) {
-                for (int p = 0; p < P; ++p) {
-                    if (((B.pair0 + p) & 1) == r) {
-                        cseq[r].push_back((B.pair0 + p) * 4 + 0);
-                        cseq[r].push_back((B.pair0 + p) * 4 + 1);
-                    }
-                    if (p >= kTrunkCLag) cseq[r].push_back((B.pair0 + p - kTrunkCLag) * 4 + 2 + r);
-                }
-                for (int p = P > kTrunkCLag ? P - kTrunkCLag : 0; p < P; ++p) cseq[r].push_back((B.pair0 + p) * 4 + 2 + r);
-            }
-        }
-        ARA_CUDA_OK(cudaMalloc(&T->d_timg, img.size()));
-        ARA_CUDA_OK(cudaMalloc(&T->d_taux, aux.size()));
-        ARA_CUDA_OK(cudaMalloc(&T->d_tseq, seq.size() * sizeof(int)));
-        ARA_CUDA_OK(cudaMemcpy(T->d_timg, img.data(), img.size(), cudaMemcpyHostToDevice));
-        ARA_CUDA_OK(cudaMemcpy(T->d_taux, aux.data(), aux.size(), cudaMemcpyHostToDevice));
-        ARA_CUDA_OK(cudaMemcpy(T->d_tseq, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice));
-        T->args.t_img = static_cast<const uint8_t*>(T->d_timg);
-        T->args.t_aux = static_cast<const uint8_t*>(T->d_taux);
-        T->args.t_seq = static_cast<const int*>(T->d_tseq);
-        T->args.t_units = static_cast<int>(seq.size());
-        ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_t_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRttSmemBytes));
-        ARA_CUDA_OK(cudaMalloc(&T->d_cseq, (cseq[0].size() + cseq[1].size()) * sizeof(int)));
-        ARA_CUDA_OK(cudaMemcpy(T->d_cseq, cseq[0].data(), cseq[0].size() * sizeof(int), cudaMemcpyHostToDevice));
-        ARA_CUDA_OK(cudaMemcpy(static_cast<int*>(T->d_cseq) + cseq[0].size(), cseq[1].data(), cseq[1].size() * sizeof(int), cudaMemcpyHostToDevice));
-        T->args.c_seq[0] = static_cast<const int*>(T->d_cseq);
-        T->args.c_seq[1] = static_cast<const int*>(T->d_cseq) + cseq[0].size();
-        T->args.c_units[0] = static_cast<int>(cseq[0].size());
-        T->args.c_units[1] = static_cast<int>(cseq[1].size());
-        ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRtcSmemBytes));
-    }
     ARA_CUDA_OK(cudaMalloc(&T->d_prof, 32 * sizeof(unsigned long long)));
     ARA_CUDA_OK(cudaMemset(T->d_prof, 0, 32 * sizeof(unsigned long long)));
     T->args.prof = static_cast<unsigned long long*>(T->d_prof);
-    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRtSmemBytes));
-    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRtSmemBytes));
+    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<1>::kSmemBytes));
+    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<2>::kSmemBytes));
     {
         int dev = 0;
         cudaDeviceProp prop;
@@ -204,38 +105,13 @@ int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const
     if (x_in != nullptr) a.x_in = x_in;
     a.M = boards * 64;
     a.boards_dev = boards_dev;
-    // one board per CTA while that still fits the GPU in one wave (twice the SMs on a small batch), else two
+    // one board per CTA while that fits one wave, else two sharing a weight stream (ARA_TRUNK_ROWS=64 / 128 forces)
     const char* force = getenv("ARA_TRUNK_ROWS");
     const bool one_board = force ? atoi(force) == 64 : boards <= T->sm_count;
-    // small batches: channels in the tensor core's M dimension (rise_trunk_t.cuh; ARA_TRUNK_T=0: the M = 64 variant of
-    // rise_trunk.cuh instead -- same bits, slower)
-    const char* et = getenv("ARA_TRUNK_T");
-    const bool transposed = et == nullptr || atoi(et) != 0;
-    // ... on CTA pairs while two CTAs per board still fit one wave (rise_trunk_c.cuh; ARA_TRUNK_PAIR=0: one CTA per board)
-    const char* ep = getenv("ARA_TRUNK_PAIR");
-    const bool paired = ep == nullptr || atoi(ep) != 0;
-    if (one_board && transposed && paired && 2 * boards <= T->sm_count) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(2 * boards);
-        cfg.blockDim = dim3(kRtcThreads);
-        cfg.dynamicSmemBytes = kRtcSmemBytes;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = pdl_enabled() ? 2 : 1;
-        ARA_CUDA_OK(cudaLaunchKernelEx(&cfg, rise_trunk_c_kernel, a));
-    } else if (one_board && transposed)
-        ARA_CUDA_OK(launch_pdl(rise_trunk_t_kernel, dim3(boards), dim3(kRttThreads), kRttSmemBytes, stream, a));
-    else if (one_board)
-        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<64>, dim3(boards), dim3(kRtThreads), kRtSmemBytes, stream, a));
+    if (one_board)
+        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<1>, dim3(boards), dim3(RtCfg<1>::kThreads), RtCfg<1>::kSmemBytes, stream, a));
     else
-        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<128>, dim3((boards + 1) / 2), dim3(kRtThreads), kRtSmemBytes, stream, a));
+        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<2>, dim3((boards + 1) / 2), dim3(RtCfg<2>::kThreads), RtCfg<2>::kSmemBytes, stream, a));
     return 0;
 }
 
@@ -243,12 +119,6 @@ void rise_trunk_destroy(RiseTrunk* T) {
     if (T->d_w1) cudaFree(T->d_w1);
     if (T->d_w2) cudaFree(T->d_w2);
     if (T->d_prof) cudaFree(T->d_prof);
-    if (T->d_timg) cudaFree(T->d_timg);
-    if (T->d_taux) cudaFree(T->d_taux);
-    if (T->d_tseq) cudaFree(T->d_tseq);
-    if (T->d_cseq) cudaFree(T->d_cseq);
-    T->d_cseq = nullptr;
-    T->d_timg = T->d_taux = T->d_tseq = nullptr;
     for (void* p : T->d_se) cudaFree(p);
     T->d_se.clear();
     T->d_w1 = T->d_w2 = T->d_prof = nullptr;

@@ -1,5 +1,5 @@
 // Host handle of the persistent trunk kernel (rise_trunk.cuh): stacks the weights of every bottleneck block into the
-// two matrices the kernel streams through its TMA rings and builds the per-chunk vector records.
+// two matrices the kernel streams through its weight ring and builds the per-chunk vector records.
 #pragma once
 #include <cuda.h>
 
@@ -27,11 +27,7 @@ struct RiseTrunk {
     TrunkArgs args;
     void* d_w1 = nullptr;
     void* d_w2 = nullptr;
-    void* d_timg = nullptr;  // rise_trunk_t.cuh: pair images, vector records, unit order
-    void* d_taux = nullptr;
-    void* d_tseq = nullptr;
-    void* d_cseq = nullptr;  // rise_trunk_c.cuh: unit order of the two cluster ranks
-    int sm_count = 148;
+    int sm_count = 0;
     void* d_prof = nullptr;  // [2][16] cycle counters, written only by -DARA_TRUNK_PROF builds
     std::vector<void*> d_se;  // fp16 copies of the squeeze-excitation matrices
 };

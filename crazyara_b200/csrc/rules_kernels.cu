@@ -63,7 +63,7 @@ static int check_device() {
     ARA_CUDA_OK(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     ARA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) return set_error("this library only runs on sm_100 (B200); device %d is sm_%d%d", dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return set_error("this library only runs on sm_90a (H100); device %d is sm_%d%d", dev, prop.major, prop.minor);
     return 0;
 }
 

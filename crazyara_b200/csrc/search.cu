@@ -6,7 +6,7 @@
 //            trees (select_wave_kernel, search_wave.cuh) -- sequential semantics either way
 //   (pack)   many trees: the new leaves' rows of the network batch; expand: move lists, edges, planes written straight into
 //            the network's NHWC input, one warp per new leaf
-//   network  tcgen05 conv stack (CUDA graph), or the hash-derived fake backend for search-parity tests
+//   network  wgmma conv stack (CUDA graph), or the hash-derived fake backend for search-parity tests
 //   update   scatter priors / values into the new nodes, prepare their next children, backups, collision reverts
 // Threads = 1: all on one stream.  Threads = 2: the two logical threads' tree kernels on one stream in the fixed schedule
 // of oracle/mcts.h, their forwards on a second stream (enqueue_slot).  The host only looks at the per-tree `done` flag
@@ -547,12 +547,9 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     {
         cudaDeviceProp prop;
         ARA_CUDA_OK(cudaGetDeviceProperties(&prop, device_));
-        if (prop.major < 10) return set_error("ara_search_create: device %d is not sm_100 (B200)", device_);
+        if (prop.major != 9 || prop.minor != 0) return set_error("ara_search_create: device %d is not sm_90a (H100)", device_);
     }
-    // few trees cannot fill 148 SMs with one warp each: their playouts overlap inside a CTA instead (search_wave.cuh)
-    // (measured: up to 16 trees it pays from Batch_Size 8 on -- self-play with 8 / 16 games per GPU: +14 % / +8 % games per
-    // hour; with 32 trees of narrow mini-batches the one-warp kernel is faster, a playout may only start while the batch
-    // cannot end before its turn)
+    // few trees cannot fill the SMs with one warp each: their playouts overlap inside a CTA instead (search_wave.cuh)
     wave_ = !eps_ && ((n_trees <= 16 && sp.batch_size >= 8) || (n_trees <= 32 && sp.batch_size >= 16));
     if (const char* e = getenv("ARA_WAVE")) wave_ = !eps_ && atoi(e) != 0;
     if (wave_)

@@ -159,7 +159,7 @@ int main() {
         }
         try {
             if (cmd == "uci") {
-                std::cout << "id name CrazyAra-B200\nid author crazyara_b200 (hot path of QueensGambit/CrazyAra on sm_100a)\n";
+                std::cout << "id name CrazyAra-B200\nid author crazyara_b200 (hot path of QueensGambit/CrazyAra on sm_90a)\n";
                 for (const auto& kv : opt.kv) std::cout << "option name " << kv.first << " type string default " << kv.second << "\n";
                 std::cout << "uciok" << std::endl;
             } else if (cmd == "isready") {

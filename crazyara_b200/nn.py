@@ -2,7 +2,7 @@
 
 Same names and argument meaning as the reference class: predict(inputPlanes, valueOutput, probOutputs,
 auxiliaryOutputs) on caller-owned host buffers; shape getters.  No fallback: construction raises AraError when the
-CUDA library or an sm_100 device is missing.
+CUDA library or an sm_90 device is missing.
 """
 import ctypes
 

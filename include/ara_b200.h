@@ -1,9 +1,9 @@
-/* ara_b200.h -- C-ABI of the B200-native (sm_100a) leaf-evaluation + MCTS engine.
+/* ara_b200.h -- C-ABI of the H100-native (sm_90a) leaf-evaluation + MCTS engine.
  *
  * Every entry point is what the reference's C++ seam for this hot path would bind (file:line refer to
  * QueensGambit/CrazyAra, engine/src/...).  Plain pointers and sizes only; all functions return 0 on success
  * and -1 on failure with a message retrievable through ara_last_error() (thread local).  There is no CPU
- * fallback: creation fails on anything that is not an sm_100 device.
+ * fallback: creation fails on anything that is not an sm_90 device.
  */
 #ifndef ARA_B200_H
 #define ARA_B200_H
@@ -24,7 +24,7 @@ const char* ara_last_error(void);
  *                     device buffers and one CUDA stream on `device`, fixed maximum batch size.  `precision` is the
  *                     reference's UCI option `Precision` (uci/optionsuci.cpp:144, nn/tensorrtapi.cpp:334-360):
  *                     ARA_PRECISION_FLOAT16 (its default) = fp16 tensor-core operands, fp32 accumulation, fp16
- *                     activations; ARA_PRECISION_FLOAT32 = fp32-accurate: the same tcgen05 GEMMs with every operand
+ *                     activations; ARA_PRECISION_FLOAT32 = fp32-accurate: the same wgmma GEMMs with every operand
  *                     carried as an fp16 hi + lo pair (3x the K extent), fp32 activations between the layers --
  *                     value / probabilities within 1e-4 of an fp32 evaluation (tests/test_net_gpu.py).
  * ara_net_shape   <-> get_nb_input_values_total / get_nb_policy_values / get_nb_auxiliary_outputs /
@@ -293,7 +293,7 @@ long long ara_search_launch_count(ara_search_t s); /* search kernels launched so
  * room left for another search on top of the dead siblings (instead of giving the tree up). */
 long long ara_search_compaction_count(ara_search_t s);
 
-/* ---- debug / unit-test entries (one tcgen05 convolution layer on caller-provided device buffers) */
+/* ---- debug / unit-test entries (one wgmma convolution layer on caller-provided device buffers) */
 int ara_debug_conv(const void* act_half, int boards_cap, int boards, int cin, const void* w_half, int w_rows, int n_out,
                    int ksize, const float* bias, int relu, const void* residual, int ldr, void* out_half,
                    float* out_f32, int ldo, int bn, void* stream);

@@ -1,4 +1,4 @@
-"""tcgen05 convolution GEMM vs a plain torch fp32 convolution of the same fp16-rounded operands."""
+"""wgmma convolution GEMM vs a plain torch fp32 convolution of the same fp16-rounded operands."""
 import ctypes
 
 import pytest

@@ -3,7 +3,7 @@ buffers, in both settings of the reference's UCI option `Precision` (engine/src/
 
   float16 (the reference's default): fp16 tensor-core operands and activations, fp32 accumulation -> value within
           4e-3, probabilities within 3 % of the fp32 oracle;
-  float32: the same tcgen05 GEMMs with fp16 hi + lo operand splitting and fp32 activations between the layers ->
+  float32: the same wgmma GEMMs with fp16 hi + lo operand splitting and fp32 activations between the layers ->
           value and every probability within 1e-4 (north_star's float tolerance), in practice ~1e-6."""
 import os
 
@@ -151,23 +151,21 @@ def test_float16_and_float32_networks_agree(tmp_path, monkeypatch, name, cin, pc
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,cin,pch", [("risev2", 34, 81), ("risev33", 52, 76)])
 def test_tower_variants_are_bit_identical(tmp_path, monkeypatch, name, cin, pch):
-    """The four tower kernels must give the same bits: a search with many trees evaluates the same positions in bigger
-    batches than a single-tree search.  Two boards per CTA (large batches); one board per CTA with the squares in the
-    tensor core's M (the old small-batch kernel); one board per CTA with the channels in M (rise_trunk_t.cuh); one board per
-    CTA pair, each CTA streaming half of the weights (rise_trunk_c.cuh, the default up to 74 boards)."""
+    """The tower kernel's two shapes (one / two boards per CTA) must give the same bits: a search with many trees evaluates
+    the same positions in bigger batches.  At 140 boards the default is two boards per CTA."""
     arch = onet.arch_risev2(cin, pch) if name == "risev2" else onet.arch_risev33(cin, pch, True)
-    variants = [{"ARA_TRUNK_ROWS": "128"}, {"ARA_TRUNK_ROWS": "64", "ARA_TRUNK_T": "0"}, {"ARA_TRUNK_PAIR": "0"}, {}]
-    for n in (5, 64):  # (64: every SM of the wave busy, the hand-offs see real contention)
+    for n, variants in ((5, [{"ARA_TRUNK_ROWS": "128"}, {"ARA_TRUNK_ROWS": "64"}]),
+                        (64, [{"ARA_TRUNK_ROWS": "128"}, {"ARA_TRUNK_ROWS": "64"}]),
+                        (140, [{}, {"ARA_TRUNK_ROWS": "64"}])):
         x = golden_input(arch, n=n, seed=11)
         outs = []
         for env in variants:
-            for k in ("ARA_TRUNK_ROWS", "ARA_TRUNK_T", "ARA_TRUNK_PAIR"):
-                monkeypatch.delenv(k, raising=False)
+            monkeypatch.delenv("ARA_TRUNK_ROWS", raising=False)
             for k, v in env.items():
                 monkeypatch.setenv(k, v)
             net, _ = _make_net(tmp_path, arch, n, 10 if name == "risev2" else 30)
             v, p = np.zeros(n, np.float32), np.zeros((n, pch * 64), np.float32)
-            for _ in range(3):  # (repeated: a race between the hand-offs would not show every time)
+            for _ in range(3):  # (repeated: a race in the weight ring would not show every time)
                 net.predict(x, v, p, None, n=n)
                 outs.append((v.copy(), p.copy()))
             net.close()

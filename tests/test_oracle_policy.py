@@ -13,7 +13,6 @@ from oracle.chess import Position, lib
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "policy_tables.json")
 MODES = {"crazyhouse": 0, "chess": 1, "lichess": 2}
-REF = "/root/reference/engine"
 
 
 def _tables(mode):
@@ -32,19 +31,6 @@ def test_tables_match_golden_hashes(name):
     assert hashlib.sha256(",".join(map(str, flat)).encode()).hexdigest() == g["flat_sha256"]
     for lab, (idx, fl) in g["spot"].items():
         assert labels[idx] == lab and flat[idx] == fl
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present")
-def test_tables_match_reference_sources():
-    src = open(os.path.join(REF, "src/environments/chess_related/policymaprepresentation.h")).read()
-    parts = re.split(r"const unsigned long FLAT_PLANE_IDX\[\] = \{", src)[1:]
-    tabs = [[int(x) for x in re.findall(r"\d+", p.split("};")[0])] for p in parts]
-    leg = open(os.path.join(REF, "tests/legacyconstants.h")).read()
-    lists = [re.findall(r'"([^"]+)"', b.split("};")[0]) for b in re.split(r"const std::string LABELS\[\] = \{", leg)[1:]]
-    for name, ti in (("crazyhouse", 0), ("lichess", 1), ("chess", 2)):
-        labels, flat = _tables(MODES[name])
-        assert flat == tabs[ti], name
-        assert labels == lists[ti], name
 
 
 def test_move_index_semantics():

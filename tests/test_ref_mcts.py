@@ -1,14 +1,15 @@
 """Pins the search oracle (oracle/mcts.c) to the REFERENCE'S OWN CODE.
 
-`make -C oracle ref` compiles the reference's search sources unchanged, from where they lie under /root/reference --
-node.cpp, nodedata.cpp, searchthread.cpp, agents/mctsagent.cpp, agents/agent.cpp, evalinfo.cpp, manager/*.cpp,
+`make -C oracle ref` compiles the reference's search sources unchanged -- node.cpp, nodedata.cpp, searchthread.cpp, agents/mctsagent.cpp, agents/agent.cpp, evalinfo.cpp, manager/*.cpp,
 util/blazeutil.h, the settings structs -- into oracle/_ref/libref_mcts.so, over three stand-ins for what the tree lacks:
 oracle/ref/blaze/Math.h (blaze-lib), oracle/ref/pommermanstate.h (the environment: a `State` over oracle/chess.c,
 planes.c, policy.c) and a NeuralNetAPI subclass that calls back into the test.  Every case below runs
 MCTSAgent::evaluate_board_state (Threads 1) there and oracle/mcts.c here on the same position, settings and network, and
 demands IDENTICAL bits: visit counts, Q values, priors, MCTS posterior, root value, best-move Q, node counters -- at node
 temperature 1 and 1.7 (std::pow -> glibc powf), with Dirichlet noise (the real std::gamma_distribution over
-std::default_random_engine), with the MCTS solver on mate positions, in every virtual-loss style.
+std::default_random_engine), with the MCTS solver on mate positions, in every virtual-loss style.  The compiled
+reference's results are recorded in tests/golden/ref_mcts.npz (tests/golden/gen_ref_mcts_golden.py), keyed by the case's
+inputs, so the comparison runs wherever the oracle builds.
 
 What stays a stand-in, and is therefore NOT pinned by this: blaze's evaluation of get_current_u_values
 ((v*s)*w restructured to (v*w)*s, see blaze/Math.h), blaze::sum's reduction order, and the order of Stockfish's move
@@ -16,15 +17,41 @@ generator (the environment returns moves in ascending policy-index order).
 
 The network is oracle.search.hash_net (tie-free priors): with oracle/fake.c's 2048-level priors tied moves are common
 and std::sort's unspecified order among them (node.cpp:464-470) would be compared, not the search."""
+import hashlib
+import os
+
 import numpy as np
 import pytest
 
-from oracle import refmcts
 from oracle import search as osr
 from oracle.chess import Position
 from tests.test_search_hostemu import CASES, case_settings
 
-pytestmark = pytest.mark.skipif(not refmcts.available(), reason="oracle/_ref/libref_mcts.so not built (needs /root/reference)")
+GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "ref_mcts.npz")
+SCALARS = ("root_value", "best_move_q", "visit_sum", "free_visits", "nodes", "best_idx", "no_visit_idx")
+_RECORDED = {}
+
+
+def case_key(pos, fen, premoves, st, threads):
+    """The inputs of a search: start position and the moves played from it, every setting, thread count."""
+    return hashlib.sha1(f"{fen}|{' '.join(premoves)}|{pos.fen()}|{threads}|".encode() + bytes(st)).hexdigest()
+
+
+def recorded(key):
+    """The compiled reference's result for these inputs (per-move arrays of all cases concatenated, n_moves each)."""
+    if not _RECORDED:
+        z = np.load(GOLDEN)
+        _RECORDED["g"] = g = {k: z[k] for k in z.files}
+        ends = np.cumsum(g["n_moves"])
+        for i, (k, n, e) in enumerate(zip(g["keys"], g["n_moves"], ends)):
+            _RECORDED[str(k)] = (i, int(e - n), int(e))
+    g = _RECORDED["g"]
+    i, a, b = _RECORDED[key]
+    r = {name: g["scalars"][i][j].item() for j, name in enumerate(SCALARS)}
+    r.update({name: int(r[name]) for name in SCALARS[2:]})
+    r.update(moves=[str(m) for m in g["moves"][a:b]], visits=g["visits"][a:b], q=g["q_bits"][a:b].view(np.float32),
+             prior=g["prior_bits"][a:b].view(np.float32), policy=g["policy"][a:b])
+    return r
 
 
 def _bits(a):
@@ -35,7 +62,7 @@ def assert_oracle_equals_reference(pos, fen, vid, is960, premoves, st, threads=1
     S = osr.Search(st)
     net = osr.hash_net(S.n_labels)
     ro = S.run(pos, net, with_keys=True, threads=threads)
-    rr = refmcts.run(pos, fen, vid, is960, premoves, st, net_fn=net, channels=S.channels, n_labels=S.n_labels)
+    rr = recorded(case_key(pos, fen, premoves, st, threads))
     assert ro["visit_sum"] > 0
     assert ro["moves"] == rr["moves"]                      # same prior order (no ties with this network)
     assert np.array_equal(ro["visits"], rr["visits"])

@@ -1,7 +1,7 @@
 """GPU search (one warp per tree, device-resident SoA tree) against the CPU search oracle.
 
  (a) hash-derived fake backend on both sides -> visit counts, Q, priors, posterior, root value, counters BIT-EXACT
- (b) real tcgen05 network: the oracle search is driven by the SAME GPU network through its host API, so both sides
+ (b) real wgmma network: the oracle search is driven by the SAME GPU network through its host API, so both sides
      consume identical policy/value floats -> bit-exact at node temperature 1 and at the UCI default 1.7 (glibc's
      powf restated on the device, crazyara_b200/csrc/glibc_flt32.cuh).
 """

@@ -1,5 +1,6 @@
-// Microbenchmark: issue rate of FFMA, FHFMA (fma.rn.f32.f16) and HFMA2 on one SM (16 warps, 8 independent chains).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 tools/micro/fma_rate.cu -o build/fma_rate
+// Microbenchmark: issue rate of FFMA, the fp16 x fp16 + fp32 FMA of the depthwise stage (two halves widened to fp32, then
+// FFMA; sm_90 has no mixed-precision FMA) and HFMA2 on one SM (16 warps, 8 independent chains).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 tools/micro/fma_rate.cu -o build/fma_rate
 #include <cuda_fp16.h>
 #include <cstdio>
 template <int MODE>
@@ -16,8 +17,9 @@ __global__ void k(float* out, unsigned a0, unsigned b0, int iters, unsigned long
             if (MODE == 0) {
                 acc[i] = fmaf(acc[i], __uint_as_float(a), __uint_as_float(b));
             } else if (MODE == 1) {
-                asm volatile("{\n\t.reg .f16 xl, xh, wl, wh;\n\tmov.b32 {xl, xh}, %1;\n\tmov.b32 {wl, wh}, %2;\n\t"
-                             "fma.rn.f32.f16 %0, xl, wl, %0;\n\t}" : "+f"(acc[i]) : "r"(a), "r"(b));
+                const unsigned x = a + i;  // (per chain, so that the widening is not hoisted out of the loop)
+                acc[i] = fmaf(__low2float(*reinterpret_cast<const __half2*>(&x)),
+                              __low2float(*reinterpret_cast<const __half2*>(&b)), acc[i]);
             } else {
                 asm volatile("fma.rn.f16x2 %0, %1, %2, %0;" : "+r"(h[i]) : "r"(a), "r"(b));
             }
@@ -33,7 +35,7 @@ int main() {
     float* out; unsigned long long* cyc;
     cudaMalloc(&out, 1 << 20); cudaMalloc(&cyc, 8);
     const int iters = 4096;
-    const char* names[3] = {"FFMA", "FHFMA (fma.rn.f32.f16)", "HFMA2 (fma.rn.f16x2)"};
+    const char* names[3] = {"FFMA", "widened fp16 FMA", "HFMA2 (fma.rn.f16x2)"};
     for (int warps : {1, 4, 16}) {
         for (int mode = 0; mode < 3; ++mode) {
             unsigned long long c = 0;

@@ -1,12 +1,12 @@
 // Microbenchmark: how fast can ONE SM pull an L2-resident weight stream into shared memory?
 //   modes: 0 = 1-D bulk copies issued by one thread; 1 = by two threads (two rings); 2 = cluster multicast (every CTA
 //   of the cluster issues 1/csz of each slot to all members); 3 = ld.global.v4 + st.shared by all threads.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -Icrazyara_b200/csrc -Iinclude tools/micro/l2_ingest.cu -o build/l2_ingest
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -Icrazyara_b200/csrc -Iinclude tools/micro/l2_ingest.cu -o build/l2_ingest
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
-#include "sm100_prims.cuh"
+#include "sm90_prims.cuh"
 using namespace ara;
 
 __device__ __forceinline__ void bulk_load_1d_mc(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint16_t mask) {
@@ -92,7 +92,7 @@ int main() {
     for (int np : {2, 3, 4, 6}) {
         cfgs.push_back({1, 8192, 12, 1, 64, np});
         cfgs.push_back({1, 16384, 12, 1, 64, np});
-        cfgs.push_back({1, 16384, 12, 1, 148, np});
+        cfgs.push_back({1, 16384, 12, 1, 132, np});
     }
     cfgs.push_back({1, 32768, 6, 1, 64, 2});
     cfgs.push_back({1, 32768, 6, 1, 64, 3});

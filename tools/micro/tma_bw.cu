@@ -1,11 +1,11 @@
 // Microbenchmark: per-SM L2->shared bandwidth of TMA tensor loads vs 1-D bulk copies (weights resident in L2).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -Icrazyara_b200/csrc -Iinclude tools/micro/tma_bw.cu -o build/tma_bw -lcuda
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -Icrazyara_b200/csrc -Iinclude tools/micro/tma_bw.cu -o build/tma_bw -lcuda
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
-#include "sm100_prims.cuh"
+#include "sm90_prims.cuh"
 using namespace ara;
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -94,7 +94,7 @@ int main() {
     cudaFuncSetAttribute(tma_bw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     const int n_slots = 2 * 104 * 2;  // about two trunk passes of W1 half chunks
     const char* names[4] = {"tensor 2x{64x64} (W1 rows)", "tensor {64x128} (W2 cols)", "bulk 1-D 16 KB", "bulk 1-D 16 x 1 KB"};
-    for (int grid : {1, 32, 148})
+    for (int grid : {1, 32, 132})
         for (int mode = 0; mode < 4; ++mode)
             for (int ring : {2, 3, 6, 10}) {
                 unsigned long long cyc = 0;

@@ -29,17 +29,11 @@ L = lib()
 L.ara_net_debug_trunk_cycles.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
 if L.ara_net_debug_trunk_cycles(net._h, out) != 0:
     raise SystemExit(L.ara_last_error().decode())
-mma = ["issue + misc", "wait H2 (compute warps)", "wait W2 ring", "wait X tile (block boundary)", "wait D1 buffer",
-       "wait W1 ring"]
-cmp_ = ["X load", "SE + tile hand-over", "wait D1 (tensor core)", "TMEM read-out", "wait chunk vectors", "barrier 1",
-        "H1 write", "barrier 2", "depthwise", "wait H2 buffer", "H2 write", "wait D2", "block epilogue (D2 + b2 + X)", "SE of the next block (rest)", "tile store + hand-over", "  SE: pooling", "  SE: fc1", "  SE: hidden", "  SE: fc2"]
-if os.environ.get("ARA_TRUNK_T", "1") != "0" and B <= 148:  # rise_trunk_t.cuh's slots
-    mma = ["issue + misc", "wait X tile (block boundary)", "wait H2 (compute warps)", "wait weight stream", "wait D1 buffer"]
-    cmp_ = ["X load", "SE + tile hand-over", "wait D1 (tensor core)", "TMEM read-out + relu", "wait H2 buffer", "depthwise + H2 write",
-            "wait D2", "block epilogue (D2 + b2 + X)", "SE of the next block (rest)", "tile store + hand-over", "  SE: pooling", "  SE: fc1", "  SE: hidden", "  SE: fc2"]
-for title, names, base in (("MMA issuer warp", mma, 0), ("compute warp 2", cmp_, 16)):
-    vals = [out[base + i] for i in range(len(names))]
-    tot = sum(vals)
-    print(f"{title}: {tot / 1e3:.1f} kcycles = {tot / 1.965e3:.1f} us at 1965 MHz")
-    for n, v in zip(names, vals):
-        print(f"    {n:34s} {v / 1e3:9.1f} kcycles {100.0 * v / max(1, tot):5.1f}%")
+# RT_PROF slots of the consumer warpgroup of board 0 (rise_trunk.cuh), flushed at offset 16
+names = ["X load", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)", "epilogue 1 (relu + b1 -> H1)",
+         "depthwise -> H2", "wait W2 image", "MMA2 (wgmma m64n256)", "block epilogue (D2 + b2 + X)"]
+vals = [out[16 + i] for i in range(len(names))]
+tot = sum(vals)
+print(f"consumer warpgroup of board 0: {tot / 1e3:.1f} kcycles")
+for n, v in zip(names, vals):
+    print(f"    {n:34s} {v / 1e3:9.1f} kcycles {100.0 * v / max(1, tot):5.1f}%")

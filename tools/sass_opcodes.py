@@ -1,7 +1,5 @@
-"""Per-kernel counts of the Blackwell-specific SASS opcodes in the built library (profiles/r02_sass_opcodes.txt):
-UTCHMMA (tcgen05.mma), LDTM / STTM (tcgen05.ld / st: tensor memory), UTMALDG (TMA tensor loads), UBLKCP (bulk copies),
-UTCBAR (tcgen05.commit), SYNCS (mbarrier), REDUX, plus the total instruction count -- proof that the contraction kernels
-run on the 5th-generation tensor cores and are fed by TMA.  CPU only:  python tools/sass_opcodes.py > profiles/...txt"""
+"""Per-kernel counts of Hopper SASS opcodes in the built library: HGMMA / WARPGROUP (wgmma), UTMALDG (TMA), UBLKCP
+(bulk copies), SYNCS (mbarrier), REDUX and the total.  CPU only:  python tools/sass_opcodes.py"""
 import collections
 import os
 import re
@@ -10,7 +8,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "crazyara_b200", "libara_b200.so")
-OPS = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "UTCATOM", "SYNCS", "REDUX", "HMMA", "FFMA", "HFMA2", "DFMA", "LDS", "STS", "LDG", "STG"]
+OPS = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "REDUX", "HMMA", "FFMA", "HFMA2", "DFMA", "LDS", "STS", "LDG", "STG"]
 
 
 def main():
@@ -33,7 +31,7 @@ def main():
                     cur[o] += 1
                     break
     demangle = subprocess.run(["c++filt"], input="\n".join(kernels), capture_output=True, text=True).stdout.splitlines()
-    print(f"# {os.path.relpath(LIB, ROOT)}: SASS opcode counts per kernel (cuobjdump -sass, sm_100a)")
+    print(f"# {os.path.relpath(LIB, ROOT)}: SASS opcode counts per kernel (cuobjdump -sass, sm_90a)")
     print("# " + " ".join(f"{o:>8}" for o in ["total"] + OPS) + "  kernel")
     for (name, c), dn in zip(kernels.items(), demangle):
         short = re.sub(r"\(.*", "", dn)
