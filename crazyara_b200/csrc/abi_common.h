@@ -33,19 +33,36 @@ struct PdlSuspend {
    private:
     bool on_;
 };
+// launch_pdl with thread-block clusters of `cluster_x` CTAs along x (1: no cluster)
 template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
+cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                               unsigned cluster_x, Args... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attr[2];
+    int n = 0;
+    if (pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    if (cluster_x > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = cluster_x;
+        attr[n].val.clusterDim.y = 1;
+        attr[n].val.clusterDim.z = 1;
+        ++n;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = n;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
+    return launch_pdl_cluster(kernel, grid, block, smem, stream, 1u, args...);
 }
 
 }  // namespace ara

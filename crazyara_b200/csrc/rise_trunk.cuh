@@ -27,7 +27,8 @@ struct RtCfg {
     static_assert(kSmemBytes <= 232448, "trunk kernel shared memory exceeds the sm_90 limit of 227 KB per block");
 };
 
-// -DARA_TRUNK_PROF: per-role cycle counters of CTA 0 (args.prof[role * 16 + slot]); see tools/prof_trunk.py
+// -DARA_TRUNK_PROF: per-role cycle counters of CTA 0 (args.prof[role * 16 + slot]; role 1: rise_trunk_kernel, role 0:
+// rise_trunk_pair_kernel); see tools/prof_trunk.py
 #if defined(ARA_TRUNK_PROF)
 #define RT_PROF_DECL() long long pt_ = clock64(); unsigned long long pacc_[16] = {}
 #define RT_PROF(idx)                                               \
@@ -101,6 +102,100 @@ __device__ __forceinline__ uint32_t rt_x_off(int row, int ch) {
     return static_cast<uint32_t>((ch >> 6) * 8192 + row * 128 + ((((ch & 63) >> 3) ^ (row & 7)) << 4) + (ch & 7) * 2);
 }
 
+// The stages below are shared by every shape of the tower kernel; t is the thread's index in its warpgroup.
+
+// stem output of `board` -> the X tile (16-byte pieces into the swizzled layout); a board without input: zeros.
+// The caller synchronises the warpgroup.
+__device__ __forceinline__ void rt_load_x(uint8_t* sX, const __half* x_in, int board, bool board_ok, int t) {
+    const uint4* src = reinterpret_cast<const uint4*>(x_in + static_cast<size_t>(board) * 64 * 256);
+#pragma unroll 4
+    for (int i = 0; i < 16; ++i) {
+        const int p = t + i * 128, r = p >> 5, c16 = p & 31;
+        const uint4 v = board_ok ? __ldg(src + p) : make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(sX + (c16 >> 3) * 8192 + r * 128 + (((c16 & 7) ^ (r & 7)) << 4)) = v;
+    }
+    fence_proxy_async();
+}
+
+// squeeze-excitation on the block input, in place: thread t owns channels 2t, 2t+1
+__device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* sX, float* sPool, float* sHid, int t, int wg) {
+    float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll 8
+    for (int r = 0; r < 64; ++r) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(sX + rt_x_off(r, 2 * t)));
+        s0 += f.x, s1 += f.y;
+    }
+    sPool[2 * t] = s0 * (1.0f / 64.0f);
+    sPool[2 * t + 1] = s1 * (1.0f / 64.0f);
+    rt_wg_sync(wg);
+    float sc0, sc1;
+    if (B.se_type == 1) {  // fc1 256 -> 128 (relu), fc2 128 -> 256 (hard sigmoid)
+        float a = 0.0f;
+#pragma unroll 16
+        for (int k = 0; k < 256; ++k) a = fmaf(__half2float(B.se_w1t[k * 128 + t]), sPool[k], a);
+        sHid[t] = fmaxf(a, 0.0f);
+        rt_wg_sync(wg);
+        float a0 = 0.0f, a1 = 0.0f;
+        const __half2* w2 = reinterpret_cast<const __half2*>(B.se_w2t) + t;
+#pragma unroll 16
+        for (int j = 0; j < 128; ++j) {
+            const float2 wf = __half22float2(__ldg(w2 + j * 128));
+            a0 = fmaf(wf.x, sHid[j], a0);
+            a1 = fmaf(wf.y, sHid[j], a1);
+        }
+        sc0 = rt_hard_sigmoid(a0), sc1 = rt_hard_sigmoid(a1);
+    } else {  // 256 -> 256 + bias (hard sigmoid)
+        float a0 = 0.0f, a1 = 0.0f;
+        const __half2* w1 = reinterpret_cast<const __half2*>(B.se_w1t) + t;
+#pragma unroll 16
+        for (int k = 0; k < 256; ++k) {
+            const float2 wf = __half22float2(__ldg(w1 + k * 128));
+            a0 = fmaf(wf.x, sPool[k], a0);
+            a1 = fmaf(wf.y, sPool[k], a1);
+        }
+        sc0 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t) + a0), sc1 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t + 1) + a1);
+    }
+#pragma unroll 8
+    for (int r = 0; r < 64; ++r) {
+        __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, 2 * t));
+        const float2 f = __half22float2(*x);
+        *x = __floats2half2_rn(f.x * sc0, f.y * sc1);
+    }
+    fence_proxy_async();
+    rt_wg_sync(wg);
+}
+
+// epilogue 1: relu(D1 + b1) -> H1.  aux: the vectors of the chunk's W1 image
+__device__ __forceinline__ void rt_epilogue1(const float (&acc1)[32], const uint8_t* aux, uint8_t* sH1, int fr, int fc) {
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+        const float2 b1 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux) + 8 * jj + fc);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+            *reinterpret_cast<__half2*>(sH1 + jj * 1024 + (fr + 8 * h) * 16 + fc * 2) =
+                __floats2half2_rn(fmaxf(acc1[4 * jj + 2 * h] + b1.x, 0.0f), fmaxf(acc1[4 * jj + 2 * h + 1] + b1.y, 0.0f));
+    }
+}
+
+// depthwise k x k of H1 -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout
+__device__ __forceinline__ void rt_depthwise_stage(const uint8_t* sH1, const uint8_t* aux, uint8_t* sH2, int ksize, int t) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int item = t + i * 128;
+        const int g = item >> 6, sub = (item >> 5) & 1, y0 = ((item >> 3) & 3) * 2, x = item & 7;
+        uint2 o[2];
+        if (ksize == 3)
+            rt_depthwise4<3>(sH1, aux, g, sub, y0, x, o);
+        else
+            rt_depthwise4<5>(sH1, aux, g, sub, y0, x, o);
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+            const int rr = (y0 + jj) * 8 + x;
+            *reinterpret_cast<uint2*>(sH2 + rr * 128 + ((g ^ (rr & 7)) << 4) + sub * 8) = o[jj];
+        }
+    }
+}
+
 template <int NB>
 // A consumer needs ~230 registers (accumulators: 160).  Two boards = 12 warps, 3 per 16 K-register SM sub-partition:
 // 168 each at launch, then the producer warpgroup drops to 40 and the consumers grow to 232 (2 x 232 + 40 = 504).
@@ -168,17 +263,8 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
     const int fr = w * 16 + (lane >> 2), fc = 2 * (lane & 3);
     RT_PROF_DECL();
 
-    {   // stem output -> the X tile (16-byte pieces into the swizzled layout); rows of a board without input: zeros
-        const uint4* src = reinterpret_cast<const uint4*>(args.x_in + static_cast<size_t>(board) * 64 * 256);
-#pragma unroll 4
-        for (int i = 0; i < 16; ++i) {
-            const int p = t + i * 128, r = p >> 5, c16 = p & 31;
-            const uint4 v = board_ok ? __ldg(src + p) : make_uint4(0u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(sX + (c16 >> 3) * 8192 + r * 128 + (((c16 & 7) ^ (r & 7)) << 4)) = v;
-        }
-        fence_proxy_async();
-        rt_wg_sync(wg);
-    }
+    rt_load_x(sX, args.x_in, board, board_ok, t);
+    rt_wg_sync(wg);
     RT_PROF(0);  // X load
 
     float acc2[128];
@@ -186,53 +272,7 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
     for (int b = 0; b < n_blocks; ++b) {
         const TrunkBlock& B = args.blk[b];
         const int nch = B.n_chunks;
-        if (B.se_type != 0) {
-            // squeeze-excitation on the block input, in place: thread t owns channels 2t, 2t+1
-            float s0 = 0.0f, s1 = 0.0f;
-#pragma unroll 8
-            for (int r = 0; r < 64; ++r) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(sX + rt_x_off(r, 2 * t)));
-                s0 += f.x, s1 += f.y;
-            }
-            sPool[2 * t] = s0 * (1.0f / 64.0f);
-            sPool[2 * t + 1] = s1 * (1.0f / 64.0f);
-            rt_wg_sync(wg);
-            float sc0, sc1;
-            if (B.se_type == 1) {  // fc1 256 -> 128 (relu), fc2 128 -> 256 (hard sigmoid)
-                float a = 0.0f;
-#pragma unroll 16
-                for (int k = 0; k < 256; ++k) a = fmaf(__half2float(B.se_w1t[k * 128 + t]), sPool[k], a);
-                sHid[t] = fmaxf(a, 0.0f);
-                rt_wg_sync(wg);
-                float a0 = 0.0f, a1 = 0.0f;
-                const __half2* w2 = reinterpret_cast<const __half2*>(B.se_w2t) + t;
-#pragma unroll 16
-                for (int j = 0; j < 128; ++j) {
-                    const float2 wf = __half22float2(__ldg(w2 + j * 128));
-                    a0 = fmaf(wf.x, sHid[j], a0);
-                    a1 = fmaf(wf.y, sHid[j], a1);
-                }
-                sc0 = rt_hard_sigmoid(a0), sc1 = rt_hard_sigmoid(a1);
-            } else {  // 256 -> 256 + bias (hard sigmoid)
-                float a0 = 0.0f, a1 = 0.0f;
-                const __half2* w1 = reinterpret_cast<const __half2*>(B.se_w1t) + t;
-#pragma unroll 16
-                for (int k = 0; k < 256; ++k) {
-                    const float2 wf = __half22float2(__ldg(w1 + k * 128));
-                    a0 = fmaf(wf.x, sPool[k], a0);
-                    a1 = fmaf(wf.y, sPool[k], a1);
-                }
-                sc0 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t) + a0), sc1 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t + 1) + a1);
-            }
-#pragma unroll 8
-            for (int r = 0; r < 64; ++r) {
-                __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, 2 * t));
-                const float2 f = __half22float2(*x);
-                *x = __floats2half2_rn(f.x * sc0, f.y * sc1);
-            }
-            fence_proxy_async();
-            rt_wg_sync(wg);
-        }
+        if (B.se_type != 0) rt_squeeze_excite(B, sX, sPool, sHid, t, wg);
         RT_PROF(1);  // squeeze-excitation
 
         for (int j = 0; j < nch; ++j) {
@@ -256,32 +296,11 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
             RT_PROF(3);  // MMA1
             // ---- epilogue 1: relu(D1 + b1) -> H1
             const uint8_t* aux = w1 + kTrunkW1Tile;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                const float2 b1 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux) + 8 * jj + fc);
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    *reinterpret_cast<__half2*>(sH1 + jj * 1024 + (fr + 8 * h) * 16 + fc * 2) =
-                        __floats2half2_rn(fmaxf(acc1[4 * jj + 2 * h] + b1.x, 0.0f), fmaxf(acc1[4 * jj + 2 * h + 1] + b1.y, 0.0f));
-            }
+            rt_epilogue1(acc1, aux, sH1, fr, fc);
             rt_wg_sync(wg);  // H1 complete (and MMA2 of the previous chunk, waited by every thread, is done with H2)
             RT_PROF(4);  // epilogue 1
             // ---- depthwise k x k -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int item = t + i * 128;
-                const int g = item >> 6, sub = (item >> 5) & 1, y0 = ((item >> 3) & 3) * 2, x = item & 7;
-                uint2 o[2];
-                if (B.ksize == 3)
-                    rt_depthwise4<3>(sH1, aux, g, sub, y0, x, o);
-                else
-                    rt_depthwise4<5>(sH1, aux, g, sub, y0, x, o);
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    const int rr = (y0 + jj) * 8 + x;
-                    *reinterpret_cast<uint2*>(sH2 + rr * 128 + ((g ^ (rr & 7)) << 4) + sub * 8) = o[jj];
-                }
-            }
+            rt_depthwise_stage(sH1, aux, sH2, B.ksize, t);
             fence_proxy_async();
             rt_wg_sync(wg);
             if (t == 0) mbar_arrive(&empty[s1]);  // the W1 image (tile and vectors) is no longer read
@@ -327,6 +346,227 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
         RT_PROF(8);  // block epilogue
     }
     if (t == 0 && wg == 0) RT_PROF_FLUSH(1);
+#endif
+}
+
+
+// ------------------------------------------------------------------------------------------------------------------
+// Small batches: ONE BOARD PER CLUSTER OF TWO CTAs (one consumer warpgroup each), which puts a 64-board batch on 128
+// SMs and halves each CTA's depthwise work and weight stream.  Chunk gc (counted over the whole tower) belongs to CTA
+// gc & 1: the owner streams its W1 image, runs MMA1, epilogue 1 and the depthwise stage, and bulk-copies the 8 KB H2
+// tile into the partner's buffer of the same index.  Both CTAs run MMA2 for every chunk, in chunk order, each for its
+// own 128 trunk channels (wgmma m64n128, rows 128 r .. 128 r + 127 of the W2 image).  The block epilogue writes the
+// new X of the CTA's channels into both CTAs' X tiles; the squeeze-excitation runs in full in both CTAs on their
+// identical X copies.  Every sum has the operands and the order of the one-CTA kernel: the outputs are the same bits.
+struct RtPairCfg {
+    static constexpr int kW1Ring = 2, kW2Ring = 4, kH2Bufs = 4;  // H2 buffer gc & 3 is filled by CTA gc & 1
+    static constexpr int kW2Half = kTrunkW2Image / 2;
+    static constexpr int kThreads = 128 + 64;  // consumer warpgroup + the W1 and W2 producer warps
+    static constexpr int kOffW1 = 0;
+    static constexpr int kOffW2 = kOffW1 + kW1Ring * kTrunkW1Image;
+    static constexpr int kOffX = kOffW2 + kW2Ring * kW2Half;  // [4 K panels][64 rows][128 B]
+    static constexpr int kOffH2 = kOffX + 32768;              // [4 buffers][64 rows][128 B]
+    static constexpr int kOffH1 = kOffH2 + kH2Bufs * 8192;    // [8 groups][64 squares][16 B]
+    static constexpr int kOffSe = kOffH1 + 8192;              // pool[256] | hid[256] f32
+    static constexpr int kOffBar = kOffSe + 2048;
+    static constexpr int kSmemBytes = kOffBar + 256 + 1024 /*align slack*/;
+    static_assert(kSmemBytes <= 232448, "pair trunk kernel shared memory exceeds the sm_90 limit of 227 KB per block");
+};
+
+// launched with clusters of 2 CTAs along x: CTAs 2 i and 2 i + 1 run board i
+__global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel(const __grid_constant__ TrunkArgs args) {
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 900)
+    using Cfg = RtPairCfg;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kOffBar);
+    uint64_t* w1_full = bars;                        // [2]
+    uint64_t* w1_empty = w1_full + Cfg::kW1Ring;     // [2]
+    uint64_t* w2_full = w1_empty + Cfg::kW1Ring;     // [4]
+    uint64_t* w2_empty = w2_full + Cfg::kW2Ring;     // [4]
+    uint64_t* h2_full = w2_empty + Cfg::kW2Ring;     // [4] (partner's buffers) local arm + the partner's bulk copy
+    uint64_t* h2_free = h2_full + Cfg::kH2Bufs;      // [4] (own buffers) MMA2 done with it, here and in the partner
+    uint64_t* x_full = h2_free + Cfg::kH2Bufs;       // 128 partner threads: their channels of the new X are stored
+    uint64_t* x_free = x_full + 1;                   // the partner no longer reads its X tile of this block
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const uint32_t rank = cluster_ctarank(), peer = rank ^ 1u;
+    const int board = static_cast<int>(blockIdx.x) >> 1;
+    const int n_blocks = args.n_blocks;
+    const int n_chunks = args.blk[n_blocks - 1].chunk0 + args.blk[n_blocks - 1].n_chunks;
+    // device-side batch size: both CTAs of a cluster share the board, so they leave together
+    if (args.boards_dev != nullptr && board >= *args.boards_dev) return;
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < Cfg::kW1Ring; ++i) mbar_init(&w1_full[i], 1), mbar_init(&w1_empty[i], 1);
+        for (int i = 0; i < Cfg::kW2Ring; ++i) mbar_init(&w2_full[i], 1), mbar_init(&w2_empty[i], 1);
+        for (int i = 0; i < Cfg::kH2Bufs; ++i) mbar_init(&h2_full[i], 1), mbar_init(&h2_free[i], 2);
+        mbar_init(x_full, 128);
+        mbar_init(x_free, 1);
+        fence_mbar_init();
+    }
+    pdl_wait();
+    pdl_launch_dependents();
+
+    const int t = threadIdx.x & 127;
+    const int w = t >> 5;
+    const bool board_ok = board * 64 < args.M;
+    uint8_t* sX = smem + Cfg::kOffX;
+    uint8_t* sH1 = smem + Cfg::kOffH1;
+    float* sPool = reinterpret_cast<float*>(smem + Cfg::kOffSe);
+    float* sHid = sPool + 256;
+    RT_PROF_DECL();
+    if (warp < 4) rt_load_x(sX, args.x_in, board, board_ok, t);
+    // the partner's barriers exist before anything arrives on them, and both CTAs have read their input before either
+    // writes the output (which may alias it)
+    cluster_sync_all();
+
+    if (warp >= 4) {
+        // ---------------------------------------------------------------- producers: W1 images of the own chunks, W2 halves of all
+        if (lane == 0) {
+            if (warp == 4) {
+                for (int gc = static_cast<int>(rank), u = 0; gc < n_chunks; gc += 2, ++u) {
+                    const int s = u % Cfg::kW1Ring;
+                    mbar_wait_relaxed(&w1_empty[s], ((u / Cfg::kW1Ring) & 1) ^ 1);
+                    mbar_arrive_expect_tx(&w1_full[s], kTrunkW1Image);
+                    bulk_load_1d(smem + Cfg::kOffW1 + s * kTrunkW1Image, args.w1_img + static_cast<size_t>(gc) * kTrunkW1Image,
+                                 kTrunkW1Image, &w1_full[s]);
+                }
+            } else {
+                for (int gc = 0; gc < n_chunks; ++gc) {
+                    const int s = gc % Cfg::kW2Ring;
+                    mbar_wait_relaxed(&w2_empty[s], ((gc / Cfg::kW2Ring) & 1) ^ 1);
+                    mbar_arrive_expect_tx(&w2_full[s], Cfg::kW2Half);
+                    bulk_load_1d(smem + Cfg::kOffW2 + s * Cfg::kW2Half,
+                                 args.w2_img + static_cast<size_t>(gc) * kTrunkW2Image + rank * Cfg::kW2Half, Cfg::kW2Half, &w2_full[s]);
+                }
+            }
+        }
+        __syncwarp();
+    } else {
+        // -------------------------------------------------------------------- consumer warpgroup: half of one board
+        const uint32_t aX = smem_u32(sX);
+        const uint32_t rX = cluster_map(sX, peer);
+        const int fr = w * 16 + (lane >> 2), fc = 2 * (lane & 3);
+        RT_PROF(0);  // X load (and the cluster barrier)
+        float acc2[64];
+        for (int b = 0; b < n_blocks; ++b) {
+            const TrunkBlock& B = args.blk[b];
+            const int nch = B.n_chunks;
+            if (B.se_type != 0) rt_squeeze_excite(B, sX, sPool, sHid, t, 0);
+            RT_PROF(1);  // squeeze-excitation
+            int own = B.chunk0 + ((B.chunk0 & 1) != static_cast<int>(rank));  // the next own chunk without its H2
+            for (int j = 0; j < nch; ++j) {
+                const int gc = B.chunk0 + j;
+                // the own chunk of {gc, gc + 1} first, so that the two CTAs run their depthwise stages side by side
+                for (; own < B.chunk0 + nch && own <= gc + 1; own += 2) {
+                    // ---- MMA1, epilogue 1, depthwise -> H2 buffer, and its copy to the partner
+                    const int u1 = own >> 1, s1 = u1 % Cfg::kW1Ring;
+                    uint8_t* oH2 = smem + Cfg::kOffH2 + (own & 3) * 8192;
+                    mbar_wait(&w1_full[s1], (u1 / Cfg::kW1Ring) & 1);
+                    RT_PROF(2);  // wait for the W1 image
+                    const uint8_t* w1 = smem + Cfg::kOffW1 + s1 * kTrunkW1Image;
+                    const uint32_t aW1 = smem_u32(w1);
+                    float acc1[32];
+                    wgmma_fence();
+#pragma unroll
+                    for (int p = 0; p < 4; ++p)
+#pragma unroll
+                        for (int k = 0; k < 4; ++k)
+                            wgmma_f16<64>(acc1, wgmma_desc_k_sw128(aX + p * 8192 + k * 32, 1024),
+                                          wgmma_desc_k_sw128(aW1 + p * 8192 + k * 32, 1024), (p > 0 || k > 0) ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(acc1);
+                    RT_PROF(3);  // MMA1
+                    const uint8_t* aux = w1 + kTrunkW1Tile;
+                    rt_epilogue1(acc1, aux, sH1, fr, fc);
+                    rt_wg_sync(0);
+                    RT_PROF(4);  // epilogue 1
+                    // both CTAs' MMA2 of chunk own - 4 are done with the buffer
+                    mbar_wait_cluster(&h2_free[own & 3], ((own >> 2) & 1) ^ 1);
+                    RT_PROF(5);  // wait for the H2 buffer
+                    rt_depthwise_stage(sH1, aux, oH2, B.ksize, t);
+                    fence_proxy_async();
+                    rt_wg_sync(0);
+                    if (t == 0) {
+                        mbar_arrive(&w1_empty[s1]);
+                        bulk_copy_to_cta(cluster_map(oH2, peer), oH2, 8192, cluster_map(&h2_full[own & 3], peer));
+                    }
+                    RT_PROF(6);  // depthwise
+                }
+                const int buf = gc & 3;
+                uint8_t* sH2 = smem + Cfg::kOffH2 + buf * 8192;
+                if ((gc & 1) != static_cast<int>(rank)) {
+                    // ---- the partner's H2 of this chunk
+                    if (t == 0) mbar_arrive_expect_tx(&h2_full[buf], 8192);
+                    mbar_wait(&h2_full[buf], (gc >> 2) & 1);
+                    RT_PROF(7);  // wait for the partner's H2
+                }
+                // ---- MMA2: D2[:, 128 r .. 128 r + 127] += H2 . W2[128 r .. 128 r + 127]^T
+                const int s2 = gc % Cfg::kW2Ring;
+                mbar_wait(&w2_full[s2], (gc / Cfg::kW2Ring) & 1);
+                RT_PROF(8);  // wait for the W2 half
+                const uint32_t aW2 = smem_u32(smem + Cfg::kOffW2 + s2 * Cfg::kW2Half), aH2 = smem_u32(sH2);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    wgmma_f16<128>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
+                                   (j > 0 || k > 0) ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs(acc2);
+                if (t == 0) {
+                    mbar_arrive(&w2_empty[s2]);
+                    if ((gc & 1) == static_cast<int>(rank))
+                        mbar_arrive(&h2_free[buf]);
+                    else
+                        mbar_arrive_cluster(cluster_map(&h2_free[buf], peer));
+                }
+                RT_PROF(9);  // MMA2
+            }
+            // ---- block epilogue: X <- (D2 + b2) + X for the own 128 channels, into both X tiles (the last block: to
+            // global memory)
+            const bool last = b == n_blocks - 1;
+            if (!last) {
+                if (t == 0) mbar_arrive_cluster(cluster_map(x_free, peer));  // every read of this block's X is done
+                mbar_wait_cluster(x_free, b & 1);
+            }
+            RT_PROF(10);  // wait for the partner to release its X tile
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj) {
+                const int c = static_cast<int>(rank) * 128 + 8 * jj + fc;
+                const float2 b2 = __ldg(reinterpret_cast<const float2*>(B.b2 + c));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = fr + 8 * h;
+                    const uint32_t off = rt_x_off(r, c);
+                    __half2* x = reinterpret_cast<__half2*>(sX + off);
+                    const float2 xr = __half22float2(*x);
+                    const __half2 y = __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
+                    if (!last) {
+                        *x = y;
+                        st_cluster_b32(rX + off, *reinterpret_cast<const uint32_t*>(&y));
+                    } else if (board_ok) {
+                        *reinterpret_cast<__half2*>(args.out + (static_cast<size_t>(board) * 64 + r) * 256 + c) = y;
+                    }
+                }
+            }
+            if (!last) {
+                fence_proxy_async_cluster();
+                mbar_arrive_cluster(cluster_map(x_full, peer));
+                RT_PROF(11);  // block epilogue and the exchange
+                mbar_wait_cluster(x_full, b & 1);
+                fence_proxy_async();
+                rt_wg_sync(0);
+                RT_PROF(12);  // wait for the partner's channels of X
+            }
+        }
+        if (t == 0 && rank == 0) RT_PROF_FLUSH(0);
+    }
+    // no CTA leaves while its partner may still copy into or arrive on its shared memory
+    cluster_sync_all();
 #endif
 }
 

@@ -90,12 +90,26 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
     T->args.prof = static_cast<unsigned long long*>(T->d_prof);
     ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<1>::kSmemBytes));
     ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<2>::kSmemBytes));
+    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RtPairCfg::kSmemBytes));
     {
         int dev = 0;
         cudaDeviceProp prop;
         ARA_CUDA_OK(cudaGetDevice(&dev));
         ARA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
         T->sm_count = prop.multiProcessorCount;
+        // how many CTA pairs can be resident at once (a cluster lives inside one GPC, so this can be below sm_count / 2)
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(2 * (T->sm_count / 2));
+        cfg.blockDim = dim3(RtPairCfg::kThreads);
+        cfg.dynamicSmemBytes = RtPairCfg::kSmemBytes;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        ARA_CUDA_OK(cudaOccupancyMaxActiveClusters(&T->pair_clusters, rise_trunk_pair_kernel, &cfg));
     }
     return 0;
 }
@@ -105,10 +119,15 @@ int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const
     if (x_in != nullptr) a.x_in = x_in;
     a.M = boards * 64;
     a.boards_dev = boards_dev;
-    // one board per CTA while that fits one wave, else two sharing a weight stream (ARA_TRUNK_ROWS=64 / 128 forces)
+    // one board per CTA pair while every pair is resident at once, else one board per CTA while that fits one wave, else
+    // two boards per CTA sharing a weight stream.  ARA_TRUNK_ROWS (trunk rows per CTA) forces a shape: 32 = the pair
+    // (half of a board's channels per CTA), 64 = one board per CTA, any other value = two boards per CTA.
     const char* force = getenv("ARA_TRUNK_ROWS");
-    const bool one_board = force ? atoi(force) == 64 : boards <= T->sm_count;
-    if (one_board)
+    const int rows = force ? atoi(force) : boards <= T->pair_clusters ? 32 : boards <= T->sm_count ? 64 : 128;
+    if (rows == 32)
+        ARA_CUDA_OK(launch_pdl_cluster(rise_trunk_pair_kernel, dim3(2 * boards), dim3(RtPairCfg::kThreads), RtPairCfg::kSmemBytes,
+                                       stream, 2u, a));
+    else if (rows == 64)
         ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<1>, dim3(boards), dim3(RtCfg<1>::kThreads), RtCfg<1>::kSmemBytes, stream, a));
     else
         ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<2>, dim3((boards + 1) / 2), dim3(RtCfg<2>::kThreads), RtCfg<2>::kSmemBytes, stream, a));

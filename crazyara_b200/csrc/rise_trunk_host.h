@@ -28,6 +28,7 @@ struct RiseTrunk {
     void* d_w1 = nullptr;
     void* d_w2 = nullptr;
     int sm_count = 0;
+    int pair_clusters = 0;  // CTA pairs of rise_trunk_pair_kernel resident at once
     void* d_prof = nullptr;  // [2][16] cycle counters, written only by -DARA_TRUNK_PROF builds
     std::vector<void*> d_se;  // fp16 copies of the squeeze-excitation matrices
 };

@@ -64,9 +64,26 @@ __device__ __forceinline__ uint32_t cluster_map(const void* local, uint32_t cta)
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(local)), "r"(cta));
     return r;
 }
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
 __device__ __forceinline__ void st_cluster_v4(uint32_t raddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(raddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void st_cluster_b32(uint32_t raddr, uint32_t v) {
+    asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(raddr), "r"(v) : "memory");
+}
+// bulk copy of this CTA's shared memory into another CTA's (dst and bar: cluster_map addresses); completes `bytes` on
+// the receiver's mbarrier.  Sizes and addresses are multiples of 16.
+__device__ __forceinline__ void bulk_copy_to_cta(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+                 "r"(smem_u32(src)), "r"(bytes), "r"(bar)
+                 : "memory");
+}
+// generic-proxy shared-memory writes of this thread (to any CTA of the cluster) become visible to the async proxy
+__device__ __forceinline__ void fence_proxy_async_cluster() { asm volatile("fence.proxy.async.shared::cluster;" ::: "memory"); }
 // arrive on an mbarrier of another CTA of the cluster; release at cluster scope: the arriving thread's earlier
 // remote stores are visible to whoever acquires the barrier phase
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t rbar) {

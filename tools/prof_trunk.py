@@ -29,11 +29,20 @@ L = lib()
 L.ara_net_debug_trunk_cycles.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
 if L.ara_net_debug_trunk_cycles(net._h, out) != 0:
     raise SystemExit(L.ara_last_error().decode())
-# RT_PROF slots of the consumer warpgroup of board 0 (rise_trunk.cuh), flushed at offset 16
-names = ["X load", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)", "epilogue 1 (relu + b1 -> H1)",
-         "depthwise -> H2", "wait W2 image", "MMA2 (wgmma m64n256)", "block epilogue (D2 + b2 + X)"]
-vals = [out[16 + i] for i in range(len(names))]
+# RT_PROF slots of the consumer warpgroup of board 0 (rise_trunk.cuh): rise_trunk_kernel flushes at offset 16, the pair
+# kernel (its CTA of rank 0) at offset 0
+if any(out[i] for i in range(16)):
+    shape, base = "pair kernel, CTA of rank 0", 0
+    names = ["X load + cluster barrier", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)",
+             "epilogue 1 (relu + b1 -> H1)", "wait own H2 buffer free", "depthwise -> H2 + copy", "wait partner's H2",
+             "wait W2 half", "MMA2 (wgmma m64n128)", "wait partner's X free", "block epilogue + X exchange",
+             "wait partner's X"]
+else:
+    shape, base = "one / two boards per CTA", 16
+    names = ["X load", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)", "epilogue 1 (relu + b1 -> H1)",
+             "depthwise -> H2", "wait W2 image", "MMA2 (wgmma m64n256)", "block epilogue (D2 + b2 + X)"]
+vals = [out[base + i] for i in range(len(names))]
 tot = sum(vals)
-print(f"consumer warpgroup of board 0: {tot / 1e3:.1f} kcycles")
+print(f"consumer warpgroup of board 0 ({shape}): {tot / 1e3:.1f} kcycles")
 for n, v in zip(names, vals):
     print(f"    {n:34s} {v / 1e3:9.1f} kcycles {100.0 * v / max(1, tot):5.1f}%")
