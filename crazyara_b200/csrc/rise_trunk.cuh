@@ -165,23 +165,28 @@ __device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* 
     rt_wg_sync(wg);
 }
 
-// epilogue 1: relu(D1 + b1) -> H1.  aux: the vectors of the chunk's W1 image
-__device__ __forceinline__ void rt_epilogue1(const float (&acc1)[32], const uint8_t* aux, uint8_t* sH1, int fr, int fc) {
+// epilogue 1: relu(D1 + b1) -> H1 for the N / 4 8-channel groups g0 .. g0 + N / 4 - 1.  acc1: the N accumulator
+// registers of a wgmma m64n(2 N) over those channels.  aux: the vectors of the chunk's W1 image
+template <int N>
+__device__ __forceinline__ void rt_epilogue1(const float (&acc1)[N], const uint8_t* aux, uint8_t* sH1, int fr, int fc, int g0 = 0) {
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-        const float2 b1 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux) + 8 * jj + fc);
+    for (int jj = 0; jj < N / 4; ++jj) {
+        const int g = g0 + jj;
+        const float2 b1 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux) + 8 * g + fc);
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-            *reinterpret_cast<__half2*>(sH1 + jj * 1024 + (fr + 8 * h) * 16 + fc * 2) =
+            *reinterpret_cast<__half2*>(sH1 + g * 1024 + (fr + 8 * h) * 16 + fc * 2) =
                 __floats2half2_rn(fmaxf(acc1[4 * jj + 2 * h] + b1.x, 0.0f), fmaxf(acc1[4 * jj + 2 * h + 1] + b1.y, 0.0f));
     }
 }
 
-// depthwise k x k of H1 -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout
-__device__ __forceinline__ void rt_depthwise_stage(const uint8_t* sH1, const uint8_t* aux, uint8_t* sH2, int ksize, int t) {
+// depthwise k x k of H1 -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout, for the NG 8-channel groups
+// g0 .. g0 + NG - 1, by the 128 threads of a warpgroup
+template <int NG = 8>
+__device__ __forceinline__ void rt_depthwise_stage(const uint8_t* sH1, const uint8_t* aux, uint8_t* sH2, int ksize, int t, int g0 = 0) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int item = t + i * 128;
+    for (int i = 0; i < NG / 2; ++i) {
+        const int item = g0 * 64 + t + i * 128;
         const int g = item >> 6, sub = (item >> 5) & 1, y0 = ((item >> 3) & 3) * 2, x = item & 7;
         uint2 o[2];
         if (ksize == 3)
@@ -351,43 +356,134 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// Small batches: ONE BOARD PER CLUSTER OF TWO CTAs (one consumer warpgroup each), which puts a 64-board batch on 128
-// SMs and halves each CTA's depthwise work and weight stream.  Chunk gc (counted over the whole tower) belongs to CTA
-// gc & 1: the owner streams its W1 image, runs MMA1, epilogue 1 and the depthwise stage, and bulk-copies the 8 KB H2
-// tile into the partner's buffer of the same index.  Both CTAs run MMA2 for every chunk, in chunk order, each for its
-// own 128 trunk channels (wgmma m64n128, rows 128 r .. 128 r + 127 of the W2 image).  The block epilogue writes the
-// new X of the CTA's channels into both CTAs' X tiles; the squeeze-excitation runs in full in both CTAs on their
-// identical X copies.  Every sum has the operands and the order of the one-CTA kernel: the outputs are the same bits.
+// Small batches: ONE BOARD PER CLUSTER OF TWO CTAs, which puts a 64-board batch on 128 SMs and halves each CTA's
+// depthwise work and weight stream.  Chunk gc (counted over the whole tower) belongs to CTA gc & 1: the owner streams its
+// W1 image, runs MMA1, epilogue 1 and the depthwise stage, and bulk-copies the 8 KB H2 tile into the partner's buffer of
+// the same index.  Both CTAs run MMA2 for every chunk, in chunk order, each for its own 128 trunk channels (rows
+// 128 r .. 128 r + 127 of the W2 image).
+// Each CTA has two consumer warpgroups split by output channel, so that two warps share every SM sub-partition in the
+// CUDA-core stages.  Warpgroup w runs MMA1 (wgmma m64n32), epilogue 1 and the depthwise stage for operating channels
+// 32 w .. 32 w + 31 of a chunk (H1 / H2 channel groups 4 w .. 4 w + 3), and MMA2 (m64n64) and the block epilogue for trunk
+// channels 128 r + 64 w .. 128 r + 64 w + 63, which are K panel 2 r + w of X: the new panel goes to the partner as one
+// 8 KB bulk copy.  The squeeze-excitation is split across the pair: each CTA computes the outputs of its own channels
+// from weights streamed through its W2 ring and stores them into both CTAs over DSMEM, so both scale their X copies
+// with the same bits.  Every sum has the operands and the order of the one-CTA kernel: the outputs are the same bits.
 struct RtPairCfg {
     static constexpr int kW1Ring = 2, kW2Ring = 4, kH2Bufs = 4;  // H2 buffer gc & 3 is filled by CTA gc & 1
     static constexpr int kW2Half = kTrunkW2Image / 2;
-    static constexpr int kThreads = 128 + 64;  // consumer warpgroup + the W1 and W2 producer warps
+    static constexpr int kSeUnits = kTrunkSeImage / kW2Half;  // W2 ring units of a block's SE image, all resident at once
+    static constexpr int kThreads = 256 + 64;  // two consumer warpgroups + the W1 and W2 producer warps
     static constexpr int kOffW1 = 0;
     static constexpr int kOffW2 = kOffW1 + kW1Ring * kTrunkW1Image;
     static constexpr int kOffX = kOffW2 + kW2Ring * kW2Half;  // [4 K panels][64 rows][128 B]
     static constexpr int kOffH2 = kOffX + 32768;              // [4 buffers][64 rows][128 B]
     static constexpr int kOffH1 = kOffH2 + kH2Bufs * 8192;    // [8 groups][64 squares][16 B]
-    static constexpr int kOffSe = kOffH1 + 8192;              // pool[256] | hid[256] f32
-    static constexpr int kOffBar = kOffSe + 2048;
+    static constexpr int kOffSe = kOffH1 + 8192;              // pool[256] | hid[128] | scale[256] f32
+    static constexpr int kOffBar = kOffSe + 2560;
     static constexpr int kSmemBytes = kOffBar + 256 + 1024 /*align slack*/;
+    static_assert(kSeUnits <= kW2Ring, "a block's SE image must fit the W2 ring");
     static_assert(kSmemBytes <= 232448, "pair trunk kernel shared memory exceeds the sm_90 limit of 227 KB per block");
 };
+
+// both consumer warpgroups of a pair CTA (named barrier 3; 1 and 2 are the warpgroups' own)
+__device__ __forceinline__ void rt_pair_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
+
+// squeeze-excitation of the pair on the block input, in place; tid: 0 .. 255 over both consumer warpgroups.  Each CTA
+// pools all 256 channels of its own X copy (thread tid: channel tid), then computes the outputs of its rank r from its
+// SE image (unit i in ring slot (u2 + i) % kW2Ring), each one sequential sum: ca_se hidden 64 r .. 64 r + 63 (threads
+// 0..63), exchanged through hid_bar, then the scales of channels 128 r .. 128 r + 127 (threads 0..127); eca_se those
+// scales directly.  Every output is stored into both CTAs; hid_bar / scale_bar (64 / 128 arrivals from the partner)
+// complete when the partner's share is in.  hid_bar advances on ca_se blocks only, scale_bar on every SE block, so each
+// has its own phase parity.  On return no thread reads the SE image any more.
+__device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint8_t* sX, const uint8_t* ring, int u2, float* sPool,
+                                                       float* sHid, float* sScale, uint64_t* hid_bar, uint64_t* scale_bar,
+                                                       uint32_t hid_parity, uint32_t scale_parity, uint32_t rank, int tid) {
+    const uint32_t peer = rank ^ 1u;
+    const auto unit = [&](int i) {
+        return reinterpret_cast<const __half*>(ring + ((u2 + i) % RtPairCfg::kW2Ring) * RtPairCfg::kW2Half);
+    };
+    float s = 0.0f;
+#pragma unroll 8
+    for (int r = 0; r < 64; ++r) s += __half2float(*reinterpret_cast<const __half*>(sX + rt_x_off(r, tid)));
+    sPool[tid] = s * (1.0f / 64.0f);
+    rt_pair_sync();
+    float sc = 0.0f;
+    if (B.se_type == 1) {  // fc1 256 -> 128 (relu), fc2 128 -> 256 (hard sigmoid)
+        if (tid < 64) {
+            float a = 0.0f;
+#pragma unroll 1
+            for (int q = 0; q < 2; ++q) {  // [256 k][64]: 128 k per unit
+                const __half* wq = unit(q) + tid;
+#pragma unroll 16
+                for (int k = 0; k < 128; ++k) a = fmaf(__half2float(wq[k * 64]), sPool[128 * q + k], a);
+            }
+            const float h = fmaxf(a, 0.0f);
+            const int o = 64 * static_cast<int>(rank) + tid;
+            sHid[o] = h;
+            st_cluster_b32(cluster_map(sHid + o, peer), __float_as_uint(h));
+            mbar_arrive_cluster(cluster_map(hid_bar, peer));
+        }
+        if (tid < 128) {
+            rt_wg_sync(0);                       // the own hidden values
+            mbar_wait_cluster(hid_bar, hid_parity);  // the partner's
+            float a = 0.0f;
+#pragma unroll 1
+            for (int q = 0; q < 2; ++q) {  // [128 j][128]: 64 j per unit
+                const __half* wq = unit(2 + q) + tid;
+#pragma unroll 16
+                for (int j = 0; j < 64; ++j) a = fmaf(__half2float(wq[j * 128]), sHid[64 * q + j], a);
+            }
+            sc = rt_hard_sigmoid(a);
+        }
+    } else if (tid < 128) {  // 256 -> 256 + bias (hard sigmoid): [256 k][128], 64 k per unit
+        float a = 0.0f;
+#pragma unroll 1
+        for (int q = 0; q < 4; ++q) {
+            const __half* wq = unit(q) + tid;
+#pragma unroll 16
+            for (int k = 0; k < 64; ++k) a = fmaf(__half2float(wq[k * 128]), sPool[64 * q + k], a);
+        }
+        sc = rt_hard_sigmoid(__ldg(B.se_b + 128 * rank + tid) + a);
+    }
+    if (tid < 128) {
+        const int c = 128 * static_cast<int>(rank) + tid;
+        sScale[c] = sc;
+        st_cluster_b32(cluster_map(sScale + c, peer), __float_as_uint(sc));
+        mbar_arrive_cluster(cluster_map(scale_bar, peer));
+    }
+    mbar_wait_cluster(scale_bar, scale_parity);  // the partner's scales
+    rt_pair_sync();                        // the own scales
+    // X *= scale: thread tid scales channels 2 (tid & 127), 2 (tid & 127) + 1 in rows 32 (tid >> 7) .. + 31
+    const int cp = 2 * (tid & 127), r0 = 32 * (tid >> 7);
+    const float sc0 = sScale[cp], sc1 = sScale[cp + 1];
+#pragma unroll 8
+    for (int r = r0; r < r0 + 32; ++r) {
+        __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, cp));
+        const float2 f = __half22float2(*x);
+        *x = __floats2half2_rn(f.x * sc0, f.y * sc1);
+    }
+    fence_proxy_async();
+    rt_pair_sync();
+}
 
 // launched with clusters of 2 CTAs along x: CTAs 2 i and 2 i + 1 run board i
 __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel(const __grid_constant__ TrunkArgs args) {
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 900)
     using Cfg = RtPairCfg;
+    constexpr int R2 = Cfg::kW2Ring;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kOffBar);
     uint64_t* w1_full = bars;                        // [2]
     uint64_t* w1_empty = w1_full + Cfg::kW1Ring;     // [2]
     uint64_t* w2_full = w1_empty + Cfg::kW1Ring;     // [4]
-    uint64_t* w2_empty = w2_full + Cfg::kW2Ring;     // [4]
-    uint64_t* h2_full = w2_empty + Cfg::kW2Ring;     // [4] (partner's buffers) local arm + the partner's bulk copy
-    uint64_t* h2_free = h2_full + Cfg::kH2Bufs;      // [4] (own buffers) MMA2 done with it, here and in the partner
-    uint64_t* x_full = h2_free + Cfg::kH2Bufs;       // 128 partner threads: their channels of the new X are stored
+    uint64_t* w2_empty = w2_full + R2;               // [4] one arrival per consumer warpgroup
+    uint64_t* h2_full = w2_empty + R2;               // [4] (partner's buffers) local arm + the partner's bulk copy
+    uint64_t* h2_free = h2_full + Cfg::kH2Bufs;      // [4] (own buffers) MMA2 done with it, both warpgroups of both CTAs
+    uint64_t* x_full = h2_free + Cfg::kH2Bufs;       // local arm + the partner's two bulk copies of its X panels
     uint64_t* x_free = x_full + 1;                   // the partner no longer reads its X tile of this block
+    uint64_t* se_hid = x_free + 1;                   // 64 partner threads: their ca_se hidden values are stored
+    uint64_t* se_scale = se_hid + 1;                 // 128 partner threads: their SE scales are stored
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -400,15 +496,18 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < Cfg::kW1Ring; ++i) mbar_init(&w1_full[i], 1), mbar_init(&w1_empty[i], 1);
-        for (int i = 0; i < Cfg::kW2Ring; ++i) mbar_init(&w2_full[i], 1), mbar_init(&w2_empty[i], 1);
-        for (int i = 0; i < Cfg::kH2Bufs; ++i) mbar_init(&h2_full[i], 1), mbar_init(&h2_free[i], 2);
-        mbar_init(x_full, 128);
+        for (int i = 0; i < R2; ++i) mbar_init(&w2_full[i], 1), mbar_init(&w2_empty[i], 2);
+        for (int i = 0; i < Cfg::kH2Bufs; ++i) mbar_init(&h2_full[i], 1), mbar_init(&h2_free[i], 4);
+        mbar_init(x_full, 1);
         mbar_init(x_free, 1);
+        mbar_init(se_hid, 64);
+        mbar_init(se_scale, 128);
         fence_mbar_init();
     }
     pdl_wait();
     pdl_launch_dependents();
 
+    const int wg = warp >> 2;
     const int t = threadIdx.x & 127;
     const int w = t >> 5;
     const bool board_ok = board * 64 < args.M;
@@ -416,16 +515,18 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
     uint8_t* sH1 = smem + Cfg::kOffH1;
     float* sPool = reinterpret_cast<float*>(smem + Cfg::kOffSe);
     float* sHid = sPool + 256;
+    float* sScale = sHid + 128;
     RT_PROF_DECL();
     if (warp < 4) rt_load_x(sX, args.x_in, board, board_ok, t);
     // the partner's barriers exist before anything arrives on them, and both CTAs have read their input before either
     // writes the output (which may alias it)
     cluster_sync_all();
 
-    if (warp >= 4) {
-        // ---------------------------------------------------------------- producers: W1 images of the own chunks, W2 halves of all
+    if (warp >= 8) {
+        // ---------------------------------------------------------------- producers: W1 images of the own chunks; SE
+        // images and W2 halves of every block, in the order the consumers read them
         if (lane == 0) {
-            if (warp == 4) {
+            if (warp == 8) {
                 for (int gc = static_cast<int>(rank), u = 0; gc < n_chunks; gc += 2, ++u) {
                     const int s = u % Cfg::kW1Ring;
                     mbar_wait_relaxed(&w1_empty[s], ((u / Cfg::kW1Ring) & 1) ^ 1);
@@ -434,86 +535,104 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                                  kTrunkW1Image, &w1_full[s]);
                 }
             } else {
-                for (int gc = 0; gc < n_chunks; ++gc) {
-                    const int s = gc % Cfg::kW2Ring;
-                    mbar_wait_relaxed(&w2_empty[s], ((gc / Cfg::kW2Ring) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&w2_full[s], Cfg::kW2Half);
-                    bulk_load_1d(smem + Cfg::kOffW2 + s * Cfg::kW2Half,
-                                 args.w2_img + static_cast<size_t>(gc) * kTrunkW2Image + rank * Cfg::kW2Half, Cfg::kW2Half, &w2_full[s]);
+                int u = 0;
+                for (int b = 0; b < n_blocks; ++b) {
+                    const TrunkBlock& B = args.blk[b];
+                    const int n_se = B.se_type != 0 ? Cfg::kSeUnits : 0;
+                    for (int i = 0; i < n_se + B.n_chunks; ++i, ++u) {
+                        const int s = u % R2;
+                        mbar_wait_relaxed(&w2_empty[s], ((u / R2) & 1) ^ 1);
+                        const uint8_t* src = i < n_se ? B.se_img + rank * kTrunkSeImage + i * Cfg::kW2Half
+                                                      : args.w2_img + static_cast<size_t>(B.chunk0 + i - n_se) * kTrunkW2Image + rank * Cfg::kW2Half;
+                        mbar_arrive_expect_tx(&w2_full[s], Cfg::kW2Half);
+                        bulk_load_1d(smem + Cfg::kOffW2 + s * Cfg::kW2Half, src, Cfg::kW2Half, &w2_full[s]);
+                    }
                 }
             }
         }
         __syncwarp();
     } else {
-        // -------------------------------------------------------------------- consumer warpgroup: half of one board
+        // -------------------------------------------------------------------- consumer warpgroup wg: a quarter of one board
         const uint32_t aX = smem_u32(sX);
-        const uint32_t rX = cluster_map(sX, peer);
         const int fr = w * 16 + (lane >> 2), fc = 2 * (lane & 3);
         RT_PROF(0);  // X load (and the cluster barrier)
-        float acc2[64];
+        float acc2[32];
+        int u2 = 0;    // position in the W2 ring's stream
+        int n_se = 0;  // squeeze-excitations so far (phase of se_scale)
+        int n_ca = 0;  // ca_se squeeze-excitations so far (phase of se_hid: eca_se blocks do not arrive on it)
         for (int b = 0; b < n_blocks; ++b) {
             const TrunkBlock& B = args.blk[b];
             const int nch = B.n_chunks;
-            if (B.se_type != 0) rt_squeeze_excite(B, sX, sPool, sHid, t, 0);
-            RT_PROF(1);  // squeeze-excitation
+            if (B.se_type != 0) {
+                for (int i = 0; i < Cfg::kSeUnits; ++i) mbar_wait(&w2_full[(u2 + i) % R2], ((u2 + i) / R2) & 1);
+                RT_PROF(1);  // wait for the SE image
+                rt_pair_squeeze_excite(B, sX, smem + Cfg::kOffW2, u2, sPool, sHid, sScale, se_hid, se_scale, n_ca & 1, n_se & 1, rank,
+                                       threadIdx.x);
+                if (t == 0)
+                    for (int i = 0; i < Cfg::kSeUnits; ++i) mbar_arrive(&w2_empty[(u2 + i) % R2]);
+                u2 += Cfg::kSeUnits;
+                ++n_se;
+                n_ca += B.se_type == 1;
+            }
+            RT_PROF(2);  // squeeze-excitation
             int own = B.chunk0 + ((B.chunk0 & 1) != static_cast<int>(rank));  // the next own chunk without its H2
             for (int j = 0; j < nch; ++j) {
                 const int gc = B.chunk0 + j;
                 // the own chunk of {gc, gc + 1} first, so that the two CTAs run their depthwise stages side by side
                 for (; own < B.chunk0 + nch && own <= gc + 1; own += 2) {
-                    // ---- MMA1, epilogue 1, depthwise -> H2 buffer, and its copy to the partner
+                    // ---- MMA1, epilogue 1, depthwise -> H2 buffer (this warpgroup's 32 channels), its copy to the partner
                     const int u1 = own >> 1, s1 = u1 % Cfg::kW1Ring;
                     uint8_t* oH2 = smem + Cfg::kOffH2 + (own & 3) * 8192;
                     mbar_wait(&w1_full[s1], (u1 / Cfg::kW1Ring) & 1);
-                    RT_PROF(2);  // wait for the W1 image
+                    RT_PROF(3);  // wait for the W1 image
                     const uint8_t* w1 = smem + Cfg::kOffW1 + s1 * kTrunkW1Image;
-                    const uint32_t aW1 = smem_u32(w1);
-                    float acc1[32];
+                    const uint32_t aW1 = smem_u32(w1) + wg * 4096;  // rows 32 wg .. of every K panel
+                    float acc1[16];
                     wgmma_fence();
 #pragma unroll
                     for (int p = 0; p < 4; ++p)
 #pragma unroll
                         for (int k = 0; k < 4; ++k)
-                            wgmma_f16<64>(acc1, wgmma_desc_k_sw128(aX + p * 8192 + k * 32, 1024),
+                            wgmma_f16<32>(acc1, wgmma_desc_k_sw128(aX + p * 8192 + k * 32, 1024),
                                           wgmma_desc_k_sw128(aW1 + p * 8192 + k * 32, 1024), (p > 0 || k > 0) ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<0>();
                     wgmma_fence_regs(acc1);
-                    RT_PROF(3);  // MMA1
+                    RT_PROF(4);  // MMA1
                     const uint8_t* aux = w1 + kTrunkW1Tile;
-                    rt_epilogue1(acc1, aux, sH1, fr, fc);
-                    rt_wg_sync(0);
-                    RT_PROF(4);  // epilogue 1
+                    rt_epilogue1(acc1, aux, sH1, fr, fc, 4 * wg);
+                    rt_wg_sync(wg);  // the warpgroup's H1 groups are complete
+                    RT_PROF(5);  // epilogue 1
                     // both CTAs' MMA2 of chunk own - 4 are done with the buffer
                     mbar_wait_cluster(&h2_free[own & 3], ((own >> 2) & 1) ^ 1);
-                    RT_PROF(5);  // wait for the H2 buffer
-                    rt_depthwise_stage(sH1, aux, oH2, B.ksize, t);
+                    RT_PROF(6);  // wait for the H2 buffer
+                    rt_depthwise_stage<4>(sH1, aux, oH2, B.ksize, t, 4 * wg);
                     fence_proxy_async();
-                    rt_wg_sync(0);
-                    if (t == 0) {
+                    rt_pair_sync();  // H2 complete; no warpgroup reads the W1 image any more
+                    if (threadIdx.x == 0) {
                         mbar_arrive(&w1_empty[s1]);
                         bulk_copy_to_cta(cluster_map(oH2, peer), oH2, 8192, cluster_map(&h2_full[own & 3], peer));
                     }
-                    RT_PROF(6);  // depthwise
+                    RT_PROF(7);  // depthwise
                 }
                 const int buf = gc & 3;
                 uint8_t* sH2 = smem + Cfg::kOffH2 + buf * 8192;
                 if ((gc & 1) != static_cast<int>(rank)) {
                     // ---- the partner's H2 of this chunk
-                    if (t == 0) mbar_arrive_expect_tx(&h2_full[buf], 8192);
+                    if (threadIdx.x == 0) mbar_arrive_expect_tx(&h2_full[buf], 8192);
                     mbar_wait(&h2_full[buf], (gc >> 2) & 1);
-                    RT_PROF(7);  // wait for the partner's H2
+                    RT_PROF(8);  // wait for the partner's H2
                 }
-                // ---- MMA2: D2[:, 128 r .. 128 r + 127] += H2 . W2[128 r .. 128 r + 127]^T
-                const int s2 = gc % Cfg::kW2Ring;
-                mbar_wait(&w2_full[s2], (gc / Cfg::kW2Ring) & 1);
-                RT_PROF(8);  // wait for the W2 half
-                const uint32_t aW2 = smem_u32(smem + Cfg::kOffW2 + s2 * Cfg::kW2Half), aH2 = smem_u32(sH2);
+                // ---- MMA2: D2[:, 64 p .. 64 p + 63] += H2 . W2[64 p .. 64 p + 63]^T, p = 2 r + wg
+                const int s2 = u2 % R2;
+                mbar_wait(&w2_full[s2], (u2 / R2) & 1);
+                RT_PROF(9);  // wait for the W2 half
+                const uint32_t aW2 = smem_u32(smem + Cfg::kOffW2 + s2 * Cfg::kW2Half) + wg * 8192, aH2 = smem_u32(sH2);
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    wgmma_f16<128>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
-                                   (j > 0 || k > 0) ? 1u : 0u);
+                    wgmma_f16<64>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
+                                  (j > 0 || k > 0) ? 1u : 0u);
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_regs(acc2);
@@ -524,46 +643,55 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                     else
                         mbar_arrive_cluster(cluster_map(&h2_free[buf], peer));
                 }
-                RT_PROF(9);  // MMA2
+                ++u2;
+                RT_PROF(10);  // MMA2
             }
-            // ---- block epilogue: X <- (D2 + b2) + X for the own 128 channels, into both X tiles (the last block: to
-            // global memory)
+            // ---- block epilogue: X <- (D2 + b2) + X for K panel 2 r + wg, copied into the partner's X tile (the last
+            // block: to global memory)
             const bool last = b == n_blocks - 1;
+            rt_pair_sync();  // neither warpgroup reads this block's X any more
             if (!last) {
-                if (t == 0) mbar_arrive_cluster(cluster_map(x_free, peer));  // every read of this block's X is done
+                if (threadIdx.x == 0) {
+                    mbar_arrive_expect_tx(x_full, 2 * 8192);
+                    mbar_arrive_cluster(cluster_map(x_free, peer));
+                }
                 mbar_wait_cluster(x_free, b & 1);
             }
-            RT_PROF(10);  // wait for the partner to release its X tile
+            RT_PROF(11);  // wait for the partner to release its X tile
+            const int panel = 2 * static_cast<int>(rank) + wg;
 #pragma unroll
-            for (int jj = 0; jj < 16; ++jj) {
-                const int c = static_cast<int>(rank) * 128 + 8 * jj + fc;
+            for (int jj = 0; jj < 8; ++jj) {
+                const int c = 64 * panel + 8 * jj + fc;
                 const float2 b2 = __ldg(reinterpret_cast<const float2*>(B.b2 + c));
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int r = fr + 8 * h;
-                    const uint32_t off = rt_x_off(r, c);
-                    __half2* x = reinterpret_cast<__half2*>(sX + off);
+                    __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, c));
                     const float2 xr = __half22float2(*x);
                     const __half2 y = __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
-                    if (!last) {
+                    if (!last)
                         *x = y;
-                        st_cluster_b32(rX + off, *reinterpret_cast<const uint32_t*>(&y));
-                    } else if (board_ok) {
+                    else if (board_ok)
                         *reinterpret_cast<__half2*>(args.out + (static_cast<size_t>(board) * 64 + r) * 256 + c) = y;
-                    }
                 }
             }
             if (!last) {
-                fence_proxy_async_cluster();
-                mbar_arrive_cluster(cluster_map(x_full, peer));
-                RT_PROF(11);  // block epilogue and the exchange
-                mbar_wait_cluster(x_full, b & 1);
                 fence_proxy_async();
-                rt_wg_sync(0);
-                RT_PROF(12);  // wait for the partner's channels of X
+                rt_wg_sync(wg);
+                // nothing waits for this copy to finish reading the panel: the panel is written again (the next SE's
+                // scaling, the next block epilogue) only after the partner has waited x_full for the copy and then
+                // arrived on se_scale or x_free.  Keep that order when changing either step.
+                if (t == 0) {
+                    uint8_t* pX = sX + panel * 8192;
+                    bulk_copy_to_cta(cluster_map(pX, peer), pX, 8192, cluster_map(x_full, peer));
+                }
+                RT_PROF(12);  // block epilogue and the copy
+                mbar_wait(x_full, b & 1);  // the partner's two panels
+                rt_pair_sync();            // the other warpgroup's panel
+                RT_PROF(13);  // wait for the partner's channels of X
             }
         }
-        if (t == 0 && rank == 0) RT_PROF_FLUSH(0);
+        if (t == 0 && wg == 0 && rank == 0) RT_PROF_FLUSH(0);
     }
     // no CTA leaves while its partner may still copy into or arrive on its shared memory
     cluster_sync_all();

@@ -14,6 +14,10 @@ constexpr int kTrunkW1Tile = 32768;
 constexpr int kTrunkAuxBytes = 3712;   // 64 f32 + 64 f32 + 25 * 64 f16
 constexpr int kTrunkW1Image = 36864;   // tile + aux, padded to 1 KB
 constexpr int kTrunkW2Image = 32768;
+// Squeeze-excitation image of a block for one CTA of rise_trunk_pair_kernel (rank r), fp16:
+//   ca_se:  fc1 columns 64 r .. 64 r + 63 as [256 k][64]  |  fc2 columns 128 r .. 128 r + 127 as [128 j][128]
+//   eca_se: columns 128 r .. 128 r + 127 as [256 k][128]
+constexpr int kTrunkSeImage = 65536;
 
 struct TrunkBlock {
     int n_chunks;     // ceil(Cop / 64)
@@ -24,6 +28,7 @@ struct TrunkBlock {
     const __half* se_w1t;  // ca_se: [256][128]; eca_se: [256][256] (transposed, fp16 copy owned by the trunk)
     const __half* se_w2t;  // ca_se: [128][256]
     const float* se_b;     // eca_se: [256]
+    const uint8_t* se_img;  // [2 ranks][kTrunkSeImage] (rise_trunk_pair_kernel)
 };
 
 struct TrunkArgs {

@@ -45,6 +45,24 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
             T->d_se.push_back(d);
             B.se_w1t = static_cast<const __half*>(d);
             B.se_w2t = n2 ? static_cast<const __half*>(d) + n1 : nullptr;
+            // the pair kernel's images: each CTA gets the columns of the outputs it computes
+            std::vector<__half> img(2 * kTrunkSeImage / sizeof(__half));
+            for (int r = 0; r < 2; ++r) {
+                __half* o = img.data() + r * kTrunkSeImage / sizeof(__half);
+                if (h.se_type == 1) {
+                    for (int k = 0; k < 256; ++k)
+                        for (int i = 0; i < 64; ++i) o[k * 64 + i] = hh[k * 128 + 64 * r + i];
+                    for (int j = 0; j < 128; ++j)
+                        for (int i = 0; i < 128; ++i) o[256 * 64 + j * 128 + i] = hh[n1 + j * 256 + 128 * r + i];
+                } else {
+                    for (int k = 0; k < 256; ++k)
+                        for (int i = 0; i < 128; ++i) o[k * 128 + i] = hh[k * 256 + 128 * r + i];
+                }
+            }
+            ARA_CUDA_OK(cudaMalloc(&d, img.size() * sizeof(__half)));
+            ARA_CUDA_OK(cudaMemcpy(d, img.data(), img.size() * sizeof(__half), cudaMemcpyHostToDevice));
+            T->d_se.push_back(d);
+            B.se_img = static_cast<const uint8_t*>(d);
         }
         chunks += B.n_chunks;
     }

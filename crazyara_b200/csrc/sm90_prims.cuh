@@ -82,8 +82,6 @@ __device__ __forceinline__ void bulk_copy_to_cta(uint32_t dst, const void* src, 
                  "r"(smem_u32(src)), "r"(bytes), "r"(bar)
                  : "memory");
 }
-// generic-proxy shared-memory writes of this thread (to any CTA of the cluster) become visible to the async proxy
-__device__ __forceinline__ void fence_proxy_async_cluster() { asm volatile("fence.proxy.async.shared::cluster;" ::: "memory"); }
 // arrive on an mbarrier of another CTA of the cluster; release at cluster scope: the arriving thread's earlier
 // remote stores are visible to whoever acquires the barrier phase
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t rbar) {

@@ -30,13 +30,13 @@ L.ara_net_debug_trunk_cycles.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
 if L.ara_net_debug_trunk_cycles(net._h, out) != 0:
     raise SystemExit(L.ara_last_error().decode())
 # RT_PROF slots of the consumer warpgroup of board 0 (rise_trunk.cuh): rise_trunk_kernel flushes at offset 16, the pair
-# kernel (its CTA of rank 0) at offset 0
+# kernel (warpgroup 0 of its CTA of rank 0) at offset 0
 if any(out[i] for i in range(16)):
-    shape, base = "pair kernel, CTA of rank 0", 0
-    names = ["X load + cluster barrier", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)",
-             "epilogue 1 (relu + b1 -> H1)", "wait own H2 buffer free", "depthwise -> H2 + copy", "wait partner's H2",
-             "wait W2 half", "MMA2 (wgmma m64n128)", "wait partner's X free", "block epilogue + X exchange",
-             "wait partner's X"]
+    shape, base = "pair kernel, warpgroup 0 of the CTA of rank 0", 0
+    names = ["X load + cluster barrier", "wait SE image", "squeeze-excitation (split)", "wait W1 image",
+             "MMA1 (wgmma m64n32)", "epilogue 1 (relu + b1 -> H1)", "wait own H2 buffer free",
+             "depthwise -> H2 + copy", "wait partner's H2", "wait W2 half", "MMA2 (wgmma m64n64)",
+             "wait partner's X free", "block epilogue + X panel copy", "wait partner's X"]
 else:
     shape, base = "one / two boards per CTA", 16
     names = ["X load", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)", "epilogue 1 (relu + b1 -> H1)",
