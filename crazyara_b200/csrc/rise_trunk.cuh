@@ -640,8 +640,8 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                     mbar_arrive(&w2_empty[s2]);
                     if ((gc & 1) == static_cast<int>(rank))
                         mbar_arrive(&h2_free[buf]);
-                    else
-                        mbar_arrive_cluster(cluster_map(&h2_free[buf], peer));
+                    else  // the partner overwrites this buffer with its next H2 (a bulk copy) after this arrival
+                        mbar_arrive_cluster_free(cluster_map(&h2_free[buf], peer));
                 }
                 ++u2;
                 RT_PROF(10);  // MMA2

@@ -87,6 +87,12 @@ __device__ __forceinline__ void bulk_copy_to_cta(uint32_t dst, const void* src, 
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t rbar) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
 }
+// arrive on an mbarrier of another CTA that tells it a buffer is free: this CTA's reads of the buffer are complete and
+// it publishes no data, so the arrival releases at CTA scope only.  The cluster-scope release above costs a
+// MEMBAR.ALL.GPU per arrival.
+__device__ __forceinline__ void mbar_arrive_cluster_free(uint32_t rbar) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
+}
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
     uint32_t ok = 0;
     while (!ok) {
