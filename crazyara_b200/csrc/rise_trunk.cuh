@@ -55,44 +55,46 @@ __device__ __forceinline__ uint32_t rt_pack(float a, float b) {
     return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// depthwise k x k for 2 vertically adjacent squares (rows y0, y0+1, column x) and the 4 channels `sub` of the 8-channel
-// group g.  sH1: [8 groups][64 squares][8 channels] fp16; aux: b1[64] f32 | bd[64] f32 | wd[k*k][64] f16
+// depthwise k x k, + bd, relu for the whole column x (8 squares) of the channel pair 8 g + 2 p, 8 g + 2 p + 1, into the
+// H2 tile.  sH1: [8 groups][64 squares][8 channels] fp16; aux: b1[64] f32 | bd[64] f32 | wd[k*k][64] f16.
+// Each H1 value and each weight is loaded and widened once; the 16 accumulators stay in registers.  Every output
+// keeps one FMA order: bd, then dxi outer (columns outside the board skipped), dyi inner (rows outside the board as
+// zero operands), each a fp32 fmaf of the widened fp16 operands (their product is exact in fp32, so this gives the bits
+// of a mixed-precision fp16 x fp16 + fp32 FMA).  The three tower shapes share that order, so their outputs are the same
+// bits; tests/test_trunk_depthwise_bits_gpu.py pins it.
 template <int K>
-__device__ __forceinline__ void rt_depthwise4(const uint8_t* sH1, const uint8_t* aux, int g, int sub, int y0, int x,
-                                              uint2 (&out)[2]) {
-    constexpr int R = K / 2, NR = 2 + 2 * R;
-    const float4 b0 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(aux + 256) + g * 8 + sub * 4);
-    const uint8_t* wd = aux + 512 + g * 16 + sub * 8;
-    float acc[2][4];
+__device__ __forceinline__ void rt_depthwise_column(const uint8_t* sH1, const uint8_t* aux, uint8_t* sH2, int g, int p, int x) {
+    constexpr int R = K / 2;
+    const float2 b0 = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(aux + 256) + g * 8 + 2 * p);
+    const uint8_t* wd = aux + 512 + g * 16 + p * 4;
+    const uint8_t* col = sH1 + g * 1024 + p * 4;  // square s of the pair: col + 16 s
+    float acc[8][2];
 #pragma unroll
-    for (int j = 0; j < 2; ++j) acc[j][0] = b0.x, acc[j][1] = b0.y, acc[j][2] = b0.z, acc[j][3] = b0.w;
-    const uint8_t* base = sH1 + g * 1024 + sub * 8;  // 64 rows of 16 bytes per channel group
+    for (int y = 0; y < 8; ++y) acc[y][0] = b0.x, acc[y][1] = b0.y;
 #pragma unroll
     for (int dxi = 0; dxi < K; ++dxi) {
         const int xx = x + dxi - R;
         if (xx < 0 || xx > 7) continue;
-        uint2 in[NR];
+        float2 in[8], w[K];
 #pragma unroll
-        for (int i = 0; i < NR; ++i) {
-            const int yy = y0 - R + i;
-            in[i] = make_uint2(0u, 0u);
-            if (yy >= 0 && yy <= 7) in[i] = *reinterpret_cast<const uint2*>(base + ((yy * 8 + xx) << 4));
-        }
+        for (int yy = 0; yy < 8; ++yy) in[yy] = rt_unpack(*reinterpret_cast<const uint32_t*>(col + ((yy * 8 + xx) << 4)));
 #pragma unroll
-        for (int dyi = 0; dyi < K; ++dyi) {
-            const uint2 w = *reinterpret_cast<const uint2*>(wd + (dyi * K + dxi) * 128);
+        for (int dyi = 0; dyi < K; ++dyi) w[dyi] = rt_unpack(*reinterpret_cast<const uint32_t*>(wd + (dyi * K + dxi) * 128));
 #pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                fhfma2(acc[j][0], acc[j][1], in[j + dyi].x, w.x);
-                fhfma2(acc[j][2], acc[j][3], in[j + dyi].y, w.y);
+        for (int y = 0; y < 8; ++y)
+#pragma unroll
+            for (int dyi = 0; dyi < K; ++dyi) {
+                const int yy = y + dyi - R;
+                const float2 v = yy >= 0 && yy <= 7 ? in[yy] : make_float2(0.0f, 0.0f);
+                acc[y][0] = fmaf(v.x, w[dyi].x, acc[y][0]);
+                acc[y][1] = fmaf(v.y, w[dyi].y, acc[y][1]);
             }
-        }
     }
+    // H2 row s = 8 y + x (s & 7 = x): channel group g sits in 16-byte chunk g ^ x
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        out[j].x = rt_pack(fmaxf(acc[j][0], 0.0f), fmaxf(acc[j][1], 0.0f));
-        out[j].y = rt_pack(fmaxf(acc[j][2], 0.0f), fmaxf(acc[j][3], 0.0f));
-    }
+    for (int y = 0; y < 8; ++y)
+        *reinterpret_cast<uint32_t*>(sH2 + (y * 8 + x) * 128 + ((g ^ x) << 4) + p * 4) =
+            rt_pack(fmaxf(acc[y][0], 0.0f), fmaxf(acc[y][1], 0.0f));
 }
 
 
@@ -181,23 +183,18 @@ __device__ __forceinline__ void rt_epilogue1(const float (&acc1)[N], const uint8
 }
 
 // depthwise k x k of H1 -> H2 (A operand of MMA2) in the 128B-swizzled K-major layout, for the NG 8-channel groups
-// g0 .. g0 + NG - 1, by the 128 threads of a warpgroup
+// g0 .. g0 + NG - 1, by the 128 threads of a warpgroup.  Warp w takes groups g0 + w, g0 + w + 4, ...: lane = 4 x + p,
+// so that each row of a group is one conflict-free 128-byte load of the warp, and each H2 row one conflict-free store.
 template <int NG = 8>
 __device__ __forceinline__ void rt_depthwise_stage(const uint8_t* sH1, const uint8_t* aux, uint8_t* sH2, int ksize, int t, int g0 = 0) {
+    const int x = (t >> 2) & 7, p = t & 3;
 #pragma unroll
-    for (int i = 0; i < NG / 2; ++i) {
-        const int item = g0 * 64 + t + i * 128;
-        const int g = item >> 6, sub = (item >> 5) & 1, y0 = ((item >> 3) & 3) * 2, x = item & 7;
-        uint2 o[2];
+    for (int i = 0; i < NG / 4; ++i) {
+        const int g = g0 + (t >> 5) + 4 * i;
         if (ksize == 3)
-            rt_depthwise4<3>(sH1, aux, g, sub, y0, x, o);
+            rt_depthwise_column<3>(sH1, aux, sH2, g, p, x);
         else
-            rt_depthwise4<5>(sH1, aux, g, sub, y0, x, o);
-#pragma unroll
-        for (int jj = 0; jj < 2; ++jj) {
-            const int rr = (y0 + jj) * 8 + x;
-            *reinterpret_cast<uint2*>(sH2 + rr * 128 + ((g ^ (rr & 7)) << 4) + sub * 8) = o[jj];
-        }
+            rt_depthwise_column<5>(sH1, aux, sH2, g, p, x);
     }
 }
 
@@ -392,9 +389,9 @@ __device__ __forceinline__ void rt_pair_sync() { asm volatile("bar.sync 3, 256;"
 // pools all 256 channels of its own X copy (thread tid: channel tid), then computes the outputs of its rank r from its
 // SE image (unit i in ring slot (u2 + i) % kW2Ring), each one sequential sum: ca_se hidden 64 r .. 64 r + 63 (threads
 // 0..63), exchanged through hid_bar, then the scales of channels 128 r .. 128 r + 127 (threads 0..127); eca_se those
-// scales directly.  Every output is stored into both CTAs; hid_bar / scale_bar (64 / 128 arrivals from the partner)
-// complete when the partner's share is in.  hid_bar advances on ca_se blocks only, scale_bar on every SE block, so each
-// has its own phase parity.  On return no thread reads the SE image any more.
+// scales directly.  Every output is stored into both CTAs; the partner's stores are st.async that complete bytes on
+// hid_bar / scale_bar, which thread 0 arms for 64 / 128 values.  hid_bar advances on ca_se blocks only, scale_bar on
+// every SE block, so each has its own phase parity.  On return no thread reads the SE image any more.
 __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint8_t* sX, const uint8_t* ring, int u2, float* sPool,
                                                        float* sHid, float* sScale, uint64_t* hid_bar, uint64_t* scale_bar,
                                                        uint32_t hid_parity, uint32_t scale_parity, uint32_t rank, int tid) {
@@ -402,6 +399,13 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
     const auto unit = [&](int i) {
         return reinterpret_cast<const __half*>(ring + ((u2 + i) % RtPairCfg::kW2Ring) * RtPairCfg::kW2Half);
     };
+    // thread 0 waited for the previous phase of both barriers in the previous SE.  The partner's stores of this phase may
+    // land before the arm; those of the next phase cannot: the partner makes them only after it has received this CTA's
+    // X panels of this block, which this CTA sends after this SE.
+    if (tid == 0) {
+        if (B.se_type == 1) mbar_arrive_expect_tx(hid_bar, 64 * 4);
+        mbar_arrive_expect_tx(scale_bar, 128 * 4);
+    }
     float s = 0.0f;
 #pragma unroll 8
     for (int r = 0; r < 64; ++r) s += __half2float(*reinterpret_cast<const __half*>(sX + rt_x_off(r, tid)));
@@ -420,8 +424,7 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
             const float h = fmaxf(a, 0.0f);
             const int o = 64 * static_cast<int>(rank) + tid;
             sHid[o] = h;
-            st_cluster_b32(cluster_map(sHid + o, peer), __float_as_uint(h));
-            mbar_arrive_cluster(cluster_map(hid_bar, peer));
+            st_async_cluster_b32(cluster_map(sHid + o, peer), __float_as_uint(h), cluster_map(hid_bar, peer));
         }
         if (tid < 128) {
             rt_wg_sync(0);                       // the own hidden values
@@ -448,8 +451,7 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
     if (tid < 128) {
         const int c = 128 * static_cast<int>(rank) + tid;
         sScale[c] = sc;
-        st_cluster_b32(cluster_map(sScale + c, peer), __float_as_uint(sc));
-        mbar_arrive_cluster(cluster_map(scale_bar, peer));
+        st_async_cluster_b32(cluster_map(sScale + c, peer), __float_as_uint(sc), cluster_map(scale_bar, peer));
     }
     mbar_wait_cluster(scale_bar, scale_parity);  // the partner's scales
     rt_pair_sync();                        // the own scales
@@ -482,8 +484,8 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
     uint64_t* h2_free = h2_full + Cfg::kH2Bufs;      // [4] (own buffers) MMA2 done with it, both warpgroups of both CTAs
     uint64_t* x_full = h2_free + Cfg::kH2Bufs;       // local arm + the partner's two bulk copies of its X panels
     uint64_t* x_free = x_full + 1;                   // the partner no longer reads its X tile of this block
-    uint64_t* se_hid = x_free + 1;                   // 64 partner threads: their ca_se hidden values are stored
-    uint64_t* se_scale = se_hid + 1;                 // 128 partner threads: their SE scales are stored
+    uint64_t* se_hid = x_free + 1;                   // local arm + the partner's 64 ca_se hidden values (st.async)
+    uint64_t* se_scale = se_hid + 1;                 // local arm + the partner's 128 SE scales (st.async)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -500,8 +502,8 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
         for (int i = 0; i < Cfg::kH2Bufs; ++i) mbar_init(&h2_full[i], 1), mbar_init(&h2_free[i], 4);
         mbar_init(x_full, 1);
         mbar_init(x_free, 1);
-        mbar_init(se_hid, 64);
-        mbar_init(se_scale, 128);
+        mbar_init(se_hid, 1);
+        mbar_init(se_scale, 1);
         fence_mbar_init();
     }
     pdl_wait();
@@ -653,7 +655,10 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
             if (!last) {
                 if (threadIdx.x == 0) {
                     mbar_arrive_expect_tx(x_full, 2 * 8192);
-                    mbar_arrive_cluster(cluster_map(x_free, peer));
+                    // the partner bulk-copies its panels 2 peer + {0, 1} into this CTA's X tile after this arrival.  It
+                    // publishes no data: this CTA's MMA1 reads of X completed at wgmma.wait_group and its SE reads were
+                    // consumed before the pair barrier above, and its block epilogue touches only its own panels.
+                    mbar_arrive_cluster_free(cluster_map(x_free, peer));
                 }
                 mbar_wait_cluster(x_free, b & 1);
             }

@@ -161,4 +161,59 @@ void rise_trunk_destroy(RiseTrunk* T) {
     T->d_w1 = T->d_w2 = T->d_prof = nullptr;
 }
 
+namespace {
+
+int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1, const float* b1,
+                    const float* wd, const float* bd, const float* w2, const float* b2, __half* out_h, RiseTrunk* T,
+                    std::vector<void*>& dev) {
+    if (n < 1 || n_blocks < 1 || n_blocks > kTrunkMaxBlocks) return set_error("ara_debug_trunk: %d boards, %d blocks", n, n_blocks);
+    const size_t x_bytes = static_cast<size_t>(n) * 64 * 256 * sizeof(__half);
+    std::vector<TrunkBlockHost> blocks(n_blocks);
+    for (int i = 0; i < n_blocks; ++i) {
+        TrunkBlockHost& h = blocks[i];
+        const int c = c_op[i], kk = ksize[i] * ksize[i];
+        if (c < 1) return set_error("ara_debug_trunk: block %d has no operating channels", i);
+        h.c_op = c;
+        h.ksize = ksize[i];
+        h.w1.assign(w1, w1 + static_cast<size_t>(c) * 256);
+        h.b1.assign(b1, b1 + c);
+        h.wd.assign(wd, wd + static_cast<size_t>(c) * kk);
+        h.bd.assign(bd, bd + c);
+        h.w2.assign(w2, w2 + static_cast<size_t>(256) * c);
+        w1 += static_cast<size_t>(c) * 256, b1 += c, wd += static_cast<size_t>(c) * kk, bd += c, w2 += static_cast<size_t>(256) * c;
+        void* d = nullptr;
+        ARA_CUDA_OK(cudaMalloc(&d, 256 * sizeof(float)));
+        dev.push_back(d);
+        ARA_CUDA_OK(cudaMemcpy(d, b2 + 256 * i, 256 * sizeof(float), cudaMemcpyHostToDevice));
+        h.b2 = static_cast<const float*>(d);
+    }
+    void *d_x = nullptr, *d_out = nullptr;
+    ARA_CUDA_OK(cudaMalloc(&d_x, x_bytes));
+    dev.push_back(d_x);
+    ARA_CUDA_OK(cudaMalloc(&d_out, x_bytes));
+    dev.push_back(d_out);
+    ARA_CUDA_OK(cudaMemcpy(d_x, x_h, x_bytes, cudaMemcpyHostToDevice));
+    if (rise_trunk_init(T, blocks, static_cast<const __half*>(d_x), n, static_cast<__half*>(d_out))) return -1;
+    if (rise_trunk_launch(T, n, nullptr)) return -1;
+    ARA_CUDA_OK(cudaStreamSynchronize(nullptr));
+    ARA_CUDA_OK(cudaMemcpy(out_h, d_out, x_bytes, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+}  // namespace
+
 }  // namespace ara
+
+// Debug / unit-test entry: the tower kernel alone, on the shape ARA_TRUNK_ROWS selects (else the one the batch
+// selects).  Host buffers: x_half and out_half [n][64 squares][256] fp16; the folded weights of the blocks (no
+// squeeze-excitation) one block after the other in the layouts of TrunkBlockHost; b2 [n_blocks][256].
+extern "C" int ara_debug_trunk(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1,
+                               const float* b1, const float* wd, const float* bd, const float* w2, const float* b2, void* out_half) {
+    ara::RiseTrunk T;
+    std::vector<void*> dev;
+    const int rc = ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2,
+                                        static_cast<__half*>(out_half), &T, dev);
+    ara::rise_trunk_destroy(&T);
+    for (void* p : dev) cudaFree(p);
+    return rc;
+}

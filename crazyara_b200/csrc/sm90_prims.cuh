@@ -72,8 +72,11 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void st_cluster_v4(uint32_t raddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(raddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-__device__ __forceinline__ void st_cluster_b32(uint32_t raddr, uint32_t v) {
-    asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(raddr), "r"(v) : "memory");
+// store into another CTA's shared memory that completes 4 bytes on the receiver's mbarrier (raddr and rbar: cluster_map
+// addresses in the same CTA).  The receiver's wait on the barrier phase sees the value; no fence is issued.
+__device__ __forceinline__ void st_async_cluster_b32(uint32_t raddr, uint32_t v, uint32_t rbar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(raddr), "r"(v), "r"(rbar)
+                 : "memory");
 }
 // bulk copy of this CTA's shared memory into another CTA's (dst and bar: cluster_map addresses); completes `bytes` on
 // the receiver's mbarrier.  Sizes and addresses are multiples of 16.
@@ -89,7 +92,7 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t rbar) {
 }
 // arrive on an mbarrier of another CTA that tells it a buffer is free: this CTA's reads of the buffer are complete and
 // it publishes no data, so the arrival releases at CTA scope only.  The cluster-scope release above costs a
-// MEMBAR.ALL.GPU per arrival.
+// MEMBAR.ALL.GPU per arrival; data goes with st_async_cluster_b32 or a bulk copy instead.
 __device__ __forceinline__ void mbar_arrive_cluster_free(uint32_t rbar) {
     asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory");
 }
@@ -158,14 +161,6 @@ template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-// FMA on packed halves into fp32: acc0 += x.lo * w.lo, acc1 += x.hi * w.hi.  The product of two fp16 values is exact in
-// fp32, so widening first and using the fp32 FMA gives the bits of a mixed-precision fp16 x fp16 + fp32 FMA.
-__device__ __forceinline__ void fhfma2(float& acc0, float& acc1, uint32_t x, uint32_t w) {
-    const float2 xf = __half22float2(*reinterpret_cast<const __half2*>(&x));
-    const float2 wf = __half22float2(*reinterpret_cast<const __half2*>(&w));
-    acc0 = fmaf(xf.x, wf.x, acc0);
-    acc1 = fmaf(xf.y, wf.y, acc1);
 }
 
 }  // namespace ara

@@ -298,6 +298,11 @@ int ara_debug_conv(const void* act_half, int boards_cap, int boards, int cin, co
                    int ksize, const float* bias, int relu, const void* residual, int ldr, void* out_half,
                    float* out_f32, int ldo, int bn, void* stream);
 int ara_debug_choose_bn(int boards, int n_out);
+/* the residual tower kernel alone on host buffers, on the shape ARA_TRUNK_ROWS selects: x_half, out_half [n][64][256]
+ * fp16; per block (no squeeze-excitation), one after the other: w1 [c_op][256], b1 [c_op], wd [c_op][k*k], bd [c_op],
+ * w2 [256][c_op], b2 [256] (BN folded) */
+int ara_debug_trunk(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1,
+                    const float* b1, const float* wd, const float* bd, const float* w2, const float* b2, void* out_half);
 /* the device build of the glibc powf / logf restatement the search uses for apply_temperature (util/blazeutil.h:78-88)
  * and the Dirichlet gamma sampler (:113-124): pow_out[i] = powf(x[i], y[i]), log_out[i] = logf(x[i]); host buffers,
  * either output may be NULL.  tests/test_glibc_flt32.py compares it with the host libm bit for bit. */
