@@ -1,7 +1,5 @@
 #include "abi_common.h"
 
-#include <cstdlib>
-
 namespace ara {
 
 std::string& last_error_ref() {
@@ -27,15 +25,7 @@ PdlSuspend::~PdlSuspend() {
     if (on_) --g_pdl_suspended;
 }
 
-bool pdl_enabled() {
-    if (g_pdl_suspended > 0) return false;
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("ARA_NO_PDL");
-        v = (e != nullptr && e[0] == '1') ? 0 : 1;
-    }
-    return v == 1;
-}
+bool pdl_enabled() { return g_pdl_suspended == 0; }
 
 }  // namespace ara
 

@@ -1,9 +1,10 @@
-// Shared host-side plumbing for the C-ABI: last-error string, CUDA error checks.
+// Shared host-side plumbing for the C-ABI: last-error string, CUDA error checks, device buffers, graph capture.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>
 #include <cstdio>
 #include <string>
+#include <vector>
 
 namespace ara {
 
@@ -17,8 +18,48 @@ int set_error(const char* fmt, ...);
             return ::ara::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
     } while (0)
 
+// Owner of device buffers: every allocation is zero-filled and recorded, and all of them are freed with the owner, on
+// every return path.
+class DeviceBuffers {
+   public:
+    DeviceBuffers() = default;
+    ~DeviceBuffers() {
+        for (void* p : ptrs_) cudaFree(p);
+    }
+    DeviceBuffers(const DeviceBuffers&) = delete;
+    DeviceBuffers& operator=(const DeviceBuffers&) = delete;
+    template <typename T>
+    int dalloc(T** p, size_t count) {
+        void* q = nullptr;
+        ARA_CUDA_OK(cudaMalloc(&q, count * sizeof(T)));
+        ptrs_.push_back(q);
+        ARA_CUDA_OK(cudaMemset(q, 0, count * sizeof(T)));
+        *p = static_cast<T*>(q);
+        return 0;
+    }
+
+   private:
+    std::vector<void*> ptrs_;
+};
+
+// Captures the work enqueue() (0 or -1 with the error set) puts on stream s into *exec.
+template <typename F>
+int capture_graph(cudaStream_t s, cudaGraphExec_t* exec, F&& enqueue) {
+    cudaGraph_t g;
+    ARA_CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    const int rc = enqueue();
+    const cudaError_t e = cudaStreamEndCapture(s, &g);
+    if (e == cudaSuccess && rc != 0) cudaGraphDestroy(g);
+    if (rc) return -1;
+    ARA_CUDA_OK(e);
+    const cudaError_t ie = cudaGraphInstantiate(exec, g, 0);
+    cudaGraphDestroy(g);
+    ARA_CUDA_OK(ie);
+    return 0;
+}
+
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor in the stream is
-// still draining; kernels call pdl_wait() before touching the predecessor's outputs.  ARA_NO_PDL=1 disables it.
+// still draining; kernels call pdl_wait() before touching the predecessor's outputs.
 bool pdl_enabled();
 // While one lives on the calling thread, launch_pdl launches (and captures) plain kernels.  A search with Threads = 2 runs
 // the network on a second stream beside the tree kernels; thread blocks of early-launched network kernels parked at

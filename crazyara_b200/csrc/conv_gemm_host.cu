@@ -1,7 +1,6 @@
 // Host side of the wgmma convolution GEMM: TMA tensor-map construction and launch.
 #include "conv_gemm_host.h"
 
-#include <cstdlib>
 #include <cstring>
 
 namespace ara {
@@ -54,11 +53,6 @@ int make_weight_tensor_map(CUtensorMap* m, const __half* w, int k_total, int row
 }
 
 int conv_layer_choose_bn(int boards, int n_out) {
-    const char* env = getenv("ARA_FORCE_BN");
-    if (env != nullptr) {
-        int v = atoi(env);
-        if (v == 64 || v == 128 || v == 256) return v;
-    }
     const int m_tiles = (boards + 1) / 2;
     const int cands[3] = {256, 128, 64};
     for (int i = 0; i < 3; ++i) {
@@ -70,11 +64,14 @@ int conv_layer_choose_bn(int boards, int n_out) {
     return 64;
 }
 
+template <int BN>
+static cudaError_t allow_smem() {
+    return cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvGemmCfg<BN>::kSmemBytes);
+}
+
 int conv_layer_init(ConvLayer* L, const __half* act, int boards_cap, int cin, const __half* w, int w_rows,
                     int n_out, int ksize, const float* bias, int relu, const __half* residual, int ldr,
                     __half* out_h, float* out_f, int ldo, int bn) {
-    PFN_encodeTiled enc = get_encode_fn();
-    if (enc == nullptr) return set_error("cuTensorMapEncodeTiled entry point not available");
     if (cin % 8 != 0) return set_error("conv_layer_init: cin=%d must be a multiple of 8", cin);
     if (ldo % 32 != 0) return set_error("conv_layer_init: ldo=%d must be a multiple of 32", ldo);
     if (boards_cap < 2 || (boards_cap & 1)) return set_error("conv_layer_init: boards_cap=%d must be even >= 2", boards_cap);
@@ -85,26 +82,8 @@ int conv_layer_init(ConvLayer* L, const __half* act, int boards_cap, int cin, co
     const int c_chunks = (cin + 63) / 64;
     const int cw = c_chunks * 64;
     const int taps = ksize * ksize;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)cin, 8, 8, (cuuint64_t)boards_cap};
-        cuuint64_t strides[3] = {(cuuint64_t)cin * 2, (cuuint64_t)cin * 16, (cuuint64_t)cin * 128};
-        cuuint32_t box[4] = {64, 8, 8, 2};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&L->tm_a, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(act), dims, strides, box,
-                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error("cuTensorMapEncodeTiled(A) failed: %d (cin=%d boards=%d)", (int)r, cin, boards_cap);
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)taps * cw, (cuuint64_t)w_rows};
-        cuuint64_t strides[1] = {(cuuint64_t)taps * cw * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)bn};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&L->tm_b, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(w), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return set_error("cuTensorMapEncodeTiled(B) failed: %d", (int)r);
-    }
+    if (make_act_tensor_map(&L->tm_a, act, boards_cap, cin) || make_weight_tensor_map(&L->tm_b, w, taps * cw, w_rows, bn)) return -1;
+    ARA_CUDA_OK(bn == 64 ? allow_smem<64>() : bn == 128 ? allow_smem<128>() : allow_smem<256>());
     L->bn = bn;
     L->n_out = n_out;
     L->args.M = 0;
@@ -131,14 +110,7 @@ void conv_layer_set_precise(ConvLayer* L, const float* residual_f, int ldr, __ha
 
 template <int BN>
 static int launch_bn(const ConvLayer* L, const ConvGemmArgs& a, dim3 grid, cudaStream_t stream) {
-    using Cfg = ConvGemmCfg<BN>;
-    static bool attr_done = false;
-    if (!attr_done) {
-        ARA_CUDA_OK(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes));
-        attr_done = true;
-    }
-    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN>, grid, dim3(kGemmThreads), Cfg::kSmemBytes, stream, L->tm_a, L->tm_b, a));
+    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN>, grid, dim3(kGemmThreads), ConvGemmCfg<BN>::kSmemBytes, stream, L->tm_a, L->tm_b, a));
     return 0;
 }
 

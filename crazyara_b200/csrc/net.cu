@@ -2,7 +2,6 @@
 #include "net.h"
 
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <memory>
 
@@ -35,18 +34,8 @@ inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 }  // namespace
 
-template <typename T>
-int Net::dalloc(T** p, size_t count) {
-    void* q = nullptr;
-    ARA_CUDA_OK(cudaMalloc(&q, count * sizeof(T)));
-    ARA_CUDA_OK(cudaMemset(q, 0, count * sizeof(T)));
-    allocs_.push_back(q);
-    *p = static_cast<T*>(q);
-    return 0;
-}
-
 int Net::upload_f32(const float* src, size_t count, size_t padded, float** dst) {
-    if (dalloc(dst, padded) != 0) return -1;
+    if (mem_.dalloc(dst, padded) != 0) return -1;
     ARA_CUDA_OK(cudaMemcpy(*dst, src, count * 4, cudaMemcpyHostToDevice));
     return 0;
 }
@@ -61,7 +50,7 @@ int Net::upload_conv_w(const float* w, int n_out, int cin, int ksize, __half** d
         for (int c = 0; c < cin; ++c)
             for (int t = 0; t < taps; ++t)
                 h[(static_cast<size_t>(n) * taps + t) * cw + c] = __float2half_rn(w[(static_cast<size_t>(n) * cin + c) * taps + t]);
-    if (dalloc(dst, h.size()) != 0) return -1;
+    if (mem_.dalloc(dst, h.size()) != 0) return -1;
     ARA_CUDA_OK(cudaMemcpy(*dst, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
     *rows = r;
     return 0;
@@ -85,7 +74,7 @@ int Net::upload_conv_w_split(const float* w, int n_out, int cin, int ksize, __ha
                 col[cw + c] = lo;
                 col[2 * cw + c] = hi;
             }
-    if (dalloc(dst, h.size()) != 0) return -1;
+    if (mem_.dalloc(dst, h.size()) != 0) return -1;
     ARA_CUDA_OK(cudaMemcpy(*dst, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
     *rows = r;
     return 0;
@@ -93,10 +82,8 @@ int Net::upload_conv_w_split(const float* w, int n_out, int cin, int ksize, __ha
 
 Net::~Net() {
     cudaSetDevice(device);
-    for (int k = 0; k < 4; ++k)
-        for (auto& g : graphs_[k]) cudaGraphExecDestroy(g.second);
-    for (void* p : allocs_) cudaFree(p);
-    rise_trunk_destroy(&trunk_);
+    for (auto& family : graphs_)
+        for (auto& g : family) cudaGraphExecDestroy(g.second);
     if (stream) cudaStreamDestroy(stream);
     if (head_stream) cudaStreamDestroy(head_stream);
     if (ev_fork) cudaEventDestroy(ev_fork);
@@ -210,8 +197,8 @@ int Net::build_half(const HostWeights& hw) {
     const int C = hdr.channels;
     const size_t rows = static_cast<size_t>(batch_cap) * 64;
     if (hdr.n_blocks > kTrunkMaxBlocks) return set_error("ara_net_create: %d blocks (max %d)", hdr.n_blocks, kTrunkMaxBlocks);
-    if (dalloc(&d_in_h, rows * cin_pad)) return -1;
-    if (dalloc(&d_x[0], rows * C) || dalloc(&d_x[1], rows * C) || dalloc(&d_p1, rows * C)) return -1;
+    if (mem_.dalloc(&d_in_h, rows * cin_pad)) return -1;
+    if (mem_.dalloc(&d_x[0], rows * C) || mem_.dalloc(&d_x[1], rows * C) || mem_.dalloc(&d_p1, rows * C)) return -1;
     int wrows = 0;
     if (upload_conv_w(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
     if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
@@ -219,7 +206,6 @@ int Net::build_half(const HostWeights& hw) {
                         conv_layer_choose_bn(batch, C)))
         return -1;
     std::vector<TrunkBlockHost> tb(hdr.n_blocks);
-    std::vector<float> ta, tbv;
     for (int i = 0; i < hdr.n_blocks; ++i) {
         const BlockDesc& bd = blocks[i];
         const HostBlock& hb = hw.blocks[i];
@@ -231,19 +217,11 @@ int Net::build_half(const HostWeights& hw) {
         tb[i].wd = hb.wd;
         tb[i].bd = hb.bd;
         tb[i].w2 = hb.w2;
-        float *b2 = nullptr, *sa = nullptr, *sb = nullptr;
-        if (upload_f32(hb.b2.data(), C, 256, &b2)) return -1;
-        tb[i].b2 = b2;
-        if (bd.se_type != 0) {
-            se_transposed(bd, hb, &ta, &tbv);
-            if (upload_f32(ta.data(), ta.size(), ta.size(), &sa) || upload_f32(tbv.data(), tbv.size(), tbv.size(), &sb)) return -1;
-            tb[i].se_w1t = sa;
-            if (bd.se_type == 1) tb[i].se_w2t = sb;
-            else tb[i].se_b = sb;
-        }
+        tb[i].b2 = hb.b2;
+        se_transposed(bd, hb, &tb[i].se_w1t, bd.se_type == 1 ? &tb[i].se_w2t : &tb[i].se_b);
     }
     __half* xfinal = d_x[1];
-    if (rise_trunk_init(&trunk_, tb, d_x[0], batch_cap, xfinal)) return -1;
+    if (rise_trunk_init(&trunk_, tb, d_x[0], xfinal)) return -1;
     if (upload_conv_w(hw.pol_w1.data(), C, C, 3, &pol_w1, &wrows)) return -1;
     if (upload_f32(hw.pol_b1.data(), C, 256, &pol_b1)) return -1;
     if (conv_layer_init(&pol_conv1, xfinal, batch_cap, C, pol_w1, wrows, C, 3, pol_b1, 1, nullptr, 0, d_p1, nullptr, C,
@@ -262,10 +240,10 @@ int Net::build_precise(const HostWeights& hw) {
     const int C = hdr.channels;
     const size_t rows = static_cast<size_t>(batch_cap) * 64;
     const int max_cp = round_up(max_cop_, 64);
-    if (dalloc(&d_in_h, rows * 3 * cin_pad)) return -1;
+    if (mem_.dalloc(&d_in_h, rows * 3 * cin_pad)) return -1;
     for (int k = 0; k < 2; ++k)
-        if (dalloc(&d_xf[k], rows * C) || dalloc(&d_xs[k], rows * 3 * C)) return -1;
-    if (dalloc(&d_h1f, rows * max_cop_) || dalloc(&d_h2s, rows * 3 * max_cp) || dalloc(&d_p1, rows * 3 * C)) return -1;
+        if (mem_.dalloc(&d_xf[k], rows * C) || mem_.dalloc(&d_xs[k], rows * 3 * C)) return -1;
+    if (mem_.dalloc(&d_h1f, rows * max_cop_) || mem_.dalloc(&d_h2s, rows * 3 * max_cp) || mem_.dalloc(&d_p1, rows * 3 * C)) return -1;
     int wrows = 0;
     if (upload_conv_w_split(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
     if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
@@ -345,20 +323,17 @@ int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
     ARA_CUDA_OK(cudaStreamCreateWithFlags(&head_stream, cudaStreamNonBlocking));
     ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
     ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-    if (const char* e = getenv("ARA_NET_FORK_HEADS")) fork_heads = atoi(e) != 0;
-    const char* g = getenv("ARA_NO_GRAPH");
-    use_graph = !(g != nullptr && g[0] == '1');
 
     HostWeights hw;
     if (read_blob(blob_path, &hw)) return -1;
     cin_pad = round_up(hdr.in_channels, 64);
     ldp = round_up(hdr.policy_channels, 32);
     const size_t rows = static_cast<size_t>(batch_cap) * 64;
-    if (dalloc(&d_in_f32, static_cast<size_t>(batch) * hdr.in_channels * 64)) return -1;
-    if (dalloc(&d_logits, rows * ldp)) return -1;
-    if (dalloc(&d_prob, static_cast<size_t>(batch) * n_labels())) return -1;
-    if (dalloc(&d_value, batch)) return -1;
-    if (dalloc(&d_aux, static_cast<size_t>(batch) * 4)) return -1;
+    if (mem_.dalloc(&d_in_f32, static_cast<size_t>(batch) * hdr.in_channels * 64)) return -1;
+    if (mem_.dalloc(&d_logits, rows * ldp)) return -1;
+    if (mem_.dalloc(&d_prob, static_cast<size_t>(batch) * n_labels())) return -1;
+    if (mem_.dalloc(&d_value, batch)) return -1;
+    if (mem_.dalloc(&d_aux, static_cast<size_t>(batch) * 4)) return -1;
     if (upload_value_head(hw)) return -1;
     if (precision == 0 ? build_half(hw) : build_precise(hw)) return -1;
     io_in_h[0] = d_in_h, io_prob[0] = d_prob, io_value[0] = d_value, io_aux[0] = d_aux;
@@ -377,13 +352,13 @@ int Net::enable_second_io() {
     ARA_CUDA_OK(cudaSetDevice(device));
     const size_t rows = static_cast<size_t>(batch_cap) * 64;
     const int cin = precision == 0 ? cin_pad : 3 * cin_pad;
-    if (dalloc(&io_in_h[1], rows * cin)) return -1;
-    if (dalloc(&io_prob[1], static_cast<size_t>(batch) * n_labels())) return -1;
-    if (dalloc(&io_value[1], batch) || dalloc(&io_aux[1], static_cast<size_t>(batch) * 4)) return -1;
+    if (mem_.dalloc(&io_in_h[1], rows * cin)) return -1;
+    if (mem_.dalloc(&io_prob[1], static_cast<size_t>(batch) * n_labels())) return -1;
+    if (mem_.dalloc(&io_value[1], batch) || mem_.dalloc(&io_aux[1], static_cast<size_t>(batch) * 4)) return -1;
     stem_conv2 = stem_conv;  // same weights and epilogue; the activation map differs ...
     if (make_act_tensor_map(&stem_conv2.tm_a, io_in_h[1], batch_cap, cin)) return -1;
     if (precision == 0) {  // ... and the output buffer: the two sets' stems may then run while the other set's tower reads its own
-        if (dalloc(&d_x0_alt, rows * static_cast<size_t>(hdr.channels))) return -1;
+        if (mem_.dalloc(&d_x0_alt, rows * static_cast<size_t>(hdr.channels))) return -1;
         stem_conv2.args.out_h = d_x0_alt;
     }
     return 0;
@@ -452,18 +427,15 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
     ++launches;
     __half* xfinal = d_x[1];
     ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
-    if (fork_heads) {  // value head on the side stream (a second branch of the captured graph), policy head on s
-        ARA_CUDA_OK(cudaEventRecord(ev_fork, s));
-        ARA_CUDA_OK(cudaStreamWaitEvent(head_stream, ev_fork, 0));
-        value_head_kernel<__half><<<dim3(n), dim3(256), value_head_smem<__half>(), head_stream>>>(xfinal, vw, io_value[io], io_aux[io], cnt);
-        ARA_CUDA_OK(cudaEventRecord(ev_join, head_stream));
-    } else {
-        ARA_CUDA_OK(launch_pdl(value_head_kernel<__half>, dim3(n), dim3(256), value_head_smem<__half>(), s, xfinal, vw, io_value[io], io_aux[io], cnt));
-    }
+    // value head on the side stream (a second branch of the captured graph), policy head on s
+    ARA_CUDA_OK(cudaEventRecord(ev_fork, s));
+    ARA_CUDA_OK(cudaStreamWaitEvent(head_stream, ev_fork, 0));
+    value_head_kernel<__half><<<dim3(n), dim3(256), value_head_smem<__half>(), head_stream>>>(xfinal, vw, io_value[io], io_aux[io], cnt);
+    ARA_CUDA_OK(cudaEventRecord(ev_join, head_stream));
     if (conv_layer_launch(&pol_conv1, n, s, cnt)) return -1;
     if (conv_layer_launch(&pol_conv2, n, s, cnt)) return -1;
     ARA_CUDA_OK(launch_pdl(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt));
-    if (fork_heads) ARA_CUDA_OK(cudaStreamWaitEvent(s, ev_join, 0));
+    ARA_CUDA_OK(cudaStreamWaitEvent(s, ev_join, 0));
     launches += 4;
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
@@ -476,7 +448,6 @@ int Net::forward_device(int n, cudaStream_t s, const int* cnt, int io, bool stem
     // two input / output sets = a search with Threads = 2: this forward runs on the network stream beside the other
     // thread's tree kernels (see PdlSuspend)
     PdlSuspend no_pdl(io_in_h[1] != nullptr && (precision != 0 || !stem_done));  // (not split: everything plain, as before)
-    if (!use_graph) return enqueue(n, s, false, cnt, io, stem_done);
     {   // inside somebody else's capture (the search's iteration graph) the kernels go in directly
         cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
         ARA_CUDA_OK(cudaStreamIsCapturing(s, &cs));
@@ -489,52 +460,31 @@ int Net::forward_device(int n, cudaStream_t s, const int* cnt, int io, bool stem
         graphs_[gk].clear();
         baked = cnt;
     }
-    auto& graphs = graphs_[gk];
-    auto it = graphs.find(n);
-    if (it == graphs.end()) {
-        // warm-up launch outside capture (sets function attributes), then capture
-        if (enqueue(n, s, false, cnt, io, stem_done)) return -1;
-        ARA_CUDA_OK(cudaStreamSynchronize(s));
-        const long long before = launches;
-        cudaGraph_t g;
-        ARA_CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue(n, s, false, cnt, io, stem_done);
-        cudaError_t e = cudaStreamEndCapture(s, &g);
-        launches = before;
-        if (rc) return -1;
-        ARA_CUDA_OK(e);
-        cudaGraphExec_t ge;
-        ARA_CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
-        cudaGraphDestroy(g);
-        it = graphs.emplace(n, ge).first;
-    }
-    ARA_CUDA_OK(cudaGraphLaunch(it->second, s));
-    launches += kernels_per_forward(false) - (stem_done ? 1 : 0);
-    return 0;
+    return launch_graph(gk, n, s, false, cnt, io, stem_done);
 }
 
 int Net::forward_from_f32_device(int n, cudaStream_t s) {
     if (n < 1 || n > batch) return set_error("forward: n=%d outside [1,%d]", n, batch);
-    if (!use_graph) return enqueue(n, s, true);
-    auto it = graphs_[1].find(n);
-    if (it == graphs_[1].end()) {
-        if (enqueue(n, s, true)) return -1;
+    return launch_graph(1, n, s, true, nullptr, 0, false);
+}
+
+// The forward as one launch of graph family `family`'s graph for n boards.  The first forward of a size runs eagerly as a
+// warm-up and is then captured; the launches of the capture are not counted.
+int Net::launch_graph(int family, int n, cudaStream_t s, bool from_f32, const int* cnt, int io, bool stem_done) {
+    auto& graphs = graphs_[family];
+    auto it = graphs.find(n);
+    if (it == graphs.end()) {
+        if (enqueue(n, s, from_f32, cnt, io, stem_done)) return -1;
         ARA_CUDA_OK(cudaStreamSynchronize(s));
         const long long before = launches;
-        cudaGraph_t g;
-        ARA_CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue(n, s, true);
-        cudaError_t e = cudaStreamEndCapture(s, &g);
+        cudaGraphExec_t ge;
+        const int rc = capture_graph(s, &ge, [&] { return enqueue(n, s, from_f32, cnt, io, stem_done); });
         launches = before;
         if (rc) return -1;
-        ARA_CUDA_OK(e);
-        cudaGraphExec_t ge;
-        ARA_CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
-        cudaGraphDestroy(g);
-        it = graphs_[1].emplace(n, ge).first;
+        it = graphs.emplace(n, ge).first;
     }
     ARA_CUDA_OK(cudaGraphLaunch(it->second, s));
-    launches += kernels_per_forward(true);
+    launches += kernels_per_forward(from_f32) - (stem_done ? 1 : 0);
     return 0;
 }
 
@@ -581,8 +531,8 @@ int Net::predict_priors(const float* planes_host, int n, const int* policy_idx, 
     if (!planes_host || !value_host || !policy_idx || !counts || !priors_host || stride < 1 || stride > 512)
         return set_error("ara_net_predict_priors: bad arguments");
     if (stride > gather_stride) {
-        if (dalloc(&d_gather_idx, static_cast<size_t>(batch) * stride) || dalloc(&d_gather_out, static_cast<size_t>(batch) * stride)) return -1;
-        if (d_gather_cnt == nullptr && dalloc(&d_gather_cnt, batch)) return -1;
+        if (mem_.dalloc(&d_gather_idx, static_cast<size_t>(batch) * stride) || mem_.dalloc(&d_gather_out, static_cast<size_t>(batch) * stride)) return -1;
+        if (d_gather_cnt == nullptr && mem_.dalloc(&d_gather_cnt, batch)) return -1;
         gather_stride = stride;
     }
     ARA_CUDA_OK(cudaMemcpyAsync(d_in_f32, planes_host, static_cast<size_t>(n) * hdr.in_channels * 64 * 4, cudaMemcpyHostToDevice, stream));

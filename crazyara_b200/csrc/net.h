@@ -92,7 +92,6 @@ class Net {
     // the value head runs beside the policy head: forked side stream, joined before the forward ends
     cudaStream_t head_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    bool fork_heads = true;  // ARA_NET_FORK_HEADS=0: both heads in sequence on one stream
 
     // device buffers
     float* d_in_f32 = nullptr;   // [batch, C, 64]
@@ -118,7 +117,6 @@ class Net {
     float* d_gather_out = nullptr;
     int gather_stride = 0;
     long long launches = 0;      // kernels launched so far (bench bookkeeping)
-    bool use_graph = true;
 
    private:
     int enqueue(int n, cudaStream_t s, bool from_f32, const int* boards_dev = nullptr, int io = 0, bool stem_done = false);
@@ -127,7 +125,8 @@ class Net {
     int build_precise(const HostWeights& hw);
     int upload_value_head(const HostWeights& hw);
     int enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io);
-    std::vector<void*> allocs_;
+    int launch_graph(int family, int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io, bool stem_done);
+    DeviceBuffers mem_;
     int max_cop_ = 0;
     __half* stem_w = nullptr;
     float* stem_b = nullptr;
@@ -142,8 +141,6 @@ class Net {
     ConvLayer pol_conv1, pol_conv2;
     std::map<int, cudaGraphExec_t> graphs_[6];  // plain, from fp32 input, with a device-side count (io 0), the same for io 1
     const int* baked_[6] = {};                  // the counter pointer each graph family was captured with
-    template <typename T>
-    int dalloc(T** p, size_t count);
     int upload_conv_w(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows);
     int upload_conv_w_split(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows);
     int upload_f32(const float* src, size_t count, size_t padded, float** dst);

@@ -13,10 +13,18 @@ namespace {
 // with the row index modulo 8): the layout TMA's SWIZZLE_128B produces and the wgmma shared-memory descriptor reads
 inline size_t sw128_offset(int row, int k) { return static_cast<size_t>(row) * 128 + ((((k >> 3) ^ (row & 7)) << 4)) + (k & 7) * 2; }
 
+template <typename T>
+int upload(DeviceBuffers& mem, const std::vector<T>& h, const T** dst) {
+    T* d = nullptr;
+    if (mem.dalloc(&d, h.size())) return -1;
+    ARA_CUDA_OK(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *dst = d;
+    return 0;
+}
+
 }  // namespace
 
-int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, const __half* x_in, int boards_cap, __half* out) {
-    (void)boards_cap;
+int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, const __half* x_in, __half* out) {
     const int nb = static_cast<int>(blocks.size());
     if (nb < 1 || nb > kTrunkMaxBlocks) return set_error("rise_trunk_init: %d blocks unsupported (max %d)", nb, kTrunkMaxBlocks);
     memset(&T->args, 0, sizeof(T->args));
@@ -30,21 +38,15 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
         B.ksize = h.ksize;
         B.se_type = h.se_type;
         B.chunk0 = chunks;
-        B.b2 = h.b2;
-        B.se_b = h.se_b;
+        if (upload(T->mem, h.b2, &B.b2)) return -1;
         if (h.se_type != 0) {  // fp16 copies of the squeeze-excitation matrices (the kernel is bound by their traffic)
             const size_t n1 = h.se_type == 1 ? 256 * 128 : 256 * 256, n2 = h.se_type == 1 ? 128 * 256 : 0;
-            std::vector<float> f(n1 + n2);
-            ARA_CUDA_OK(cudaMemcpy(f.data(), h.se_w1t, n1 * 4, cudaMemcpyDeviceToHost));
-            if (n2) ARA_CUDA_OK(cudaMemcpy(f.data() + n1, h.se_w2t, n2 * 4, cudaMemcpyDeviceToHost));
+            if (h.se_type == 2 && upload(T->mem, h.se_b, &B.se_b)) return -1;
             std::vector<__half> hh(n1 + n2);
-            for (size_t k = 0; k < hh.size(); ++k) hh[k] = __float2half_rn(f[k]);
-            void* d = nullptr;
-            ARA_CUDA_OK(cudaMalloc(&d, hh.size() * sizeof(__half)));
-            ARA_CUDA_OK(cudaMemcpy(d, hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice));
-            T->d_se.push_back(d);
-            B.se_w1t = static_cast<const __half*>(d);
-            B.se_w2t = n2 ? static_cast<const __half*>(d) + n1 : nullptr;
+            for (size_t k = 0; k < n1; ++k) hh[k] = __float2half_rn(h.se_w1t[k]);
+            for (size_t k = 0; k < n2; ++k) hh[n1 + k] = __float2half_rn(h.se_w2t[k]);
+            if (upload(T->mem, hh, &B.se_w1t)) return -1;
+            B.se_w2t = n2 ? B.se_w1t + n1 : nullptr;
             // the pair kernel's images: each CTA gets the columns of the outputs it computes
             std::vector<__half> img(2 * kTrunkSeImage / sizeof(__half));
             for (int r = 0; r < 2; ++r) {
@@ -59,10 +61,9 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
                         for (int i = 0; i < 128; ++i) o[k * 128 + i] = hh[k * 256 + 128 * r + i];
                 }
             }
-            ARA_CUDA_OK(cudaMalloc(&d, img.size() * sizeof(__half)));
-            ARA_CUDA_OK(cudaMemcpy(d, img.data(), img.size() * sizeof(__half), cudaMemcpyHostToDevice));
-            T->d_se.push_back(d);
-            B.se_img = static_cast<const uint8_t*>(d);
+            const __half* d_img = nullptr;
+            if (upload(T->mem, img, &d_img)) return -1;
+            B.se_img = reinterpret_cast<const uint8_t*>(d_img);
         }
         chunks += B.n_chunks;
     }
@@ -97,15 +98,9 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
             }
         }
     }
-    ARA_CUDA_OK(cudaMalloc(&T->d_w1, w1.size()));
-    ARA_CUDA_OK(cudaMalloc(&T->d_w2, w2.size()));
-    ARA_CUDA_OK(cudaMemcpy(T->d_w1, w1.data(), w1.size(), cudaMemcpyHostToDevice));
-    ARA_CUDA_OK(cudaMemcpy(T->d_w2, w2.data(), w2.size(), cudaMemcpyHostToDevice));
-    T->args.w1_img = static_cast<const uint8_t*>(T->d_w1);
-    T->args.w2_img = static_cast<const uint8_t*>(T->d_w2);
-    ARA_CUDA_OK(cudaMalloc(&T->d_prof, 32 * sizeof(unsigned long long)));
-    ARA_CUDA_OK(cudaMemset(T->d_prof, 0, 32 * sizeof(unsigned long long)));
-    T->args.prof = static_cast<unsigned long long*>(T->d_prof);
+    if (upload(T->mem, w1, &T->args.w1_img) || upload(T->mem, w2, &T->args.w2_img)) return -1;
+    if (T->mem.dalloc(&T->d_prof, 32)) return -1;
+    T->args.prof = T->d_prof;
     ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<1>::kSmemBytes));
     ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<2>::kSmemBytes));
     ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RtPairCfg::kSmemBytes));
@@ -152,22 +147,12 @@ int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const
     return 0;
 }
 
-void rise_trunk_destroy(RiseTrunk* T) {
-    if (T->d_w1) cudaFree(T->d_w1);
-    if (T->d_w2) cudaFree(T->d_w2);
-    if (T->d_prof) cudaFree(T->d_prof);
-    for (void* p : T->d_se) cudaFree(p);
-    T->d_se.clear();
-    T->d_w1 = T->d_w2 = T->d_prof = nullptr;
-}
-
 namespace {
 
 int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1, const float* b1,
-                    const float* wd, const float* bd, const float* w2, const float* b2, __half* out_h, RiseTrunk* T,
-                    std::vector<void*>& dev) {
+                    const float* wd, const float* bd, const float* w2, const float* b2, __half* out_h) {
     if (n < 1 || n_blocks < 1 || n_blocks > kTrunkMaxBlocks) return set_error("ara_debug_trunk: %d boards, %d blocks", n, n_blocks);
-    const size_t x_bytes = static_cast<size_t>(n) * 64 * 256 * sizeof(__half);
+    const size_t x_count = static_cast<size_t>(n) * 64 * 256;
     std::vector<TrunkBlockHost> blocks(n_blocks);
     for (int i = 0; i < n_blocks; ++i) {
         TrunkBlockHost& h = blocks[i];
@@ -180,23 +165,18 @@ int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, con
         h.wd.assign(wd, wd + static_cast<size_t>(c) * kk);
         h.bd.assign(bd, bd + c);
         h.w2.assign(w2, w2 + static_cast<size_t>(256) * c);
+        h.b2.assign(b2 + 256 * i, b2 + 256 * (i + 1));
         w1 += static_cast<size_t>(c) * 256, b1 += c, wd += static_cast<size_t>(c) * kk, bd += c, w2 += static_cast<size_t>(256) * c;
-        void* d = nullptr;
-        ARA_CUDA_OK(cudaMalloc(&d, 256 * sizeof(float)));
-        dev.push_back(d);
-        ARA_CUDA_OK(cudaMemcpy(d, b2 + 256 * i, 256 * sizeof(float), cudaMemcpyHostToDevice));
-        h.b2 = static_cast<const float*>(d);
     }
-    void *d_x = nullptr, *d_out = nullptr;
-    ARA_CUDA_OK(cudaMalloc(&d_x, x_bytes));
-    dev.push_back(d_x);
-    ARA_CUDA_OK(cudaMalloc(&d_out, x_bytes));
-    dev.push_back(d_out);
-    ARA_CUDA_OK(cudaMemcpy(d_x, x_h, x_bytes, cudaMemcpyHostToDevice));
-    if (rise_trunk_init(T, blocks, static_cast<const __half*>(d_x), n, static_cast<__half*>(d_out))) return -1;
-    if (rise_trunk_launch(T, n, nullptr)) return -1;
+    DeviceBuffers mem;
+    __half *d_x = nullptr, *d_out = nullptr;
+    if (mem.dalloc(&d_x, x_count) || mem.dalloc(&d_out, x_count)) return -1;
+    ARA_CUDA_OK(cudaMemcpy(d_x, x_h, x_count * sizeof(__half), cudaMemcpyHostToDevice));
+    RiseTrunk T;
+    if (rise_trunk_init(&T, blocks, d_x, d_out)) return -1;
+    if (rise_trunk_launch(&T, n, nullptr)) return -1;
     ARA_CUDA_OK(cudaStreamSynchronize(nullptr));
-    ARA_CUDA_OK(cudaMemcpy(out_h, d_out, x_bytes, cudaMemcpyDeviceToHost));
+    ARA_CUDA_OK(cudaMemcpy(out_h, d_out, x_count * sizeof(__half), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -209,11 +189,6 @@ int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, con
 // squeeze-excitation) one block after the other in the layouts of TrunkBlockHost; b2 [n_blocks][256].
 extern "C" int ara_debug_trunk(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1,
                                const float* b1, const float* wd, const float* bd, const float* w2, const float* b2, void* out_half) {
-    ara::RiseTrunk T;
-    std::vector<void*> dev;
-    const int rc = ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2,
-                                        static_cast<__half*>(out_half), &T, dev);
-    ara::rise_trunk_destroy(&T);
-    for (void* p : dev) cudaFree(p);
-    return rc;
+    return ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2,
+                                static_cast<__half*>(out_half));
 }

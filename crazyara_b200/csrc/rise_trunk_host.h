@@ -17,27 +17,24 @@ struct TrunkBlockHost {
     std::vector<float> wd;  // [c_op][k*k]   depthwise (BN folded)
     std::vector<float> bd;  // [c_op]
     std::vector<float> w2;  // [256][c_op]   conv1x1 c_op -> 256 (BN folded)
-    const float* b2 = nullptr;      // device [256]
-    const float* se_w1t = nullptr;  // device, see TrunkBlock
-    const float* se_w2t = nullptr;
-    const float* se_b = nullptr;
+    std::vector<float> b2;  // [256]
+    std::vector<float> se_w1t;  // transposed squeeze-excitation, see TrunkBlock: ca_se [256][128], eca_se [256][256]
+    std::vector<float> se_w2t;  // ca_se: [128][256]
+    std::vector<float> se_b;    // eca_se: [256]
 };
 
 struct RiseTrunk {
     TrunkArgs args;
-    void* d_w1 = nullptr;
-    void* d_w2 = nullptr;
     int sm_count = 0;
     int pair_clusters = 0;  // CTA pairs of rise_trunk_pair_kernel resident at once
-    void* d_prof = nullptr;  // [2][16] cycle counters, written only by -DARA_TRUNK_PROF builds
-    std::vector<void*> d_se;  // fp16 copies of the squeeze-excitation matrices
+    unsigned long long* d_prof = nullptr;  // [2][16] cycle counters, written only by -DARA_TRUNK_PROF builds
+    DeviceBuffers mem;  // everything the pointers in args and d_prof point to
 };
 
-// x_in: [boards_cap, 8, 8, 256] fp16 (stem output); out: [boards*64, 256] fp16 (may alias x_in: every CTA reads its
+// x_in: [boards, 8, 8, 256] fp16 (stem output); out: [boards*64, 256] fp16 (may alias x_in: every CTA reads its
 // own rows before it writes them)
-int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, const __half* x_in, int boards_cap, __half* out);
+int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, const __half* x_in, __half* out);
 // x_in (optional): another stem-output buffer than the one given to rise_trunk_init (a second input / output set)
 int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const int* boards_dev = nullptr, const __half* x_in = nullptr);
-void rise_trunk_destroy(RiseTrunk* T);
 
 }  // namespace ara

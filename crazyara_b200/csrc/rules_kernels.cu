@@ -100,16 +100,13 @@ extern "C" int ara_encode_planes(const ara_board_t* boards, int n, int mode, int
     const int c = planes_channels(mode, version);
     if (c < 0) return set_error("ara_encode_planes: unsupported mode %d / version %d", mode, version);
     if (n <= 0) return 0;
+    DeviceBuffers mem;
     Board* d_b = nullptr;
     float* d_o = nullptr;
-    ARA_CUDA_OK(cudaMalloc(&d_b, sizeof(Board) * n));
-    ARA_CUDA_OK(cudaMalloc(&d_o, sizeof(float) * n * c * 64));
+    if (mem.dalloc(&d_b, n) || mem.dalloc(&d_o, static_cast<size_t>(n) * c * 64)) return -1;
     ARA_CUDA_OK(cudaMemcpy(d_b, boards, sizeof(Board) * n, cudaMemcpyHostToDevice));
     encode_planes_f32_kernel<<<(n + kWarpsPerBlock - 1) / kWarpsPerBlock, 32 * kWarpsPerBlock>>>(d_b, n, mode, version, normalize, d_o, c);
-    cudaError_t e = cudaMemcpy(planes_out, d_o, sizeof(float) * n * c * 64, cudaMemcpyDeviceToHost);
-    cudaFree(d_b);
-    cudaFree(d_o);
-    if (e != cudaSuccess) return set_error("ara_encode_planes: %s", cudaGetErrorString(e));
+    ARA_CUDA_OK(cudaMemcpy(planes_out, d_o, sizeof(float) * n * c * 64, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -132,25 +129,18 @@ extern "C" int ara_legal_moves(const ara_board_t* boards, int n, unsigned short*
                                int* policy_idx) {
     if (check_device()) return -1;
     if (n <= 0) return 0;
+    DeviceBuffers mem;
     Board* d_b = nullptr;
     Move* d_m = nullptr;
     int *d_c = nullptr, *d_t = nullptr, *d_p = nullptr;
-    ARA_CUDA_OK(cudaMalloc(&d_b, sizeof(Board) * n));
-    ARA_CUDA_OK(cudaMalloc(&d_m, sizeof(Move) * n * kMaxMoves));
-    ARA_CUDA_OK(cudaMalloc(&d_c, sizeof(int) * n));
-    ARA_CUDA_OK(cudaMalloc(&d_t, sizeof(int) * n));
-    ARA_CUDA_OK(cudaMalloc(&d_p, sizeof(int) * n * kMaxMoves));
+    if (mem.dalloc(&d_b, n) || mem.dalloc(&d_m, static_cast<size_t>(n) * kMaxMoves) || mem.dalloc(&d_c, n) || mem.dalloc(&d_t, n) ||
+        mem.dalloc(&d_p, static_cast<size_t>(n) * kMaxMoves))
+        return -1;
     ARA_CUDA_OK(cudaMemcpy(d_b, boards, sizeof(Board) * n, cudaMemcpyHostToDevice));
     legal_moves_kernel<<<(n + kWarpsPerBlock - 1) / kWarpsPerBlock, 32 * kWarpsPerBlock>>>(d_b, n, d_m, d_c, d_t, d_p);
-    cudaError_t e = cudaMemcpy(moves_out, d_m, sizeof(Move) * n * kMaxMoves, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(counts, d_c, sizeof(int) * n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && terminal) e = cudaMemcpy(terminal, d_t, sizeof(int) * n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && policy_idx) e = cudaMemcpy(policy_idx, d_p, sizeof(int) * n * kMaxMoves, cudaMemcpyDeviceToHost);
-    cudaFree(d_b);
-    cudaFree(d_m);
-    cudaFree(d_c);
-    cudaFree(d_t);
-    cudaFree(d_p);
-    if (e != cudaSuccess) return set_error("ara_legal_moves: %s", cudaGetErrorString(e));
+    ARA_CUDA_OK(cudaMemcpy(moves_out, d_m, sizeof(Move) * n * kMaxMoves, cudaMemcpyDeviceToHost));
+    ARA_CUDA_OK(cudaMemcpy(counts, d_c, sizeof(int) * n, cudaMemcpyDeviceToHost));
+    if (terminal) ARA_CUDA_OK(cudaMemcpy(terminal, d_t, sizeof(int) * n, cudaMemcpyDeviceToHost));
+    if (policy_idx) ARA_CUDA_OK(cudaMemcpy(policy_idx, d_p, sizeof(int) * n * kMaxMoves, cudaMemcpyDeviceToHost));
     return 0;
 }

@@ -263,14 +263,11 @@ __global__ void __launch_bounds__(32) prepare_kernel(const TreeDev* trees, Searc
     prepare_item(t, sp, ws, item);
 }
 
-// scatter and prepare in one launch (the iterations' path): warp `item` < B scatters leaf `item` and goes straight on to
+// scatter and prepare in one warp (the iterations' path): warp `item` < B scatters leaf `item` and goes straight on to
 // prepare that leaf's first child; the other warps prepare the next children of the nodes expanded in the mini-batch,
 // which depend on neither.  Saves a dependent launch per iteration and takes the parents' work off the critical path.
-__global__ void __launch_bounds__(32) scatter_prepare_kernel(const TreeDev* trees, SearchParams sp, int batch, int items,
-                                                             const float* values, const float* probs, int n_labels) {
-    __shared__ WarpScratch ws;
-    const int tree = blockIdx.x / items, item = blockIdx.x - tree * items;
-    const TreeDev t = trees[tree];
+__device__ __forceinline__ void scatter_prepare_item(const TreeDev t, const SearchParams& sp, WarpScratch& ws, int item, int batch,
+                                                     const float* values, const float* probs, int n_labels) {
     if (t.st->error) return;
     if (item < batch) {
         if (item >= t.bs->n_new) return;
@@ -278,6 +275,13 @@ __global__ void __launch_bounds__(32) scatter_prepare_kernel(const TreeDev* tree
         __syncwarp();
     }
     prepare_item(t, sp, ws, item);
+}
+
+__global__ void __launch_bounds__(32) scatter_prepare_kernel(const TreeDev* trees, SearchParams sp, int batch, int items,
+                                                             const float* values, const float* probs, int n_labels) {
+    __shared__ WarpScratch ws;
+    const int tree = blockIdx.x / items, item = blockIdx.x - tree * items;
+    scatter_prepare_item(trees[tree], sp, ws, item, batch, values, probs, n_labels);
 }
 
 // The whole update step of an iteration in ONE launch: the first n_trees warps run the value backups (one per tree, the
@@ -293,14 +297,7 @@ __global__ void __launch_bounds__(32) update_kernel(const TreeDev* trees, Search
     }
     const int blk = static_cast<int>(blockIdx.x) - n_trees;
     const int tree = blk / items, item = blk - tree * items;
-    const TreeDev t = trees[tree];
-    if (t.st->error) return;
-    if (item < batch) {
-        if (item >= t.bs->n_new) return;
-        scatter_pending(t, sp, ws, item, values, probs, n_labels);
-        __syncwarp();
-    }
-    prepare_item(t, sp, ws, item);
+    scatter_prepare_item(trees[tree], sp, ws, item, batch, values, probs, n_labels);
 }
 
 __global__ void __launch_bounds__(32) result_kernel(const TreeDev* trees, SearchParams sp, SearchResult* out) {
@@ -360,8 +357,8 @@ class Search {
     bool use_tc = false;
     ara_time_control_t tc{};
     ara_time_report_t tr{};
-    // one iteration as a CUDA graph (ARA_ITER_GRAPH=0 switches it off)
-    bool use_iter_graph_ = true, iter_warm_ = false;
+    // one iteration as a CUDA graph
+    bool iter_warm_ = false;
     cudaGraphExec_t iter_graph_ = nullptr;
     cudaStream_t side_stream_ = nullptr;  // second branch of an iteration (value backups)
     cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
@@ -382,7 +379,7 @@ class Search {
     }
     bool primed_ = false;                  // S0 S1 of the current go have been enqueued
     TreeDev* d_trees_slot_[2] = {nullptr, nullptr};
-    std::vector<TreeDev> h_trees1_;        // slot 1 views (h_trees_ = slot 0)
+    std::vector<TreeDev> h_trees1_;        // slot 1 views (h_trees_ = slot 0); their batch arrays are slot 1's own
     // node-pool compaction: the second set of pools per tree (allocated at the first compaction), scan scratch
     std::vector<TreeDev> shadow_;
     std::vector<char> advanced_;           // ara_search_apply_move since the last go
@@ -392,13 +389,6 @@ class Search {
     int* d_ctotal_ = nullptr;
     long long compactions = 0;
     int compact_pools();
-    struct SlotArrays {                    // per tree: the batch arrays of slot 1
-        int32_t *exp_parent, *new_node, *traj_node, *traj_len, *traj_start;
-        uint16_t* traj_ci;
-        uint32_t* traj_edge;
-        BatchState* bs;
-    };
-    std::vector<SlotArrays> slot1_;
     int* d_count_slot_[2] = {nullptr, nullptr};
     float *d_values_slot_[2] = {nullptr, nullptr}, *d_probs_slot_[2] = {nullptr, nullptr};  // fake backend, per slot
     cudaStream_t net_stream_ = nullptr;
@@ -421,8 +411,34 @@ class Search {
     long long net_forwards = 0;
 
    private:
-    template <typename T>
-    int dalloc(T** p, size_t count);
+    // The arrays of TreeDev, listed once: f(member, length) for each.  A tree's node, edge and prepared-child pools
+    // (the compaction swaps them for its second set) ...
+    template <typename F>
+    void for_each_pool(F&& f) const {
+        const size_t nodes = max_nodes_, edges = max_edges_, slots = nodes * kPrepSlots;
+        f(&TreeDev::hdr, nodes), f(&TreeDev::board, nodes);
+        f(&TreeDev::P, edges), f(&TreeDev::Q, edges), f(&TreeDev::N, edges), f(&TreeDev::child, edges), f(&TreeDev::cbase, edges);
+        f(&TreeDev::move, edges), f(&TreeDev::vl, edges), f(&TreeDev::etype, edges);
+        f(&TreeDev::prep_board, slots), f(&TreeDev::prep_ci, slots), f(&TreeDev::prep_term, slots);
+    }
+    // ... and the batch arrays of one view of a tree (Threads = 2: each logical thread's view has its own)
+    template <typename F>
+    void for_each_batch_array(F&& f) const {
+        const size_t B = sp.batch_size, traj = 2 * B * kMaxDepth;
+        f(&TreeDev::bs, 1), f(&TreeDev::exp_parent, 3 * B), f(&TreeDev::new_node, B);
+        f(&TreeDev::traj_node, traj), f(&TreeDev::traj_ci, traj), f(&TreeDev::traj_edge, traj);
+        f(&TreeDev::traj_len, 2 * B), f(&TreeDev::traj_start, 2 * B);
+    }
+    int alloc_pools(TreeDev& t) {
+        int rc = 0;
+        for_each_pool([&](auto m, size_t n) { rc = rc ? rc : mem_.dalloc(&(t.*m), n); });
+        return rc;
+    }
+    int alloc_batch_arrays(TreeDev& t) {
+        int rc = 0;
+        for_each_batch_array([&](auto m, size_t n) { rc = rc ? rc : mem_.dalloc(&(t.*m), n); });
+        return rc;
+    }
     int iterate(int count);
     Net* net_ = nullptr;
     bool searched_ = false;  // a go has run: the device holds trees that apply_move may keep
@@ -432,7 +448,7 @@ class Search {
     cudaStream_t stream_ = nullptr;
     bool own_stream_ = false;
     int max_nodes_ = 0, max_edges_ = 0, n_labels_ = 0, hist_cap_ = 512;
-    std::vector<void*> allocs_;
+    DeviceBuffers mem_;
     std::vector<TreeDev> h_trees_;
     TreeDev* d_trees_ = nullptr;
     Board* d_roots_ = nullptr;
@@ -487,24 +503,11 @@ int Search::prof_collect() {  // events come in groups of four: before select, b
     return 0;
 }
 
-template <typename T>
-int Search::dalloc(T** p, size_t count) {
-    void* q = nullptr;
-    ARA_CUDA_OK(cudaMalloc(&q, count * sizeof(T)));
-    ARA_CUDA_OK(cudaMemset(q, 0, count * sizeof(T)));
-    allocs_.push_back(q);
-    *p = static_cast<T*>(q);
-    return 0;
-}
-
 Search::~Search() {
     cudaSetDevice(device_);
     if (stream_) cudaStreamSynchronize(stream_);
-    for (void* p : allocs_) cudaFree(p);
     if (h_done_) cudaFreeHost(h_done_);
     if (h_tstats_) cudaFreeHost(h_tstats_);
-    if (d_tstats_) cudaFree(d_tstats_);
-    if (d_count_) cudaFree(d_count_);
     if (iter_graph_) cudaGraphExecDestroy(iter_graph_);
     for (auto& a : slot_graph_)
         for (auto g : a)
@@ -514,8 +517,6 @@ Search::~Search() {
         if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ev_net_)
         if (e) cudaEventDestroy(e);
-    if (d_count_slot_[1]) cudaFree(d_count_slot_[1]);
-    if (d_node_view_) cudaFree(d_node_view_);
     if (side_stream_) cudaStreamDestroy(side_stream_);
     if (ev_fork_) cudaEventDestroy(ev_fork_);
     if (ev_join_) cudaEventDestroy(ev_join_);
@@ -565,8 +566,8 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     } else {
         ARA_CUDA_OK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
         own_stream_ = true;
-        if (dalloc(&d_values_, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
-        if (dalloc(&d_probs_, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
+        if (mem_.dalloc(&d_values_, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
+        if (mem_.dalloc(&d_probs_, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
     }
     if (max_nodes <= 0) {
         const unsigned budget = sp.simulations ? sp.simulations : (sp.nodes ? sp.nodes * 2 : 0);
@@ -589,12 +590,12 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         if (len > (1 << 22)) len = 1 << 22;
         std::vector<float> lut(len);
         for (int i = 0; i < len; ++i) lut[i] = logf((static_cast<float>(i) + sp.cpuct_base + 1) / sp.cpuct_base) + sp.cpuct_init;
-        if (dalloc(&d_lut_, lut.size())) return -1;
+        if (mem_.dalloc(&d_lut_, lut.size())) return -1;
         ARA_CUDA_OK(cudaMemcpy(d_lut_, lut.data(), lut.size() * 4, cudaMemcpyHostToDevice));
         // sqrt(double(visit_sum)): IEEE-exact on both sides, tabulated only to keep the instruction chain short
         std::vector<double> sq(len);
         for (int i = 0; i < len; ++i) sq[i] = sqrt(static_cast<double>(i));
-        if (dalloc(&d_sqrt_lut_, sq.size())) return -1;
+        if (mem_.dalloc(&d_sqrt_lut_, sq.size())) return -1;
         ARA_CUDA_OK(cudaMemcpy(d_sqrt_lut_, sq.data(), sq.size() * 8, cudaMemcpyHostToDevice));
         h_trees_.resize(n_trees);
         for (auto& t : h_trees_) t.cput_lut_len = len;
@@ -604,21 +605,8 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     d_hist_reps_.resize(n_trees);
     for (int i = 0; i < n_trees; ++i) {
         TreeDev& t = h_trees_[i];
-        if (dalloc(&t.hdr, max_nodes_) || dalloc(&t.board, max_nodes_)) return -1;
-        if (dalloc(&t.P, max_edges_) || dalloc(&t.Q, max_edges_) || dalloc(&t.N, max_edges_) || dalloc(&t.child, max_edges_) ||
-            dalloc(&t.cbase, max_edges_) ||
-            dalloc(&t.move, max_edges_) || dalloc(&t.vl, max_edges_) || dalloc(&t.etype, max_edges_))
-            return -1;
-        if (dalloc(&t.st, 1) || dalloc(&t.bs, 1)) return -1;
-        if (dalloc(&t.new_node, B) || dalloc(&t.traj_node, static_cast<size_t>(2) * B * kMaxDepth) ||
-            dalloc(&t.traj_ci, static_cast<size_t>(2) * B * kMaxDepth) || dalloc(&t.traj_len, 2 * B) || dalloc(&t.traj_start, 2 * B) ||
-            dalloc(&t.traj_edge, static_cast<size_t>(2) * B * kMaxDepth))
-            return -1;
-        const size_t slots = static_cast<size_t>(max_nodes_) * kPrepSlots;
-        if (dalloc(&t.prep_board, slots) || dalloc(&t.prep_ci, slots) || dalloc(&t.prep_term, slots) ||
-            dalloc(&t.exp_parent, 3 * B))
-            return -1;
-        if (dalloc(&d_hist_keys_[i], hist_cap_) || dalloc(&d_hist_reps_[i], hist_cap_)) return -1;
+        if (alloc_pools(t) || alloc_batch_arrays(t) || mem_.dalloc(&t.st, 1)) return -1;
+        if (mem_.dalloc(&d_hist_keys_[i], hist_cap_) || mem_.dalloc(&d_hist_reps_[i], hist_cap_)) return -1;
         t.hist_keys = d_hist_keys_[i];
         t.hist_reps = d_hist_reps_[i];
         t.hist_len = 0;
@@ -629,7 +617,9 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         t.slot_base = i * B;
         d_states_[i] = t.st;
     }
-    if (dalloc(&d_trees_, n_trees) || dalloc(&d_roots_, n_trees) || dalloc(&d_results_, n_trees) || dalloc(&d_limits_, n_trees)) return -1;
+    if (mem_.dalloc(&d_trees_, n_trees) || mem_.dalloc(&d_roots_, n_trees) || mem_.dalloc(&d_results_, n_trees) || mem_.dalloc(&d_limits_, n_trees) ||
+        mem_.dalloc(&d_tstats_, 1) || mem_.dalloc(&d_count_, 1) || mem_.dalloc(&d_node_view_, 1))
+        return -1;
     h_limits_.assign(n_trees, make_uint2(sp.simulations, sp.nodes));
     for (int i = 0; i < n_trees; ++i) {  // the trees' Dirichlet generators (TreeState::rng)
         const uint32_t x = minstd_seed(sp.seed, i);
@@ -641,43 +631,30 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     }
     d_trees_slot_[0] = d_trees_;
     if (threads_ == 2) {
-        slot1_.resize(n_trees);
-        for (int i = 0; i < n_trees; ++i) {
-            SlotArrays& a = slot1_[i];
-            if (dalloc(&a.new_node, B) || dalloc(&a.traj_node, static_cast<size_t>(2) * B * kMaxDepth) ||
-                dalloc(&a.traj_ci, static_cast<size_t>(2) * B * kMaxDepth) || dalloc(&a.traj_len, 2 * B) || dalloc(&a.traj_start, 2 * B) ||
-                dalloc(&a.traj_edge, static_cast<size_t>(2) * B * kMaxDepth) || dalloc(&a.exp_parent, 3 * B) || dalloc(&a.bs, 1))
-                return -1;
-        }
-        if (dalloc(&d_trees_slot_[1], n_trees)) return -1;
+        h_trees1_.resize(n_trees);
+        for (auto& t : h_trees1_)
+            if (alloc_batch_arrays(t)) return -1;
+        if (mem_.dalloc(&d_trees_slot_[1], n_trees)) return -1;
         if (net_ != nullptr) {
             if (net_->enable_second_io()) return -1;
         } else {
             d_values_slot_[0] = d_values_, d_probs_slot_[0] = d_probs_;
-            if (dalloc(&d_values_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
-            if (dalloc(&d_probs_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
+            if (mem_.dalloc(&d_values_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
+            if (mem_.dalloc(&d_probs_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
         }
-        {   // the network stream yields to the tree stream: a pending select / expand launch is never queued behind the
-            // thread blocks of a convolution grid
-            int lo = 0, hi = 0;
-            ARA_CUDA_OK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-            const char* e = getenv("ARA_NET_STREAM_PRIO");
-            ARA_CUDA_OK(cudaStreamCreateWithPriority(&net_stream_, cudaStreamNonBlocking, (e && atoi(e) == 0) ? hi : lo));
-        }
+        // the network stream has the same (default) priority as the tree stream: neither yields to the other
+        ARA_CUDA_OK(cudaStreamCreateWithFlags(&net_stream_, cudaStreamNonBlocking));
         for (int k = 0; k < 2; ++k) {
             ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_sel_[k], cudaEventDisableTiming));
             ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_net_[k], cudaEventDisableTiming));
         }
-        ARA_CUDA_OK(cudaMalloc(&d_count_slot_[1], sizeof(int)));
+        if (mem_.dalloc(&d_count_slot_[1], 1)) return -1;
     }
     h_roots_.resize(n_trees);
     results.resize(n_trees);
     ARA_CUDA_OK(cudaMallocHost(&h_done_, sizeof(int) * n_trees));
     ARA_CUDA_OK(cudaMallocHost(&h_tstats_, sizeof(RootTimeStats)));
-    ARA_CUDA_OK(cudaMalloc(&d_tstats_, sizeof(RootTimeStats)));
-    ARA_CUDA_OK(cudaMalloc(&d_count_, sizeof(int)));
     d_count_slot_[0] = d_count_;
-    if (const char* e = getenv("ARA_ITER_GRAPH")) use_iter_graph_ = atoi(e) != 0;
     ARA_CUDA_OK(cudaStreamCreateWithFlags(&side_stream_, cudaStreamNonBlocking));
     ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
     ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_join_, cudaEventDisableTiming));
@@ -771,20 +748,12 @@ int Search::enqueue_slot_tree_ops(int slot, bool with_update) {
 int Search::enqueue_slot(int slot, bool with_update) {
     const int B = sp.batch_size;
     if (with_update) ARA_CUDA_OK(cudaStreamWaitEvent(stream_, ev_net_[slot], 0));
-    const bool graphed = use_iter_graph_ && !profile;
     cudaGraphExec_t& ge = slot_graph_[slot][with_update ? 1 : 0];
     if (profile) prof_event();
-    if (graphed && ge != nullptr) {
+    if (!profile && ge != nullptr) {
         ARA_CUDA_OK(cudaGraphLaunch(ge, stream_));
-    } else if (graphed && slot_warm_) {
-        cudaGraph_t g;
-        ARA_CUDA_OK(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-        const int rc = enqueue_slot_tree_ops(slot, with_update);
-        const cudaError_t e = cudaStreamEndCapture(stream_, &g);
-        if (rc) return -1;
-        ARA_CUDA_OK(e);
-        ARA_CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
-        cudaGraphDestroy(g);
+    } else if (!profile && slot_warm_) {
+        if (capture_graph(stream_, &ge, [&] { return enqueue_slot_tree_ops(slot, with_update); })) return -1;
         ARA_CUDA_OK(cudaGraphLaunch(ge, stream_));
     } else {
         if (enqueue_slot_tree_ops(slot, with_update)) return -1;
@@ -831,23 +800,16 @@ int Search::iterate2(int cycles) {
 int Search::iterate(int count) {
     if (threads_ == 2) return iterate2((count + 1) / 2);
     const int search_kernels = 4 + (net_ ? 0 : 1);  // (one tree: select, expand, scatter+prepare, backup; many: + pack, one update launch)
-    const bool graphed = use_iter_graph_ && !profile;
     for (int it = 0; it < count; ++it) {
-        if (graphed && iter_graph_ != nullptr) {
+        if (!profile && iter_graph_ != nullptr) {
             ARA_CUDA_OK(cudaGraphLaunch(iter_graph_, stream_));
             if (net_) net_->launches += net_->kernels_per_forward(false);
-        } else if (graphed && iter_warm_) {
+        } else if (!profile && iter_warm_) {
             // second iteration of the handle's life (the first one ran eagerly and warmed the network's graph up)
             const long long net_before = net_ ? net_->launches : 0;
-            cudaGraph_t g;
-            ARA_CUDA_OK(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-            const int rc = enqueue_iteration(false);
-            const cudaError_t e = cudaStreamEndCapture(stream_, &g);
+            const int rc = capture_graph(stream_, &iter_graph_, [&] { return enqueue_iteration(false); });
             if (net_) net_->launches = net_before;
             if (rc) return -1;
-            ARA_CUDA_OK(e);
-            ARA_CUDA_OK(cudaGraphInstantiate(&iter_graph_, g, 0));
-            cudaGraphDestroy(g);
             --it;  // nothing ran yet: launch the graph in the next pass
             continue;
         } else {
@@ -869,8 +831,8 @@ int Search::compact_pools() {
     if (!any) return 0;
     advanced_.assign(n_trees, 0);
     if (d_cinfo_ == nullptr) {
-        if (dalloc(&d_cinfo_, n_trees) || dalloc(&d_keep_n_, static_cast<size_t>(max_nodes_) + 1) ||
-            dalloc(&d_keep_e_, static_cast<size_t>(max_nodes_) + 1) || dalloc(&d_ctotal_, 2))
+        if (mem_.dalloc(&d_cinfo_, n_trees) || mem_.dalloc(&d_keep_n_, static_cast<size_t>(max_nodes_) + 1) ||
+            mem_.dalloc(&d_keep_e_, static_cast<size_t>(max_nodes_) + 1) || mem_.dalloc(&d_ctotal_, 2))
             return -1;
         shadow_.resize(n_trees);
         for (auto& t : shadow_) t.hdr = nullptr;
@@ -895,21 +857,13 @@ int Search::compact_pools() {
         TreeDev& d = shadow_[i];
         if (d.hdr == nullptr) {
             d = t;
-            const size_t slots = static_cast<size_t>(max_nodes_) * kPrepSlots;
-            if (dalloc(&d.hdr, max_nodes_) || dalloc(&d.board, max_nodes_) || dalloc(&d.P, max_edges_) || dalloc(&d.Q, max_edges_) ||
-                dalloc(&d.N, max_edges_) || dalloc(&d.child, max_edges_) || dalloc(&d.cbase, max_edges_) || dalloc(&d.move, max_edges_) ||
-                dalloc(&d.vl, max_edges_) || dalloc(&d.etype, max_edges_) || dalloc(&d.prep_board, slots) || dalloc(&d.prep_ci, slots) ||
-                dalloc(&d.prep_term, slots))
-                return -1;
+            if (alloc_pools(d)) return -1;
         }
         compact_gather_kernel<<<(c.n_nodes + 7) / 8, 256, 0, stream_>>>(t, d, c.cand, c.n_nodes, d_keep_n_, d_keep_e_);
         compact_finish_kernel<<<1, 1, 0, stream_>>>(t.st, total[0], total[1]);
         launches += 2;
         // swap the pools: the tree now lives in what was the second set
-        std::swap(t.hdr, d.hdr), std::swap(t.board, d.board), std::swap(t.P, d.P), std::swap(t.Q, d.Q), std::swap(t.N, d.N);
-        std::swap(t.child, d.child), std::swap(t.cbase, d.cbase), std::swap(t.move, d.move), std::swap(t.vl, d.vl);
-        std::swap(t.etype, d.etype), std::swap(t.prep_board, d.prep_board), std::swap(t.prep_ci, d.prep_ci);
-        std::swap(t.prep_term, d.prep_term);
+        for_each_pool([&](auto m, size_t) { std::swap(t.*m, d.*m); });
         ++compactions;
     }
     ARA_CUDA_OK(cudaGetLastError());
@@ -929,13 +883,11 @@ int Search::begin() {
     ARA_CUDA_OK(cudaMemcpyAsync(d_roots_, h_roots_.data(), sizeof(Board) * n_trees, cudaMemcpyHostToDevice, stream_));
     if (compact_pools()) return -1;
     if (threads_ == 2) {  // the second thread's views of the trees: same pools, its own batch arrays
-        h_trees1_ = h_trees_;
         for (int i = 0; i < n_trees; ++i) {
-            TreeDev& t = h_trees1_[i];
-            const SlotArrays& a = slot1_[i];
-            t.exp_parent = a.exp_parent, t.new_node = a.new_node, t.traj_node = a.traj_node, t.traj_len = a.traj_len;
-            t.traj_ci = a.traj_ci, t.traj_edge = a.traj_edge, t.bs = a.bs, t.traj_start = a.traj_start;
-            ARA_CUDA_OK(cudaMemsetAsync(a.bs, 0, sizeof(BatchState), stream_));
+            TreeDev v = h_trees_[i];
+            for_each_batch_array([&](auto m, size_t) { v.*m = h_trees1_[i].*m; });
+            h_trees1_[i] = v;
+            ARA_CUDA_OK(cudaMemsetAsync(v.bs, 0, sizeof(BatchState), stream_));
         }
         ARA_CUDA_OK(cudaMemcpyAsync(d_trees_slot_[1], h_trees1_.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
         primed_ = false;
@@ -1000,7 +952,6 @@ int Search::node_view(int tree, int node_id, NodeView* out) {
     if (tree < 0 || tree >= n_trees) return set_error("ara_search_node: tree %d out of range", tree);
     if (!searched_) return set_error("ara_search_node: no search has been started on this handle");
     ARA_CUDA_OK(cudaSetDevice(device_));
-    if (d_node_view_ == nullptr) ARA_CUDA_OK(cudaMalloc(&d_node_view_, sizeof(NodeView)));
     node_view_kernel<<<1, 32, 0, stream_>>>(d_trees_, tree, node_id, d_node_view_);
     ++launches;
     ARA_CUDA_OK(cudaMemcpyAsync(out, d_node_view_, sizeof(NodeView), cudaMemcpyDeviceToHost, stream_));
@@ -1072,21 +1023,9 @@ int Search::go() {
             }
         }
         if (polled_root && iterate(chunk)) return -1;
-        for (int i = 0; i < n_trees; ++i)
-            ARA_CUDA_OK(cudaMemcpyAsync(&h_done_[i], &d_states_[i]->done, sizeof(int), cudaMemcpyDeviceToHost, stream_));
-        ARA_CUDA_OK(cudaStreamSynchronize(stream_));
-        all_done = true;
-        for (int i = 0; i < n_trees; ++i) all_done = all_done && (h_done_[i] != 0);
-        // errors also stop the loop: they set done through the error flag check below
-        if (!all_done) {
-            int err = 0;
-            for (int i = 0; i < n_trees && !err; ++i) {
-                TreeState st;
-                ARA_CUDA_OK(cudaMemcpy(&st, d_states_[i], sizeof(st), cudaMemcpyDeviceToHost));
-                err = st.error;
-            }
-            if (err) return set_error("ara_search_go: device search error %d (1 node pool, 2 edge pool, 3 depth > %d)", err, kMaxDepth);
-        }
+        const int running = poll_running();
+        if (running < 0) return -1;
+        all_done = running == 0;
         if (polled_root) chunk = timed ? 4 : 2;
         polled_root = true;
         if (++guard > (1 << 22)) return set_error("ara_search_go: search did not terminate");
@@ -1310,18 +1249,15 @@ __global__ void glibc_flt32_kernel(const float* x, const float* y, int n, float*
 }
 extern "C" int ara_debug_powf_logf(const float* x, const float* y, int n, float* pow_out, float* log_out) {
     if (n <= 0 || !x || !y) return ara::set_error("ara_debug_powf_logf: bad arguments");
+    ara::DeviceBuffers mem;
     float *dx = nullptr, *dy = nullptr, *dp = nullptr, *dl = nullptr;
     const size_t bytes = sizeof(float) * static_cast<size_t>(n);
-    ARA_CUDA_OK(cudaMalloc(&dx, bytes));
-    ARA_CUDA_OK(cudaMalloc(&dy, bytes));
-    ARA_CUDA_OK(cudaMalloc(&dp, bytes));
-    ARA_CUDA_OK(cudaMalloc(&dl, bytes));
+    if (mem.dalloc(&dx, n) || mem.dalloc(&dy, n) || mem.dalloc(&dp, n) || mem.dalloc(&dl, n)) return -1;
     ARA_CUDA_OK(cudaMemcpy(dx, x, bytes, cudaMemcpyHostToDevice));
     ARA_CUDA_OK(cudaMemcpy(dy, y, bytes, cudaMemcpyHostToDevice));
     glibc_flt32_kernel<<<(n + 255) / 256, 256>>>(dx, dy, n, pow_out ? dp : nullptr, log_out ? dl : nullptr);
     ARA_CUDA_OK(cudaGetLastError());
     if (pow_out) ARA_CUDA_OK(cudaMemcpy(pow_out, dp, bytes, cudaMemcpyDeviceToHost));
     if (log_out) ARA_CUDA_OK(cudaMemcpy(log_out, dl, bytes, cudaMemcpyDeviceToHost));
-    cudaFree(dx), cudaFree(dy), cudaFree(dp), cudaFree(dl);
     return 0;
 }
