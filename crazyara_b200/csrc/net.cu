@@ -94,11 +94,14 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     BlobReader rd;
     rd.f = fopen(blob_path, "rb");
     if (!rd.f) return set_error("ara_net_create: cannot open weight blob '%s'", blob_path);
+    // ARAB2001: the networks of the reference's PyTorch definition.  ARAB2002 (the MXNet symbols) adds the header flags
+    // stem_act and policy_bias, and per block flags and the squeeze-excitation gate.
     char magic[8];
-    if (!rd.read(magic, 8) || memcmp(magic, "ARAB2001", 8) != 0)
-        return set_error("ara_net_create: '%s' is not an ARAB2001 weight blob", blob_path);
-    int h[8];
-    if (!rd.read(h, sizeof(h))) return set_error("ara_net_create: truncated header");
+    if (!rd.read(magic, 8) || (memcmp(magic, "ARAB2001", 8) != 0 && memcmp(magic, "ARAB2002", 8) != 0))
+        return set_error("ara_net_create: '%s' is not an ARAB2001 / ARAB2002 weight blob", blob_path);
+    const bool v2 = magic[7] == '2';
+    int h[10] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 0};
+    if (!rd.read(h, (v2 ? 10 : 8) * sizeof(int))) return set_error("ara_net_create: truncated header");
     hdr.in_channels = h[0];
     hdr.policy_channels = h[1];
     hdr.n_blocks = h[2];
@@ -107,6 +110,10 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     hdr.value_fc = h[5];
     hdr.wdl_mode = h[6];
     hdr.input_version = h[7];
+    hdr.stem_act = h[8];
+    hdr.policy_bias = h[9];
+    if ((hdr.stem_act != 0 && hdr.stem_act != 1) || (hdr.policy_bias != 0 && hdr.policy_bias != 1))
+        return set_error("ara_net_create: header flags stem_act %d policy_bias %d", hdr.stem_act, hdr.policy_bias);
     if (hdr.channels != 256 || hdr.value_channels != 8 || hdr.value_fc != 256)
         return set_error("ara_net_create: unsupported trunk geometry (channels %d, value %d/%d)", hdr.channels,
                          hdr.value_channels, hdr.value_fc);
@@ -116,13 +123,18 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     blocks.resize(hdr.n_blocks);
     max_cop_ = 0;
     for (auto& b : blocks) {
-        int t[3];
-        if (!rd.read(t, sizeof(t))) return set_error("ara_net_create: truncated block table");
+        int t[5] = {0, 0, 0, 0, kTrunkGateHard6};
+        if (!rd.read(t, (v2 ? 5 : 3) * sizeof(int))) return set_error("ara_net_create: truncated block table");
         b.c_op = t[0];
         b.kernel = t[1];
         b.se_type = t[2];
+        b.flags = t[3];
+        b.gate = t[4];
         if (b.c_op % 32 != 0 || b.c_op < 32 || (b.kernel != 3 && b.kernel != 5) || b.se_type < 0 || b.se_type > 2)
             return set_error("ara_net_create: unsupported block (c_op %d kernel %d se %d)", b.c_op, b.kernel, b.se_type);
+        if ((b.flags & ~(kBlobShortcutPreSe | kBlobSeBias)) != 0 || b.gate < kTrunkGateHard6 || b.gate > kTrunkGateSigmoid ||
+            ((b.flags & kBlobSeBias) && b.se_type != 1))
+            return set_error("ara_net_create: unsupported block flags %d gate %d (se %d)", b.flags, b.gate, b.se_type);
         if (b.c_op > max_cop_) max_cop_ = b.c_op;
     }
     const size_t C = hdr.channels;
@@ -132,7 +144,10 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
         const BlockDesc& bd = blocks[i];
         HostBlock& hb = hw->blocks[i];
         const size_t cop = bd.c_op, kk = static_cast<size_t>(bd.kernel) * bd.kernel;
-        if (bd.se_type == 1 && (!rd.tensor(hb.se_a, 128 * 256) || !rd.tensor(hb.se_b, 256 * 128))) return -1;
+        const bool se_bias = (bd.flags & kBlobSeBias) != 0;
+        if (bd.se_type == 1 && (!rd.tensor(hb.se_a, 128 * 256) || (se_bias && !rd.tensor(hb.se_b1, 128)) ||
+                                !rd.tensor(hb.se_b, 256 * 128) || (se_bias && !rd.tensor(hb.se_b2, 256))))
+            return -1;
         if (bd.se_type == 2 && (!rd.tensor(hb.se_a, 256 * 256) || !rd.tensor(hb.se_b, 256))) return -1;
         if (!rd.tensor(hb.w1, cop * C) || !rd.tensor(hb.b1, cop) || !rd.tensor(hb.wd, cop * kk) || !rd.tensor(hb.bd, cop) ||
             !rd.tensor(hb.w2, C * cop) || !rd.tensor(hb.b2, C))
@@ -147,7 +162,8 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
             return -1;
     }
     if (!rd.tensor(hw->pol_w1, C * C * 9) || !rd.tensor(hw->pol_b1, C) ||
-        !rd.tensor(hw->pol_w2, static_cast<size_t>(hdr.policy_channels) * C * 9))
+        !rd.tensor(hw->pol_w2, static_cast<size_t>(hdr.policy_channels) * C * 9) ||
+        (hdr.policy_bias && !rd.tensor(hw->pol_b2, hdr.policy_channels)))
         return -1;
     char tail;
     if (fread(&tail, 1, 1, rd.f) != 0) return set_error("ara_net_create: trailing bytes in weight blob");
@@ -170,6 +186,12 @@ static void se_transposed(const BlockDesc& bd, const HostBlock& hb, std::vector<
             for (int k = 0; k < 256; ++k) (*a)[k * 256 + c] = hb.se_a[c * 256 + k];
         *b = hb.se_b;
     }
+}
+
+// the bias of the last policy convolution (ARAB2002 policy_bias), zero padded to the weight rows; else none
+int Net::upload_policy_bias(const HostWeights& hw, int rows) {
+    if (!hdr.policy_bias) return 0;
+    return upload_f32(hw.pol_b2.data(), hw.pol_b2.size(), rows, &pol_b2);
 }
 
 int Net::upload_value_head(const HostWeights& hw) {
@@ -202,7 +224,7 @@ int Net::build_half(const HostWeights& hw) {
     int wrows = 0;
     if (upload_conv_w(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
     if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
-    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, cin_pad, stem_w, wrows, C, 3, stem_b, 1, nullptr, 0, d_x[0], nullptr, C,
+    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, cin_pad, stem_w, wrows, C, 3, stem_b, hdr.stem_act, nullptr, 0, d_x[0], nullptr, C,
                         conv_layer_choose_bn(batch, C)))
         return -1;
     std::vector<TrunkBlockHost> tb(hdr.n_blocks);
@@ -219,6 +241,9 @@ int Net::build_half(const HostWeights& hw) {
         tb[i].w2 = hb.w2;
         tb[i].b2 = hb.b2;
         se_transposed(bd, hb, &tb[i].se_w1t, bd.se_type == 1 ? &tb[i].se_w2t : &tb[i].se_b);
+        tb[i].flags = bd.flags & kBlobShortcutPreSe ? kTrunkShortcutPreSe : 0;
+        tb[i].gate = bd.gate;
+        if (bd.se_type == 1) tb[i].se_b1 = hb.se_b1, tb[i].se_b = hb.se_b2;
     }
     __half* xfinal = d_x[1];
     if (rise_trunk_init(&trunk_, tb, d_x[0], xfinal)) return -1;
@@ -228,7 +253,8 @@ int Net::build_half(const HostWeights& hw) {
                         conv_layer_choose_bn(batch, C)))
         return -1;
     if (upload_conv_w(hw.pol_w2.data(), hdr.policy_channels, C, 3, &pol_w2, &wrows)) return -1;
-    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, C, pol_w2, wrows, hdr.policy_channels, 3, nullptr, 0, nullptr, 0, nullptr,
+    if (upload_policy_bias(hw, wrows)) return -1;
+    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, C, pol_w2, wrows, hdr.policy_channels, 3, pol_b2, 0, nullptr, 0, nullptr,
                         d_logits, ldp, conv_layer_choose_bn(batch, hdr.policy_channels)))
         return -1;
     return 0;
@@ -247,7 +273,7 @@ int Net::build_precise(const HostWeights& hw) {
     int wrows = 0;
     if (upload_conv_w_split(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
     if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
-    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, 3 * cin_pad, stem_w, wrows, C, 3, stem_b, 1, nullptr, 0, nullptr, d_xf[0], C,
+    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, 3 * cin_pad, stem_w, wrows, C, 3, stem_b, hdr.stem_act, nullptr, 0, nullptr, d_xf[0], C,
                         conv_layer_choose_bn(batch, C)))
         return -1;
     conv_layer_set_precise(&stem_conv, nullptr, 0, d_xs[0], C);
@@ -263,6 +289,8 @@ int Net::build_precise(const HostWeights& hw) {
             se_transposed(bd, hb, &ta, &tbv);
             if (upload_f32(ta.data(), ta.size(), ta.size(), &w.se_w1t)) return -1;
             if (upload_f32(tbv.data(), tbv.size(), tbv.size(), bd.se_type == 1 ? &w.se_w2t : &w.se_b)) return -1;
+            if (!hb.se_b1.empty() && (upload_f32(hb.se_b1.data(), 128, 128, &w.se_b1) || upload_f32(hb.se_b2.data(), 256, 256, &w.se_b)))
+                return -1;
         }
         // conv1 1x1 256 -> c_op, ReLU: split X -> fp32 H1
         if (upload_conv_w_split(hb.w1.data(), bd.c_op, C, 1, &w.w1, &wrows)) return -1;
@@ -293,7 +321,8 @@ int Net::build_precise(const HostWeights& hw) {
         return -1;
     conv_layer_set_precise(&pol_conv1, nullptr, 0, d_p1, C);
     if (upload_conv_w_split(hw.pol_w2.data(), hdr.policy_channels, C, 3, &pol_w2, &wrows)) return -1;
-    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, 3 * C, pol_w2, wrows, hdr.policy_channels, 3, nullptr, 0, nullptr, 0, nullptr,
+    if (upload_policy_bias(hw, wrows)) return -1;
+    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, 3 * C, pol_w2, wrows, hdr.policy_channels, 3, pol_b2, 0, nullptr, 0, nullptr,
                         d_logits, ldp, conv_layer_choose_bn(batch, hdr.policy_channels)))
         return -1;
     ARA_CUDA_OK(cudaFuncSetAttribute(value_head_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -377,7 +406,8 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
         PreciseBlock& w = pb_[i];
         const int in = i & 1;
         if (bd.se_type != 0) {
-            ARA_CUDA_OK(launch_pdl(se_f32_kernel, dim3(n), dim3(256), 0, s, d_xf[in], d_xs[in], w.se_w1t, w.se_w2t, w.se_b, bd.se_type));
+            ARA_CUDA_OK(launch_pdl(se_f32_kernel, dim3(n), dim3(256), 0, s, d_xf[in], d_xs[in], w.se_w1t, w.se_w2t, w.se_b, w.se_b1,
+                                   bd.se_type, bd.gate, (bd.flags & kBlobShortcutPreSe) ? 1 : 0));
             ++launches;
         }
         if (conv_layer_launch(&w.conv1, n, s)) return -1;

@@ -15,7 +15,12 @@ struct BlockDesc {
     int c_op;
     int kernel;   // 3 or 5
     int se_type;  // 0 none, 1 ca_se, 2 eca_se
+    int flags;    // ARAB2002: kBlobShortcutPreSe | kBlobSeBias
+    int gate;     // ARAB2002: squeeze-excitation gate (kTrunkGate*)
 };
+// ARAB2002 block flags: the shortcut adds the block input before the squeeze-excitation; the ca_se fully-connected layers
+// have biases
+constexpr int kBlobShortcutPreSe = 1, kBlobSeBias = 2;
 
 struct NetHeader {
     int in_channels;
@@ -26,11 +31,13 @@ struct NetHeader {
     int value_fc;        // 256
     int wdl_mode;        // 1: value head with WDL + plys-to-end auxiliary outputs
     int input_version;   // e.g. 10 = v1.0, 30 = v3.0
+    int stem_act;        // 1: ReLU behind the stem convolution (ARAB2001: always)
+    int policy_bias;     // 1: the last policy convolution has a bias (ARAB2001: never)
 };
 
 // Precision float32: one bottleneck block as separate launches on fp32 activations (net.cu, conv_gemm.cuh)
 struct PreciseBlock {
-    float *se_w1t = nullptr, *se_w2t = nullptr, *se_b = nullptr;
+    float *se_w1t = nullptr, *se_w2t = nullptr, *se_b = nullptr, *se_b1 = nullptr;
     __half *w1 = nullptr, *w2 = nullptr;  // operand-split weights [rows][3 * cw] per tap: hi | lo | hi
     float *b1 = nullptr, *wd = nullptr, *bd = nullptr, *b2 = nullptr;
     ConvLayer conv1, conv2;
@@ -39,13 +46,14 @@ struct PreciseBlock {
 // the tensors of a weight blob, host side, in blob order (weights.py)
 struct HostBlock {
     std::vector<float> se_a, se_b;  // ca_se: fc1 [128][256], fc2 [256][128]; eca_se: centre tap [256][256], bias [256]
+    std::vector<float> se_b1, se_b2;  // ca_se with kBlobSeBias: fc1 bias [128], fc2 bias [256]
     std::vector<float> w1, b1, wd, bd, w2, b2;
 };
 struct HostWeights {
     std::vector<float> stem_w, stem_b;
     std::vector<HostBlock> blocks;
     std::vector<float> vh_wv, vh_bv, vh_a, vh_ab, vh_b, vh_bb;  // standard: fc1 / b1 / fc2 / b2; WDL: wdl w / b, plys w / b
-    std::vector<float> pol_w1, pol_b1, pol_w2;
+    std::vector<float> pol_w1, pol_b1, pol_w2, pol_b2;  // pol_b2: [policy_channels] when hdr.policy_bias
 };
 
 class Net {
@@ -124,6 +132,7 @@ class Net {
     int build_half(const HostWeights& hw);
     int build_precise(const HostWeights& hw);
     int upload_value_head(const HostWeights& hw);
+    int upload_policy_bias(const HostWeights& hw, int rows);
     int enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io);
     int launch_graph(int family, int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io, bool stem_done);
     DeviceBuffers mem_;
@@ -137,7 +146,7 @@ class Net {
     float *vh_wv = nullptr, *vh_bv = nullptr, *vh_w1t = nullptr, *vh_b1 = nullptr, *vh_w2 = nullptr, *vh_b2 = nullptr;
     float *vh_wdl_w = nullptr, *vh_wdl_b = nullptr, *vh_plys_w = nullptr, *vh_plys_b = nullptr;
     __half *pol_w1 = nullptr, *pol_w2 = nullptr;
-    float* pol_b1 = nullptr;
+    float *pol_b1 = nullptr, *pol_b2 = nullptr;
     ConvLayer pol_conv1, pol_conv2;
     std::map<int, cudaGraphExec_t> graphs_[6];  // plain, from fp32 input, with a device-side count (io 0), the same for io 1
     const int* baked_[6] = {};                  // the counter pointer each graph family was captured with

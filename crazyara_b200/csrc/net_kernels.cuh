@@ -98,13 +98,22 @@ __global__ void dwconv_f32_kernel(const float* __restrict__ in, const float* __r
 
 // Squeeze-excitation on the 256-channel trunk (builder_util.py:49-114), fp32 in place + the split copy.  One CTA (256
 // threads) per board.
-//   mode 1 ("ca_se"):  s = hardsigmoid(W2 * relu(W1 * mean))        W1t: [256][128], W2t: [128][256] (transposed)
-//   mode 2 ("eca_se"): s = hardsigmoid(Wc * mean + bc)              W1t: [256][256] centre tap transposed, b: [256]
+//   mode 1 ("ca_se"):  s = gate(W2 * relu(W1 * mean + b1) + b)      W1t: [256][128], W2t: [128][256] (transposed)
+//   mode 2 ("eca_se"): s = gate(Wc * mean + b)                      W1t: [256][256] centre tap transposed, b: [256]
+// b1, b (ca_se): the MXNet symbols' fully-connected biases, or null.  gate: kTrunkGate* (rise_trunk_args.h).
+// keep_x: the block's shortcut is its input before the squeeze-excitation (MXNet symbols), so only the split copy, which
+// the block's first convolution reads, is scaled and x stays as it is.
 __device__ __forceinline__ float hard_sigmoid(float x) { return fminf(fmaxf(x * (1.0f / 6.0f) + 0.5f, 0.0f), 1.0f); }
+__device__ __forceinline__ float se_gate(float x, int gate) {
+    if (gate == 0) return hard_sigmoid(x);
+    if (gate == 1) return fminf(fmaxf(x * 0.2f + 0.5f, 0.0f), 1.0f);
+    return 1.0f / (1.0f + expf(-x));
+}
 
 __global__ void __launch_bounds__(256) se_f32_kernel(float* __restrict__ x, __half* __restrict__ xs,
                                                        const float* __restrict__ w1t, const float* __restrict__ w2t,
-                                                       const float* __restrict__ bias, int mode) {
+                                                       const float* __restrict__ bias, const float* __restrict__ b1, int mode,
+                                                       int gate, int keep_x) {
     __shared__ float s_pool[256];
     __shared__ float s_hid[128];
     pdl_wait();
@@ -121,23 +130,23 @@ __global__ void __launch_bounds__(256) se_f32_kernel(float* __restrict__ x, __ha
     float scale;
     if (mode == 1) {
         if (c < 128) {
-            float h = 0.0f;
+            float h = b1 != nullptr ? __ldg(b1 + c) : 0.0f;
             for (int k = 0; k < 256; ++k) h = fmaf(__ldg(w1t + k * 128 + c), s_pool[k], h);
             s_hid[c] = fmaxf(h, 0.0f);
         }
         __syncthreads();
-        float o = 0.0f;
+        float o = bias != nullptr ? __ldg(bias + c) : 0.0f;
         for (int j = 0; j < 128; ++j) o = fmaf(__ldg(w2t + j * 256 + c), s_hid[j], o);
-        scale = hard_sigmoid(o);
+        scale = se_gate(o, gate);
     } else {
         float o = __ldg(bias + c);
         for (int k = 0; k < 256; ++k) o = fmaf(__ldg(w1t + k * 256 + c), s_pool[k], o);
-        scale = hard_sigmoid(o);
+        scale = se_gate(o, gate);
     }
 #pragma unroll 8
     for (int sq = 0; sq < 64; ++sq) {
         const float v = xb[sq * 256 + c] * scale;
-        xb[sq * 256 + c] = v;
+        if (!keep_x) xb[sq * 256 + c] = v;
         store_split(sb + sq * 768, 256, c, v);
     }
 }

@@ -49,6 +49,16 @@ struct RtCfg {
 #endif
 
 __device__ __forceinline__ float rt_hard_sigmoid(float x) { return fminf(fmaxf(x * (1.0f / 6.0f) + 0.5f, 0.0f), 1.0f); }
+// the squeeze-excitation gate of a block; kernels built without MX only have the torch one
+template <bool MX>
+__device__ __forceinline__ float rt_gate(float x, int gate) {
+    if (!MX || gate == kTrunkGateHard6) return rt_hard_sigmoid(x);
+    if (gate == kTrunkGateHard5) return fminf(fmaxf(x * 0.2f + 0.5f, 0.0f), 1.0f);
+    return 1.0f / (1.0f + expf(-x));
+}
+// b[i] + a when the block has that bias (MXNet ca_se fully-connected layers), else a
+template <bool MX>
+__device__ __forceinline__ float rt_add_bias(const float* b, int i, float a) { return MX && b != nullptr ? __ldg(b + i) + a : a; }
 __device__ __forceinline__ float2 rt_unpack(uint32_t v) { return __half22float2(*reinterpret_cast<const __half2*>(&v)); }
 __device__ __forceinline__ uint32_t rt_pack(float a, float b) {
     const __half2 h = __floats2half2_rn(a, b);
@@ -120,6 +130,7 @@ __device__ __forceinline__ void rt_load_x(uint8_t* sX, const __half* x_in, int b
 }
 
 // squeeze-excitation on the block input, in place: thread t owns channels 2t, 2t+1
+template <bool MX>
 __device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* sX, float* sPool, float* sHid, int t, int wg) {
     float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll 8
@@ -135,7 +146,7 @@ __device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* 
         float a = 0.0f;
 #pragma unroll 16
         for (int k = 0; k < 256; ++k) a = fmaf(__half2float(B.se_w1t[k * 128 + t]), sPool[k], a);
-        sHid[t] = fmaxf(a, 0.0f);
+        sHid[t] = fmaxf(rt_add_bias<MX>(B.se_b1, t, a), 0.0f);
         rt_wg_sync(wg);
         float a0 = 0.0f, a1 = 0.0f;
         const __half2* w2 = reinterpret_cast<const __half2*>(B.se_w2t) + t;
@@ -145,7 +156,8 @@ __device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* 
             a0 = fmaf(wf.x, sHid[j], a0);
             a1 = fmaf(wf.y, sHid[j], a1);
         }
-        sc0 = rt_hard_sigmoid(a0), sc1 = rt_hard_sigmoid(a1);
+        sc0 = rt_gate<MX>(rt_add_bias<MX>(B.se_b, 2 * t, a0), B.gate);
+        sc1 = rt_gate<MX>(rt_add_bias<MX>(B.se_b, 2 * t + 1, a1), B.gate);
     } else {  // 256 -> 256 + bias (hard sigmoid)
         float a0 = 0.0f, a1 = 0.0f;
         const __half2* w1 = reinterpret_cast<const __half2*>(B.se_w1t) + t;
@@ -155,7 +167,7 @@ __device__ __forceinline__ void rt_squeeze_excite(const TrunkBlock& B, uint8_t* 
             a0 = fmaf(wf.x, sPool[k], a0);
             a1 = fmaf(wf.y, sPool[k], a1);
         }
-        sc0 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t) + a0), sc1 = rt_hard_sigmoid(__ldg(B.se_b + 2 * t + 1) + a1);
+        sc0 = rt_gate<MX>(__ldg(B.se_b + 2 * t) + a0, B.gate), sc1 = rt_gate<MX>(__ldg(B.se_b + 2 * t + 1) + a1, B.gate);
     }
 #pragma unroll 8
     for (int r = 0; r < 64; ++r) {
@@ -198,7 +210,8 @@ __device__ __forceinline__ void rt_depthwise_stage(const uint8_t* sH1, const uin
     }
 }
 
-template <int NB>
+// MX: the kernel also runs the blocks of MXNet RISE symbols (TrunkBlock::flags, gate, se_b1)
+template <int NB, bool MX>
 // A consumer needs ~230 registers (accumulators: 160).  Two boards = 12 warps, 3 per 16 K-register SM sub-partition:
 // 168 each at launch, then the producer warpgroup drops to 40 and the consumers grow to 232 (2 x 232 + 40 = 504).
 __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(const __grid_constant__ TrunkArgs args) {
@@ -274,7 +287,17 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
     for (int b = 0; b < n_blocks; ++b) {
         const TrunkBlock& B = args.blk[b];
         const int nch = B.n_chunks;
-        if (B.se_type != 0) rt_squeeze_excite(B, sX, sPool, sHid, t, wg);
+        // shortcut from the block input before the squeeze-excitation: MMA2 accumulates onto it
+        const bool pre = MX && (B.flags & kTrunkShortcutPreSe);
+        if (pre)
+#pragma unroll
+            for (int jj = 0; jj < 32; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float2 xr = __half22float2(*reinterpret_cast<const __half2*>(sX + rt_x_off(fr + 8 * h, 8 * jj + fc)));
+                    acc2[4 * jj + 2 * h] = xr.x, acc2[4 * jj + 2 * h + 1] = xr.y;
+                }
+        if (B.se_type != 0) rt_squeeze_excite<MX>(B, sX, sPool, sHid, t, wg);
         RT_PROF(1);  // squeeze-excitation
 
         for (int j = 0; j < nch; ++j) {
@@ -317,7 +340,7 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
 #pragma unroll
             for (int k = 0; k < 4; ++k)
                 wgmma_f16<256>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
-                               (j > 0 || k > 0) ? 1u : 0u);
+                               (pre || j > 0 || k > 0) ? 1u : 0u);
             wgmma_commit();
             wgmma_wait<0>();
             wgmma_fence_regs(acc2);
@@ -325,7 +348,7 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
             ++u;
             RT_PROF(7);  // MMA2
         }
-        // ---- block epilogue: X <- (D2 + b2) + X (the last block: to global memory)
+        // ---- block epilogue: X <- (D2 + b2) + X, or D2 + b2 with the shortcut in D2 (the last block: to global memory)
         const bool last = b == n_blocks - 1;
 #pragma unroll
         for (int jj = 0; jj < 32; ++jj) {
@@ -335,8 +358,9 @@ __global__ void __launch_bounds__(RtCfg<NB>::kThreads, 1) rise_trunk_kernel(cons
             for (int h = 0; h < 2; ++h) {
                 const int r = fr + 8 * h;
                 __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, c));
-                const float2 xr = __half22float2(*x);
-                const __half2 y = __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
+                const float2 xr = pre ? make_float2(0.0f, 0.0f) : __half22float2(*x);
+                const __half2 y = pre ? __floats2half2_rn(acc2[4 * jj + 2 * h] + b2.x, acc2[4 * jj + 2 * h + 1] + b2.y)
+                                      : __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
                 if (!last)
                     *x = y;
                 else if (board_ok)
@@ -392,6 +416,7 @@ __device__ __forceinline__ void rt_pair_sync() { asm volatile("bar.sync 3, 256;"
 // scales directly.  Every output is stored into both CTAs; the partner's stores are st.async that complete bytes on
 // hid_bar / scale_bar, which thread 0 arms for 64 / 128 values.  hid_bar advances on ca_se blocks only, scale_bar on
 // every SE block, so each has its own phase parity.  On return no thread reads the SE image any more.
+template <bool MX>
 __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint8_t* sX, const uint8_t* ring, int u2, float* sPool,
                                                        float* sHid, float* sScale, uint64_t* hid_bar, uint64_t* scale_bar,
                                                        uint32_t hid_parity, uint32_t scale_parity, uint32_t rank, int tid) {
@@ -421,8 +446,8 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
 #pragma unroll 16
                 for (int k = 0; k < 128; ++k) a = fmaf(__half2float(wq[k * 64]), sPool[128 * q + k], a);
             }
-            const float h = fmaxf(a, 0.0f);
             const int o = 64 * static_cast<int>(rank) + tid;
+            const float h = fmaxf(rt_add_bias<MX>(B.se_b1, o, a), 0.0f);
             sHid[o] = h;
             st_async_cluster_b32(cluster_map(sHid + o, peer), __float_as_uint(h), cluster_map(hid_bar, peer));
         }
@@ -436,7 +461,7 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
 #pragma unroll 16
                 for (int j = 0; j < 64; ++j) a = fmaf(__half2float(wq[j * 128]), sHid[64 * q + j], a);
             }
-            sc = rt_hard_sigmoid(a);
+            sc = rt_gate<MX>(rt_add_bias<MX>(B.se_b, 128 * static_cast<int>(rank) + tid, a), B.gate);
         }
     } else if (tid < 128) {  // 256 -> 256 + bias (hard sigmoid): [256 k][128], 64 k per unit
         float a = 0.0f;
@@ -446,7 +471,7 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
 #pragma unroll 16
             for (int k = 0; k < 64; ++k) a = fmaf(__half2float(wq[k * 128]), sPool[64 * q + k], a);
         }
-        sc = rt_hard_sigmoid(__ldg(B.se_b + 128 * rank + tid) + a);
+        sc = rt_gate<MX>(__ldg(B.se_b + 128 * rank + tid) + a, B.gate);
     }
     if (tid < 128) {
         const int c = 128 * static_cast<int>(rank) + tid;
@@ -468,7 +493,8 @@ __device__ __forceinline__ void rt_pair_squeeze_excite(const TrunkBlock& B, uint
     rt_pair_sync();
 }
 
-// launched with clusters of 2 CTAs along x: CTAs 2 i and 2 i + 1 run board i
+// launched with clusters of 2 CTAs along x: CTAs 2 i and 2 i + 1 run board i.  MX: as in rise_trunk_kernel
+template <bool MX>
 __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel(const __grid_constant__ TrunkArgs args) {
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 900)
     using Cfg = RtPairCfg;
@@ -565,10 +591,22 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
         for (int b = 0; b < n_blocks; ++b) {
             const TrunkBlock& B = args.blk[b];
             const int nch = B.n_chunks;
+            const int panel = 2 * static_cast<int>(rank) + wg;
+            // shortcut from the block input before the squeeze-excitation: MMA2 accumulates onto it
+            const bool pre = MX && (B.flags & kTrunkShortcutPreSe);
+            if (pre)
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const float2 xr =
+                            __half22float2(*reinterpret_cast<const __half2*>(sX + rt_x_off(fr + 8 * h, 64 * panel + 8 * jj + fc)));
+                        acc2[4 * jj + 2 * h] = xr.x, acc2[4 * jj + 2 * h + 1] = xr.y;
+                    }
             if (B.se_type != 0) {
                 for (int i = 0; i < Cfg::kSeUnits; ++i) mbar_wait(&w2_full[(u2 + i) % R2], ((u2 + i) / R2) & 1);
                 RT_PROF(1);  // wait for the SE image
-                rt_pair_squeeze_excite(B, sX, smem + Cfg::kOffW2, u2, sPool, sHid, sScale, se_hid, se_scale, n_ca & 1, n_se & 1, rank,
+                rt_pair_squeeze_excite<MX>(B, sX, smem + Cfg::kOffW2, u2, sPool, sHid, sScale, se_hid, se_scale, n_ca & 1, n_se & 1, rank,
                                        threadIdx.x);
                 if (t == 0)
                     for (int i = 0; i < Cfg::kSeUnits; ++i) mbar_arrive(&w2_empty[(u2 + i) % R2]);
@@ -634,7 +672,7 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
                     wgmma_f16<64>(acc2, wgmma_desc_k_sw128(aH2 + k * 32, 1024), wgmma_desc_k_sw128(aW2 + k * 32, 1024),
-                                  (j > 0 || k > 0) ? 1u : 0u);
+                                  (pre || j > 0 || k > 0) ? 1u : 0u);
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_regs(acc2);
@@ -663,7 +701,6 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                 mbar_wait_cluster(x_free, b & 1);
             }
             RT_PROF(11);  // wait for the partner to release its X tile
-            const int panel = 2 * static_cast<int>(rank) + wg;
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) {
                 const int c = 64 * panel + 8 * jj + fc;
@@ -672,8 +709,9 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                 for (int h = 0; h < 2; ++h) {
                     const int r = fr + 8 * h;
                     __half2* x = reinterpret_cast<__half2*>(sX + rt_x_off(r, c));
-                    const float2 xr = __half22float2(*x);
-                    const __half2 y = __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
+                    const float2 xr = pre ? make_float2(0.0f, 0.0f) : __half22float2(*x);
+                    const __half2 y = pre ? __floats2half2_rn(acc2[4 * jj + 2 * h] + b2.x, acc2[4 * jj + 2 * h + 1] + b2.y)
+                                          : __floats2half2_rn((acc2[4 * jj + 2 * h] + b2.x) + xr.x, (acc2[4 * jj + 2 * h + 1] + b2.y) + xr.y);
                     if (!last)
                         *x = y;
                     else if (board_ok)

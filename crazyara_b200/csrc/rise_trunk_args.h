@@ -19,6 +19,11 @@ constexpr int kTrunkW2Image = 32768;
 //   eca_se: columns 128 r .. 128 r + 127 as [256 k][128]
 constexpr int kTrunkSeImage = 65536;
 
+// the residual adds the block input as it was before the squeeze-excitation scaled it (MXNet RISE symbols)
+constexpr int kTrunkShortcutPreSe = 1;
+// squeeze-excitation gates: clamp(x / 6 + 0.5) (torch Hardsigmoid), clamp(0.2 x + 0.5) (MXNet hard_sigmoid), sigmoid
+constexpr int kTrunkGateHard6 = 0, kTrunkGateHard5 = 1, kTrunkGateSigmoid = 2;
+
 struct TrunkBlock {
     int n_chunks;     // ceil(Cop / 64)
     int ksize;        // depthwise kernel: 3 or 5
@@ -27,8 +32,12 @@ struct TrunkBlock {
     const float* b2;       // [256]
     const __half* se_w1t;  // ca_se: [256][128]; eca_se: [256][256] (transposed, fp16 copy owned by the trunk)
     const __half* se_w2t;  // ca_se: [128][256]
-    const float* se_b;     // eca_se: [256]
+    const float* se_b;     // eca_se: [256]; ca_se: fc2 bias [256] or null
     const uint8_t* se_img;  // [2 ranks][kTrunkSeImage] (rise_trunk_pair_kernel)
+    // read only by the kernels built for the MXNet semantics (RiseTrunk::mx):
+    int flags;             // kTrunkShortcutPreSe
+    int gate;              // squeeze-excitation gate, kTrunkGate*
+    const float* se_b1;    // ca_se: fc1 bias [128] or null
 };
 
 struct TrunkArgs {

@@ -38,10 +38,15 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
         B.ksize = h.ksize;
         B.se_type = h.se_type;
         B.chunk0 = chunks;
+        B.flags = h.flags;
+        B.gate = h.gate;
+        if (h.gate < kTrunkGateHard6 || h.gate > kTrunkGateSigmoid) return set_error("rise_trunk_init: block %d has gate %d", i, h.gate);
+        T->mx = T->mx || h.flags != 0 || h.gate != kTrunkGateHard6 || !h.se_b1.empty();
         if (upload(T->mem, h.b2, &B.b2)) return -1;
         if (h.se_type != 0) {  // fp16 copies of the squeeze-excitation matrices (the kernel is bound by their traffic)
             const size_t n1 = h.se_type == 1 ? 256 * 128 : 256 * 256, n2 = h.se_type == 1 ? 128 * 256 : 0;
-            if (h.se_type == 2 && upload(T->mem, h.se_b, &B.se_b)) return -1;
+            if (!h.se_b.empty() && upload(T->mem, h.se_b, &B.se_b)) return -1;
+            if (!h.se_b1.empty() && upload(T->mem, h.se_b1, &B.se_b1)) return -1;
             std::vector<__half> hh(n1 + n2);
             for (size_t k = 0; k < n1; ++k) hh[k] = __float2half_rn(h.se_w1t[k]);
             for (size_t k = 0; k < n2; ++k) hh[n1 + k] = __float2half_rn(h.se_w2t[k]);
@@ -101,9 +106,12 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
     if (upload(T->mem, w1, &T->args.w1_img) || upload(T->mem, w2, &T->args.w2_img)) return -1;
     if (T->mem.dalloc(&T->d_prof, 32)) return -1;
     T->args.prof = T->d_prof;
-    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<1>::kSmemBytes));
-    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<2>::kSmemBytes));
-    ARA_CUDA_OK(cudaFuncSetAttribute(rise_trunk_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RtPairCfg::kSmemBytes));
+    const auto k1 = T->mx ? rise_trunk_kernel<1, true> : rise_trunk_kernel<1, false>;
+    const auto k2 = T->mx ? rise_trunk_kernel<2, true> : rise_trunk_kernel<2, false>;
+    const auto kp = T->mx ? rise_trunk_pair_kernel<true> : rise_trunk_pair_kernel<false>;
+    ARA_CUDA_OK(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<1>::kSmemBytes));
+    ARA_CUDA_OK(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, RtCfg<2>::kSmemBytes));
+    ARA_CUDA_OK(cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, RtPairCfg::kSmemBytes));
     {
         int dev = 0;
         cudaDeviceProp prop;
@@ -122,7 +130,7 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
         attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        ARA_CUDA_OK(cudaOccupancyMaxActiveClusters(&T->pair_clusters, rise_trunk_pair_kernel, &cfg));
+        ARA_CUDA_OK(cudaOccupancyMaxActiveClusters(&T->pair_clusters, kp, &cfg));
     }
     return 0;
 }
@@ -138,12 +146,14 @@ int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const
     const char* force = getenv("ARA_TRUNK_ROWS");
     const int rows = force ? atoi(force) : boards <= T->pair_clusters ? 32 : boards <= T->sm_count ? 64 : 128;
     if (rows == 32)
-        ARA_CUDA_OK(launch_pdl_cluster(rise_trunk_pair_kernel, dim3(2 * boards), dim3(RtPairCfg::kThreads), RtPairCfg::kSmemBytes,
-                                       stream, 2u, a));
+        ARA_CUDA_OK(launch_pdl_cluster(T->mx ? rise_trunk_pair_kernel<true> : rise_trunk_pair_kernel<false>, dim3(2 * boards),
+                                       dim3(RtPairCfg::kThreads), RtPairCfg::kSmemBytes, stream, 2u, a));
     else if (rows == 64)
-        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<1>, dim3(boards), dim3(RtCfg<1>::kThreads), RtCfg<1>::kSmemBytes, stream, a));
+        ARA_CUDA_OK(launch_pdl(T->mx ? rise_trunk_kernel<1, true> : rise_trunk_kernel<1, false>, dim3(boards), dim3(RtCfg<1>::kThreads),
+                               RtCfg<1>::kSmemBytes, stream, a));
     else
-        ARA_CUDA_OK(launch_pdl(rise_trunk_kernel<2>, dim3((boards + 1) / 2), dim3(RtCfg<2>::kThreads), RtCfg<2>::kSmemBytes, stream, a));
+        ARA_CUDA_OK(launch_pdl(T->mx ? rise_trunk_kernel<2, true> : rise_trunk_kernel<2, false>, dim3((boards + 1) / 2),
+                               dim3(RtCfg<2>::kThreads), RtCfg<2>::kSmemBytes, stream, a));
     return 0;
 }
 

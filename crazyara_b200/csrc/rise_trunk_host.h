@@ -20,13 +20,16 @@ struct TrunkBlockHost {
     std::vector<float> b2;  // [256]
     std::vector<float> se_w1t;  // transposed squeeze-excitation, see TrunkBlock: ca_se [256][128], eca_se [256][256]
     std::vector<float> se_w2t;  // ca_se: [128][256]
-    std::vector<float> se_b;    // eca_se: [256]
+    std::vector<float> se_b;    // eca_se: [256]; ca_se: fc2 bias [256] or empty
+    std::vector<float> se_b1;   // ca_se: fc1 bias [128] or empty
+    int flags = 0, gate = kTrunkGateHard6;  // see TrunkBlock
 };
 
 struct RiseTrunk {
     TrunkArgs args;
     int sm_count = 0;
     int pair_clusters = 0;  // CTA pairs of rise_trunk_pair_kernel resident at once
+    bool mx = false;        // some block needs the kernels built for the MXNet semantics
     unsigned long long* d_prof = nullptr;  // [2][16] cycle counters, written only by -DARA_TRUNK_PROF builds
     DeviceBuffers mem;  // everything the pointers in args and d_prof point to
 };

@@ -13,12 +13,22 @@ the ORDER of its Conv / Gemm / MatMul nodes (a torch export lists them in execut
 PARITY UNPINNED: /root/reference holds no .onnx file and the `onnx` / `onnxsim` packages are absent, so this reader is
 checked against files written by tests/onnx_writer.py (same node kinds and tensor layouts as the torch exporter emits for
 these modules), not against an artefact of the reference itself.
+
+A graph exported from the reference's MXNet symbols (`convert_to_onnx.py`) computes another network from the same
+layers (crazyara_b200/weights.py, export_mx_blob).  It is recognised by its unfolded `BatchNormalization` nodes and read by
+graph edges, not node order: from the stem, each block is the `Add` fed by the block input, traced back through
+BatchNormalization / Relu / Conv to its first convolution, whose input is the block input itself or a `Mul` of it with a
+squeeze-excitation gate (`Sigmoid`, or `HardSigmoid` with its alpha; behind it a 1-D `Conv` over the channels for eca_se,
+or two `Gemm` with biases for ca_se).  The layers go, under the names the symbol code gives them, through export_mx_blob
+into an ARAB2002 blob.  PARITY UNPINNED as well: no MXNet export is in either tree; the reader is checked against files
+written by tests/onnx_mx_writer.py.
 """
 import struct
+from collections import defaultdict
 
 import numpy as np
 
-from .weights import SE_CODE
+from .weights import SE_CODE, export_mx_blob, write_blob
 
 
 # ---------------------------------------------------------------------------------------------- protobuf wire format
@@ -112,6 +122,8 @@ def read_graph(path):
                     for h, hw, hv in _fields(gv):
                         if h == 1:
                             an = bytes(hv).decode()
+                        elif h == 2 and hw == 5:
+                            ai = struct.unpack("<f", hv)[0]  # a float attribute (epsilon, alpha)
                         elif h == 3:
                             ai = hv
                         elif h == 5 and hw == 2:
@@ -134,6 +146,8 @@ def read_graph(path):
 # ---------------------------------------------------------------------------------------------- graph -> blob
 def import_onnx(onnx_path, blob_path, input_version=None, channels=256):
     nodes, inits = read_graph(onnx_path)
+    if any(nd[0] == "BatchNormalization" for nd in nodes):
+        return _import_mxnet_graph(onnx_path, nodes, inits, blob_path, input_version, channels)
     order = []  # convolutions and fully-connected layers in execution order
     for op, ins, outs, attrs in nodes:
         if op == "Conv" and len(ins) >= 2 and ins[1] in inits:
@@ -211,17 +225,147 @@ def import_onnx(onnx_path, blob_path, input_version=None, channels=256):
     arch = dict(name=f"rise_{len(kernels)}b", in_channels=int(stem_w.shape[1]), policy_channels=int(heads[1][1].shape[0]),
                 channels=int(C), kernels=kernels, se_types=se_types, c_ops=c_ops, wdl=bool(wdl), value_channels=int(vconv[0][1].shape[0]),
                 value_fc=256)
-    if input_version is None:
-        input_version = {34: 10, 63: 10, 39: 10, 51: 20, 52: 30, 64: 30, 80: 30}.get(arch["in_channels"], 10)
-    with open(blob_path, "wb") as f:
-        f.write(b"ARAB2001")
-        f.write(struct.pack("<8i", arch["in_channels"], arch["policy_channels"], len(kernels), 256, 8, 256, 1 if wdl else 0, input_version))
-        for k, se, cop in zip(kernels, se_types, c_ops):
-            f.write(struct.pack("<3i", cop, k, SE_CODE[se]))
-        for t in tensors:
-            f.write(struct.pack("<q", t.size))
-            f.write(t.tobytes())
+    write_blob(blob_path, arch, tensors, _input_version(arch, input_version))
     return arch
+
+
+def _input_version(arch, input_version):
+    if input_version is not None:
+        return input_version
+    return {34: 10, 63: 10, 39: 10, 51: 20, 52: 30, 64: 30, 80: 30}.get(arch["in_channels"], 10)
+
+
+def _import_mxnet_graph(onnx_path, nodes, inits, blob_path, input_version, channels):
+    """a graph with unfolded BatchNormalization nodes (an MXNet export), read by its edges -> ARAB2002 blob"""
+    prod, cons = {}, defaultdict(list)
+    for nd in nodes:
+        for o in nd[2]:
+            prod[o] = nd
+        for i in nd[1]:
+            cons[i].append(nd)
+
+    def fail(what):
+        raise ValueError(f"{onnx_path}: {what}")
+
+    def back(t, *ops):  # the producer of t, skipping shape-only nodes, which must be one of ops
+        nd = prod.get(t)
+        while nd is not None and nd[0] in ("Reshape", "Flatten", "Squeeze", "Unsqueeze", "Identity"):
+            nd = prod.get(nd[1][0])
+        if nd is None or nd[0] not in ops:
+            fail(f"expected {'/'.join(ops)} in front of '{t}', found {nd[0] if nd else 'a graph input'}")
+        return nd
+
+    def fwd(t, op):  # the consumer of t with type op, or None
+        return next((nd for nd in cons[t] if nd[0] == op), None)
+
+    params, eps = {}, {}
+
+    def take_bn(nd, name):
+        for key, i in (("gamma", 1), ("beta", 2), ("moving_mean", 3), ("moving_var", 4)):
+            params[f"{name}_{key}"] = inits[nd[1][i]]
+        eps[name] = float(nd[3].get("epsilon", 1e-5))  # (ONNX's default)
+
+    def take(nd, name):  # Conv / Gemm weights and bias under the MXNet layer name
+        w = inits[nd[1][1]]
+        if nd[0] == "Gemm" and not nd[3].get("transB", 0):
+            w = w.T
+        params[name + "_weight"] = np.ascontiguousarray(w)
+        if len(nd[1]) > 2 and nd[1][2] in inits:
+            params[name + "_bias"] = inits[nd[1][2]]
+
+    def conv_bn(t, name):  # t = output of Conv -> BatchNormalization: the Conv node
+        bn = back(t, "BatchNormalization")
+        conv = back(bn[1][0], "Conv")
+        take(conv, name)
+        take_bn(bn, name.replace("conv", "bn"))
+        return conv
+
+    stem = next((nd for nd in nodes if nd[0] == "Conv" and nd[1][0] not in prod and nd[1][0] not in inits), None)
+    if stem is None or inits[stem[1][1]].shape[0] != channels or inits[stem[1][1]].shape[2] != 3:
+        fail(f"no 3x3 stem convolution with {channels} channels on the graph input")
+    take(stem, "stem_conv0")
+    bn = fwd(stem[2][0], "BatchNormalization")
+    if bn is None:
+        fail("no BatchNormalization behind the stem")
+    take_bn(bn, "stem_bn0")
+    relu = fwd(bn[2][0], "Relu")
+    x, stem_act = (relu[2][0], True) if relu is not None and fwd(relu[2][0], "Add") is not None else (bn[2][0], False)
+    kernels, se_types, se_gates, c_ops, n_eca = [], [], [], [], 0
+    while True:
+        add = next((nd for nd in cons[x] if nd[0] == "Add" and len(nd[1]) == 2), None)
+        if add is None:
+            break
+        i, p = len(kernels), f"bc_res_block{len(kernels)}"
+        other = add[1][1] if add[1][0] == x else add[1][0]
+        conv3 = conv_bn(other, p + "_conv3")
+        conv2 = conv_bn(back(conv3[1][0], "Relu")[1][0], p + "_conv2")
+        conv1 = conv_bn(back(conv2[1][0], "Relu")[1][0], p + "_conv1")
+        w1, wd = params[p + "_conv1_weight"], params[p + "_conv2_weight"]
+        if w1.shape[1] != channels or wd.shape[0] != w1.shape[0] or wd.shape[2] not in (3, 5):
+            fail(f"block {i} is not a RISE bottleneck block")
+        se, gate = None, None
+        if conv1[1][0] != x:
+            mul = back(conv1[1][0], "Mul")
+            if x not in mul[1]:
+                fail(f"block {i}: the squeeze-excitation does not act on the block input")
+            g = back(mul[1][1] if mul[1][0] == x else mul[1][0], "Sigmoid", "HardSigmoid")
+            if g[0] == "Sigmoid":
+                gate = "sigmoid"
+            elif abs(g[3].get("alpha", 0.2) - 0.2) < 1e-6 and abs(g[3].get("beta", 0.5) - 0.5) < 1e-6:
+                gate = "hard_sigmoid"
+            else:
+                fail(f"block {i}: HardSigmoid alpha {g[3].get('alpha')} beta {g[3].get('beta')}")
+            fc = back(g[1][0], "Gemm", "MatMul", "Conv")
+            if fc[0] == "Conv":
+                se = "eca_se"
+                take(fc, f"convolution{n_eca}")
+                n_eca += 1
+            else:
+                se = "ca_se"
+                take(fc, p + "_se_fc1")
+                take(back(back(fc[1][0], "Relu")[1][0], "Gemm", "MatMul"), p + "_se_fc0")
+        kernels.append(int(wd.shape[2])), se_types.append(se), se_gates.append(gate), c_ops.append(int(w1.shape[0]))
+        x = add[2][0]
+    if not kernels:
+        fail("no bottleneck block found")
+    heads = [nd for nd in cons[x] if nd[0] == "Conv"]
+    vconv = [nd for nd in heads if inits[nd[1][1]].shape[2] == 1]
+    pconv = [nd for nd in heads if inits[nd[1][1]].shape[2] == 3]
+    if len(vconv) != 1 or len(pconv) != 1:
+        fail("value head (1x1 convolution) and policy head (3x3 convolution) not found behind the tower")
+    take(vconv[0], "value_conv0")
+    take_bn(fwd(vconv[0][2][0], "BatchNormalization"), "value_bn0")
+    g0 = _downstream(cons, vconv[0][2][0], ("Gemm", "MatMul"))
+    g1 = g0 and _downstream(cons, g0[2][0], ("Gemm", "MatMul"))
+    if g1 is None:
+        fail("value head: two fully-connected layers not found")
+    take(g0, "value_fc0"), take(g1, "value_fc1")
+    take(pconv[0], "policy_conv0")
+    take_bn(fwd(pconv[0][2][0], "BatchNormalization"), "policy_bn0")
+    take(_downstream(cons, pconv[0][2][0], ("Conv",)), "policy_conv1")
+    arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(inits[stem[1][1]].shape[1]),
+                policy_channels=int(params["policy_conv1_weight"].shape[0]), channels=channels, kernels=kernels,
+                se_types=se_types, se_gates=se_gates, c_ops=c_ops, wdl=False, value_channels=int(params["value_conv0_weight"].shape[0]),
+                value_fc=256, stem_act=stem_act, policy_bias="policy_conv1_bias" in params)
+    export_mx_blob(params, arch, blob_path, _input_version(arch, input_version), eps=eps, fix_gamma=False)
+    return arch
+
+
+def _downstream(cons, t, ops):
+    """the first node of one of ops reached from tensor t along single-consumer element-wise edges"""
+    seen = set()
+    frontier = [t]
+    while frontier:
+        nxt = []
+        for u in frontier:
+            for nd in cons[u]:
+                if nd[0] in ops:
+                    return nd
+                if id(nd) not in seen:
+                    seen.add(id(nd))
+                    nxt += nd[2]
+        frontier = nxt
+    return None
 
 
 if __name__ == "__main__":

@@ -76,3 +76,48 @@ def random_state_dict(arch, seed=0):
     batchnorm("policy_head.body.1", C)
     sd["policy_head.body.3.weight"] = normal((arch["policy_channels"], C, 3, 3), 2.0 * np.sqrt(2.0 / (9 * C)))
     return sd
+
+
+def mx_twin(arch):
+    """the same tower as the reference's MXNet symbols define it (rise_mobile_v2.py / rise_mobile_v3.py; see
+    crazyara_b200.weights.export_mx_blob): v2 (ca_se) with sigmoid gates, a stem ReLU and no policy bias; v3 (eca_se) with
+    clamp(0.2 x + 0.5) gates, no stem activation, a policy bias and the plain value head"""
+    v2 = "ca_se" in arch["se_types"]
+    return dict(arch, name="mx_" + arch["name"], semantics="mxnet", wdl=False, stem_act=v2, policy_bias=not v2,
+                se_gates=[(("sigmoid" if v2 else "hard_sigmoid") if s else None) for s in arch["se_types"]])
+
+
+def random_mx_params(arch, seed=0):
+    """Seeded parameters of an mx_twin network under the symbol code's names (BatchNorm as name_gamma / _beta /
+    _moving_mean / _moving_var, eca_se convolutions as convolution<n>), scaled like random_state_dict"""
+    g = np.random.default_rng(seed)
+    p = {}
+    normal = lambda shape, std: (g.standard_normal(shape) * std).astype(np.float32)
+
+    def conv_bn(name, bn, cout, cin, k, groups=1, std=None):
+        p[name + "_weight"] = normal((cout, cin // groups, k, k), std or np.sqrt(2.0 / (cin // groups * k * k)))
+        p[bn + "_gamma"], p[bn + "_beta"] = np.ones(cout, np.float32), normal(cout, 0.1)
+        p[bn + "_moving_mean"], p[bn + "_moving_var"] = normal(cout, 0.1), g.uniform(0.5, 1.5, cout).astype(np.float32)
+
+    C, n_eca = arch["channels"], 0
+    conv_bn("stem_conv0", "stem_bn0", C, arch["in_channels"], 3)
+    for i, (k, se, cop) in enumerate(zip(arch["kernels"], arch["se_types"], arch["c_ops"])):
+        b = f"bc_res_block{i}"
+        if se == "ca_se":
+            p[b + "_se_fc0_weight"], p[b + "_se_fc0_bias"] = normal((C // 2, C), 2.0 / np.sqrt(C)), normal(C // 2, 0.1)
+            p[b + "_se_fc1_weight"], p[b + "_se_fc1_bias"] = normal((C, C // 2), 2.0 / np.sqrt(C // 2)), normal(C, 0.1)
+        elif se == "eca_se":
+            p[f"convolution{n_eca}_weight"], p[f"convolution{n_eca}_bias"] = normal((1, 1, 5), 1.0), normal(1, 0.5)
+            n_eca += 1
+        conv_bn(b + "_conv1", b + "_bn1", cop, C, 1)
+        conv_bn(b + "_conv2", b + "_bn2", cop, cop, k, groups=cop)
+        conv_bn(b + "_conv3", b + "_bn3", C, cop, 1, std=0.5 / np.sqrt(cop))
+    conv_bn("value_conv0", "value_bn0", arch["value_channels"], C, 1)
+    n = arch["value_channels"] * 64
+    p["value_fc0_weight"], p["value_fc0_bias"] = normal((arch["value_fc"], n), 1.0 / np.sqrt(n)), normal(arch["value_fc"], 0.1)
+    p["value_fc1_weight"], p["value_fc1_bias"] = normal((1, arch["value_fc"]), 1.0 / np.sqrt(arch["value_fc"])), normal(1, 0.1)
+    conv_bn("policy_conv0", "policy_bn0", C, C, 3)
+    p["policy_conv1_weight"] = normal((arch["policy_channels"], C, 3, 3), np.sqrt(2.0 / (9 * C)))
+    if arch["policy_bias"]:
+        p["policy_conv1_bias"] = normal(arch["policy_channels"], 0.1)
+    return p

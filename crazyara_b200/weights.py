@@ -1,9 +1,17 @@
-"""Weight import: reference state_dict (PyTorch parameter names of RiseV3) -> ARAB2001 blob for ara_net_create.
+"""Weight import: reference state_dict (PyTorch parameter names of RiseV3) -> ARAB2001 blob for ara_net_create, and
+MXNet-named parameters of the reference's symbol networks (rise_mobile_v2.py, rise_mobile_v3.py) -> ARAB2002 blob.
 
 BatchNorm (eval mode, eps 1e-5) is folded into the preceding convolution here, in float64, so the CUDA side only
 sees conv weight + bias.  The blob is architecture-described by its header, so any RISEv2 / RISEv3.x checkpoint of
 the reference trainer (trainer_agent_pytorch.py:506-516 saves {'model_state_dict': ...}) converts without code
-changes.  Tensor order must match crazyara_b200/csrc/net.cu (Net::init).
+changes.  Tensor order must match crazyara_b200/csrc/net.cu (Net::read_blob).
+
+The MXNet symbols compute a different network from the same layers (export_mx_blob): a block's shortcut is its input
+before the squeeze-excitation, ca_se has fully-connected biases and a sigmoid (RISEv2) or clamp(0.2 x + 0.5) gate
+(v3), eca_se is a 5-tap convolution over the channel axis with one bias, the v3 stem has no activation and the v3
+policy convolution a bias, and BatchNorm has MXNet's defaults (eps 1e-3, gamma fixed to 1).  ARAB2002 carries what
+cannot be folded into weights: per block the shortcut flag and the gate, in the header the stem activation and the
+policy bias.
 """
 import struct
 
@@ -11,6 +19,10 @@ import numpy as np
 
 BN_EPS = 1e-5
 SE_CODE = {None: 0, "ca_se": 1, "se": 1, "eca_se": 2}
+MX_BN_EPS = 1e-3  # mx.sym.BatchNorm's default
+# squeeze-excitation gates: torch Hardsigmoid clamp(x / 6 + 0.5), MXNet hard_sigmoid clamp(0.2 x + 0.5), sigmoid
+GATE_CODE = {None: 0, "torch_hard_sigmoid": 0, "hard_sigmoid": 1, "sigmoid": 2}
+SHORTCUT_PRE_SE, SE_BIAS = 1, 2  # ARAB2002 block flags
 
 
 def _np(t):
@@ -64,17 +76,115 @@ def export_blob(sd, arch, path, input_version=10):
     w, b = _fold(sd, "policy_head.body.0.weight", "policy_head.body.1")
     put(w), put(b)
     put(_np(sd["policy_head.body.3.weight"]))
+    return write_blob(path, arch, tensors, input_version)
 
+
+def write_blob(path, arch, tensors, input_version):
+    """Header, block table and the float32 tensors (flattened, in net.cu's order).  ARAB2001 for the PyTorch semantics;
+    ARAB2002 when arch["semantics"] == "mxnet" (every block's shortcut from its input before the SE, ca_se with biases)."""
+    mx = arch.get("semantics") == "mxnet"
     with open(path, "wb") as f:
-        f.write(b"ARAB2001")
+        f.write(b"ARAB2002" if mx else b"ARAB2001")
         f.write(struct.pack("<8i", arch["in_channels"], arch["policy_channels"], len(arch["kernels"]), 256, 8, 256,
                             1 if arch["wdl"] else 0, input_version))
-        for k, se, cop in zip(arch["kernels"], arch["se_types"], arch["c_ops"]):
-            f.write(struct.pack("<3i", cop, k, SE_CODE[se]))
+        if mx:
+            f.write(struct.pack("<2i", int(arch["stem_act"]), int(arch["policy_bias"])))
+        for i, (k, se, cop) in enumerate(zip(arch["kernels"], arch["se_types"], arch["c_ops"])):
+            if mx:
+                flags = SHORTCUT_PRE_SE | (SE_BIAS if SE_CODE[se] == 1 else 0)
+                f.write(struct.pack("<5i", cop, k, SE_CODE[se], flags, GATE_CODE[arch["se_gates"][i]]))
+            else:
+                f.write(struct.pack("<3i", cop, k, SE_CODE[se]))
         for t in tensors:
+            t = np.ascontiguousarray(t, dtype=np.float32).reshape(-1)
             f.write(struct.pack("<q", t.size))
             f.write(t.tobytes())
     return path
+
+
+# ---------------------------------------------------------------------------------------------- MXNet symbols
+def mx_bn_prefix(params, prefix):
+    """the BatchNorm behind layer `prefix`: `<prefix>` (rise_mobile_v2.py, get_stem, the heads) or `<prefix>_bn1`
+    (rise_mobile_v3.py's get_norm_layer appends '_bn1' to the name it is given)"""
+    return prefix if prefix + "_moving_mean" in params else prefix + "_bn1"
+
+
+def mx_eca_names(params):
+    """weight names of the eca_se convolutions in block order: the symbol leaves them unnamed, so MXNet names them
+    convolution<n> in creation order (builder_util_symbol.py:321)"""
+    idx = sorted(int(k[len("convolution"):-len("_weight")]) for k in params
+                 if k.startswith("convolution") and k.endswith("_weight") and k[len("convolution"):-len("_weight")].isdigit())
+    return [f"convolution{i}" for i in idx]
+
+
+def _mx_fold(params, conv, bn, eps, fix_gamma):
+    w = _np(params[conv + "_weight"])
+    e = eps.get(bn, MX_BN_EPS) if isinstance(eps, dict) else eps
+    g = np.ones(w.shape[0]) if fix_gamma else _np(params[bn + "_gamma"])
+    s = g / np.sqrt(_np(params[bn + "_moving_var"]) + e)
+    b = _np(params[bn + "_beta"]) - _np(params[bn + "_moving_mean"]) * s
+    if conv + "_bias" in params:  # (the symbols' convolutions in front of a BatchNorm have none)
+        b = b + _np(params[conv + "_bias"]) * s
+    return w * s.reshape(-1, *([1] * (w.ndim - 1))), b
+
+
+def eca_band(w, channels=256):
+    """a one-filter 1-D convolution over the channel axis (weight [1, 1, k], zero padding k // 2) as the [out][in]
+    matrix the eca_se kernels take"""
+    taps = np.asarray(w, np.float64).reshape(-1)
+    r = taps.size // 2
+    m = np.zeros((channels, channels))
+    for c in range(channels):
+        for t in range(taps.size):
+            if 0 <= c + t - r < channels:
+                m[c, c + t - r] = taps[t]
+    return m
+
+
+def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamma=True):
+    """MXNet-named parameters (arg and aux params as the reference's symbol code names them) -> ARAB2002 blob.
+    arch: as oracle.net_mx.arch_mx_risev2 / arch_mx_risev33 (semantics "mxnet", se_gates, stem_act, policy_bias).
+    eps: BatchNorm epsilon, one value or {BatchNorm name: eps} (missing names: MXNet's default 1e-3).  fix_gamma: the
+    BatchNorm gammas are fixed to 1 (mx.sym.BatchNorm's default), whatever values the parameters hold.  ca_se hidden
+    widths below 128 are zero-padded to 128; the eca_se convolution becomes its banded 256 x 256 matrix."""
+    assert arch.get("semantics") == "mxnet"
+    tensors = []
+    put = tensors.append
+    fold = lambda conv, bn: _mx_fold(params, conv, mx_bn_prefix(params, bn), eps, fix_gamma)
+    w, b = fold("stem_conv0", "stem_bn0")
+    put(w), put(b)
+    eca = iter(mx_eca_names(params))
+    for i, (k, se, cop) in enumerate(zip(arch["kernels"], arch["se_types"], arch["c_ops"])):
+        p = f"bc_res_block{i}"
+        if SE_CODE[se] == 1:
+            w1, w2 = _np(params[p + "_se_fc0_weight"]), _np(params[p + "_se_fc1_weight"])
+            hid = w1.shape[0]
+            if hid > 128:
+                raise ValueError(f"block {i}: ca_se hidden width {hid} > 128")
+            pad = lambda a, ax: np.pad(a, [(0, 128 - hid) if d == ax else (0, 0) for d in range(a.ndim)])
+            put(pad(w1, 0)), put(pad(_np(params[p + "_se_fc0_bias"]), 0))
+            put(pad(w2, 1)), put(_np(params[p + "_se_fc1_bias"]))
+        elif SE_CODE[se] == 2:
+            name = next(eca)
+            put(eca_band(params[name + "_weight"])), put(np.full(256, _np(params[name + "_bias"]).reshape(-1)[0]))
+        w, b = fold(p + "_conv1", p + "_bn1")
+        assert w.shape[0] == cop, (i, w.shape, cop)
+        put(w), put(b)
+        w, b = fold(p + "_conv2", p + "_bn2")
+        assert w.shape == (cop, 1, k, k), (i, w.shape)
+        put(w), put(b)
+        w, b = fold(p + "_conv3", p + "_bn3")
+        put(w), put(b)
+    w, b = fold("value_conv0", "value_bn0")
+    put(w), put(b)
+    for n in ("value_fc0", "value_fc1"):
+        put(_np(params[n + "_weight"])), put(_np(params[n + "_bias"]))
+    w, b = fold("policy_conv0", "policy_bn0")
+    put(w), put(b)
+    put(_np(params["policy_conv1_weight"]))
+    if arch["policy_bias"]:
+        put(_np(params["policy_conv1_bias"]))
+    return write_blob(path, arch, tensors, input_version)
 
 
 def arch_from_state_dict(sd):

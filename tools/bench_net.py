@@ -8,18 +8,32 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from crazyara_b200.nn import NeuralNetAPI  # noqa: E402
-from crazyara_b200.weights import export_blob  # noqa: E402
-from crazyara_b200 import synthetic
+from crazyara_b200.weights import export_blob, export_mx_blob  # noqa: E402
+from crazyara_b200 import synthetic  # noqa: E402
+
+
+def _blob(name, d):
+    """the PyTorch-defined networks (ARAB2001) and their MXNet-symbol twins (ARAB2002: SE off the shortcut)"""
+    path = os.path.join(d, "w.arab")
+    if name == "risev2":
+        arch = synthetic.risev2(34, 81)
+        return arch, export_blob(synthetic.random_state_dict(arch, 0), arch, path, input_version=10)
+    if name == "risev33":
+        arch = synthetic.risev33(52, 76, True)
+        return arch, export_blob(synthetic.random_state_dict(arch, 0), arch, path, input_version=30)
+    arch = synthetic.mx_twin(synthetic.risev2(34, 81) if name == "mx_risev2" else synthetic.risev33(52, 76))
+    return arch, export_mx_blob(synthetic.random_mx_params(arch, 0), arch, path, input_version=10 if name == "mx_risev2" else 30)
 
 
 def main():
     import torch
     iters = int(os.environ.get("ITERS", "200"))
-    for name, arch, ver in (("risev2", synthetic.risev2(34, 81), 10), ("risev33", synthetic.risev33(52, 76, True), 30)):
-        sd = synthetic.random_state_dict(arch, 0)
+    names = os.environ.get("NETS", "risev2,risev33").split(",")  # also: mx_risev2, mx_risev33
+    batches = [int(b) for b in os.environ.get("BATCHES", "1,8,64,128").split(",")]
+    for name in names:
         with tempfile.TemporaryDirectory() as d:
-            blob = export_blob(sd, arch, os.path.join(d, "w.arab"), input_version=ver)
-            for batch in (1, 8, 64, 128):
+            arch, blob = _blob(name, d)
+            for batch in batches:
                 net = NeuralNetAPI("gpu", 0, batch, blob)
                 C = arch["in_channels"]
                 x = torch.rand(batch, C, 8, 8).pin_memory()
