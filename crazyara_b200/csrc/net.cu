@@ -41,50 +41,71 @@ int Net::upload_f32(const float* src, size_t count, size_t padded, float** dst) 
     return 0;
 }
 
-// w: [n_out, cin, k, k] fp32 -> fp16 [rows, taps * cw], column = tap * cw + c, rows padded to 256.
-int Net::upload_conv_w(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows) {
+// w: [n_out, cin, k, k] fp32 -> fp16 [round_up(n_out, 256), taps * parts * cw] with cw = ceil64(cin); per tap the
+// columns are w [cw] (parts 1), or for Precision float32 hi(w) [cw] | lo(w) [cw] | hi(w) [cw] (parts 3), matching
+// activations stored as hi | hi | lo (conv_gemm.cuh).
+int Net::upload_conv_w(const float* w, int n_out, int cin, int ksize, int parts, __half** dst) {
     const int taps = ksize * ksize;
     const int cw = round_up(cin, 64);
-    const int r = round_up(n_out, 256);
-    std::vector<__half> h(static_cast<size_t>(r) * taps * cw, __float2half(0.0f));
-    for (int n = 0; n < n_out; ++n)
-        for (int c = 0; c < cin; ++c)
-            for (int t = 0; t < taps; ++t)
-                h[(static_cast<size_t>(n) * taps + t) * cw + c] = __float2half_rn(w[(static_cast<size_t>(n) * cin + c) * taps + t]);
-    if (mem_.dalloc(dst, h.size()) != 0) return -1;
-    ARA_CUDA_OK(cudaMemcpy(*dst, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    *rows = r;
-    return 0;
-}
-
-// Precision float32: w [n_out, cin, k, k] fp32 -> fp16 [rows, taps * 3 * cw]; per tap the columns are
-// hi(w) [cw] | lo(w) [cw] | hi(w) [cw], matching activations stored as hi | hi | lo (conv_gemm.cuh).
-int Net::upload_conv_w_split(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows) {
-    const int taps = ksize * ksize;
-    const int cw = round_up(cin, 64);
-    const int r = round_up(n_out, 256);
-    std::vector<__half> h(static_cast<size_t>(r) * taps * 3 * cw, __float2half(0.0f));
+    std::vector<__half> h(static_cast<size_t>(round_up(n_out, 256)) * taps * parts * cw, __float2half(0.0f));
     for (int n = 0; n < n_out; ++n)
         for (int c = 0; c < cin; ++c)
             for (int t = 0; t < taps; ++t) {
                 const float v = w[(static_cast<size_t>(n) * cin + c) * taps + t];
                 const __half hi = __float2half_rn(v);
-                const __half lo = __float2half_rn(v - __half2float(hi));
-                __half* col = &h[(static_cast<size_t>(n) * taps + t) * 3 * cw];
+                __half* col = &h[(static_cast<size_t>(n) * taps + t) * parts * cw];
                 col[c] = hi;
-                col[cw + c] = lo;
-                col[2 * cw + c] = hi;
+                if (parts == 3) {
+                    col[cw + c] = __float2half_rn(v - __half2float(hi));
+                    col[2 * cw + c] = hi;
+                }
             }
     if (mem_.dalloc(dst, h.size()) != 0) return -1;
     ARA_CUDA_OK(cudaMemcpy(*dst, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    *rows = r;
+    return 0;
+}
+
+// One conv_gemm layer: uploads its weights w [n_out][cin][k][k] (split in float32), then its bias [n_out] (none if
+// empty), both zero padded to round_up(n_out, 256) rows, and points L at them and at io.
+int Net::build_conv(ConvLayer* L, const std::vector<float>& w, const std::vector<float>& bias, int n_out, int cin, int ksize,
+                    int relu, const ConvIo& io) {
+    const int rows = round_up(n_out, 256);
+    __half* dw = nullptr;
+    float* db = nullptr;
+    if (upload_conv_w(w.data(), n_out, cin, ksize, precision == 0 ? 1 : 3, &dw)) return -1;
+    if (!bias.empty() && upload_f32(bias.data(), bias.size(), rows, &db)) return -1;
+    const int act_cin = precision == 0 ? (io.act_cin ? io.act_cin : cin) : 3 * round_up(cin, 64);
+    if (conv_layer_init(L, io.act, batch_cap, act_cin, dw, rows, n_out, ksize, db, relu, io.res_h, io.ldr, io.out_h, io.out_f,
+                        io.ldo, conv_layer_choose_bn(batch, n_out), io.act_pitch))
+        return -1;
+    if (precision == 1) conv_layer_set_precise(L, io.res_f, io.ldr, io.out_s, io.split_cs);
+    if (io.n_end) L->args.n_end = io.n_end;
+    return 0;
+}
+
+template <typename... KArgs, typename... Args>
+int Net::launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
+    ARA_CUDA_OK(launch_pdl(kernel, grid, block, smem, s, args...));
+    ++launches;
+    return 0;
+}
+
+int Net::launch_conv(const ConvLayer& L, int n, cudaStream_t s, const int* cnt) {
+    if (conv_layer_launch(&L, n, s, cnt)) return -1;
+    ++launches;
+    return 0;
+}
+
+int Net::launch_tower(size_t segment, int n, cudaStream_t s, const int* cnt, const __half* x_in) {
+    if (rise_trunk_launch(trunks_[segment].get(), n, s, cnt, x_in)) return -1;
+    ++launches;
     return 0;
 }
 
 Net::~Net() {
     cudaSetDevice(device);
     for (auto& family : graphs_)
-        for (auto& g : family) cudaGraphExecDestroy(g.second);
+        for (auto& g : family) cudaGraphExecDestroy(g.second.exec);
     if (stream) cudaStreamDestroy(stream);
     if (head_stream) cudaStreamDestroy(head_stream);
     if (ev_fork) cudaEventDestroy(ev_fork);
@@ -264,12 +285,6 @@ static void se_transposed(const BlockDesc& bd, const HostBlock& hb, std::vector<
     }
 }
 
-// the bias of the last policy convolution (ARAB2002 policy_bias), zero padded to the weight rows; else none
-int Net::upload_policy_bias(const HostWeights& hw, int rows) {
-    if (!hdr.policy_bias) return 0;
-    return upload_f32(hw.pol_b2.data(), hw.pol_b2.size(), rows, &pol_b2);
-}
-
 int Net::upload_value_head(const HostWeights& hw) {
     if (upload_f32(hw.vh_wv.data(), hw.vh_wv.size(), hw.vh_wv.size(), &vh_wv)) return -1;
     if (upload_f32(hw.vh_bv.data(), 8, 8, &vh_bv)) return -1;
@@ -312,29 +327,18 @@ int Net::build_ntb_half(const BlockDesc& bd, const HostBlock& hb, NtbLayers* L) 
     const int M = bd.ntb_m, Ca = bd.ntb_ca, H = bd.ntb_h;
     std::vector<float> qkv_w, qkv_b, gc;
     ntb_device_weights(bd, hb, &qkv_w, &qkv_b, &gc);
-    // one conv_gemm layer: out[:, 0 .. n_end) of rows ldo apart (+ residual of rows ldr apart) from act (rows pitch apart)
-    auto layer = [&](ConvLayer* c, const std::vector<float>& w, const std::vector<float>* b, int n_out, int cin, int k,
-                     const __half* act, int pitch, int relu, const __half* res, int ldr, __half* out, int ldo, int n_end) {
-        __half* dw = nullptr;
-        float* db = nullptr;
-        int wrows = 0;
-        if (upload_conv_w(w.data(), n_out, cin, k, &dw, &wrows)) return -1;
-        if (b != nullptr && upload_f32(b->data(), b->size(), round_up(n_out, 256), &db)) return -1;
-        if (conv_layer_init(c, act, batch_cap, cin, dw, wrows, n_out, k, db, relu, res, ldr, out, nullptr, ldo,
-                            conv_layer_choose_bn(batch, n_out), pitch))
-            return -1;
-        c->args.n_end = n_end;
-        return 0;
-    };
     __half *x = d_x[1], *z = d_nt + M;
-    if (layer(&L->pe, hb.pe_w, &hb.pe_b, M, 256, 1, x, 0, 0, nullptr, 0, d_nt, 256, M) ||
-        layer(&L->qkv, qkv_w, &qkv_b, 3 * M, M, 1, d_nt, 256, 0, nullptr, 0, d_qkv, 3 * M, 3 * M) ||
-        layer(&L->proj, hb.proj_w, &hb.proj_b, M, M, 1, d_att, 0, 0, d_nt, 256, d_nt, 256, M) ||
-        layer(&L->prj, hb.prj_w, &hb.prj_b, Ca, M, 1, d_nt, 256, 0, nullptr, 0, z, 256, Ca) ||
-        layer(&L->gc, gc, &hb.gc_b, Ca, Ca, 3, z, 256, 1, nullptr, 0, d_g, Ca, Ca) ||
-        layer(&L->mh, hb.mh_w, nullptr, Ca, Ca, 1, d_g, 0, 0, z, 256, z, 256, Ca) ||
-        layer(&L->mlp1, hb.mlp1_w, &hb.mlp1_b, H, 256, 1, d_nt, 0, 1, nullptr, 0, d_hid, H, H) ||
-        layer(&L->mlp2, hb.mlp2_w, &hb.mlp2_b, 256, H, 1, d_hid, 0, 0, d_nt, 256, x, 256, 256))
+    // y1 and z2 share the rows of d_nt: the layers reading y1 map its M channels only (cin, not rounded to 64), and the
+    // layers writing y1 or z2 end at their own columns (n_end)
+    if (build_conv(&L->pe, hb.pe_w, hb.pe_b, M, 256, 1, 0, {.act = x, .out_h = d_nt, .ldo = 256, .n_end = M}) ||
+        build_conv(&L->qkv, qkv_w, qkv_b, 3 * M, M, 1, 0, {.act = d_nt, .act_pitch = 256, .out_h = d_qkv, .ldo = 3 * M}) ||
+        build_conv(&L->proj, hb.proj_w, hb.proj_b, M, M, 1, 0,
+                   {.act = d_att, .res_h = d_nt, .ldr = 256, .out_h = d_nt, .ldo = 256, .n_end = M}) ||
+        build_conv(&L->prj, hb.prj_w, hb.prj_b, Ca, M, 1, 0, {.act = d_nt, .act_pitch = 256, .out_h = z, .ldo = 256, .n_end = Ca}) ||
+        build_conv(&L->gc, gc, hb.gc_b, Ca, Ca, 3, 1, {.act = z, .act_pitch = 256, .out_h = d_g, .ldo = Ca}) ||
+        build_conv(&L->mh, hb.mh_w, {}, Ca, Ca, 1, 0, {.act = d_g, .res_h = z, .ldr = 256, .out_h = z, .ldo = 256, .n_end = Ca}) ||
+        build_conv(&L->mlp1, hb.mlp1_w, hb.mlp1_b, H, 256, 1, 1, {.act = d_nt, .out_h = d_hid, .ldo = H}) ||
+        build_conv(&L->mlp2, hb.mlp2_w, hb.mlp2_b, 256, H, 1, 0, {.act = d_hid, .res_h = d_nt, .ldr = 256, .out_h = x, .ldo = 256}))
         return -1;
     return 0;
 }
@@ -349,11 +353,8 @@ int Net::build_half(const HostWeights& hw) {
     if (max_m_ > 0 && (mem_.dalloc(&d_nt, rows * 256) || mem_.dalloc(&d_qkv, rows * 3 * max_m_) || mem_.dalloc(&d_att, rows * max_m_) ||
                        mem_.dalloc(&d_g, rows * max_ca_) || mem_.dalloc(&d_hid, rows * max_h_)))
         return -1;
-    int wrows = 0;
-    if (upload_conv_w(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
-    if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
-    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, cin_pad, stem_w, wrows, C, 3, stem_b, hdr.stem_act, nullptr, 0, d_x[0], nullptr, C,
-                        conv_layer_choose_bn(batch, C)))
+    if (build_conv(&stem_conv, hw.stem_w, hw.stem_b, C, hdr.in_channels, 3, hdr.stem_act,
+                   {.act = d_in_h, .act_cin = cin_pad, .out_h = d_x[0], .ldo = C}))
         return -1;
     // the first segment reads the stem output d_x[0]; every later step reads and writes d_x[1] (the tower kernel may run in
     // place, and an NTB's first GEMM reads d_x[1] before its last one writes it)
@@ -390,16 +391,8 @@ int Net::build_half(const HostWeights& hw) {
         if (bd.se_type == 1) t.se_b1 = hb.se_b1, t.se_b = hb.se_b2;
     }
     if (flush()) return -1;
-    __half* xfinal = d_x[1];
-    if (upload_conv_w(hw.pol_w1.data(), C, C, 3, &pol_w1, &wrows)) return -1;
-    if (upload_f32(hw.pol_b1.data(), C, 256, &pol_b1)) return -1;
-    if (conv_layer_init(&pol_conv1, xfinal, batch_cap, C, pol_w1, wrows, C, 3, pol_b1, 1, nullptr, 0, d_p1, nullptr, C,
-                        conv_layer_choose_bn(batch, C)))
-        return -1;
-    if (upload_conv_w(hw.pol_w2.data(), hdr.policy_channels, C, 3, &pol_w2, &wrows)) return -1;
-    if (upload_policy_bias(hw, wrows)) return -1;
-    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, C, pol_w2, wrows, hdr.policy_channels, 3, pol_b2, 0, nullptr, 0, nullptr,
-                        d_logits, ldp, conv_layer_choose_bn(batch, hdr.policy_channels)))
+    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_x[1], .out_h = d_p1, .ldo = C}) ||
+        build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp}))
         return -1;
     return 0;
 }
@@ -414,13 +407,9 @@ int Net::build_precise(const HostWeights& hw) {
     for (int k = 0; k < 2; ++k)
         if (mem_.dalloc(&d_xf[k], rows * C) || mem_.dalloc(&d_xs[k], rows * 3 * C)) return -1;
     if (mem_.dalloc(&d_h1f, rows * max_cop_) || mem_.dalloc(&d_h2s, rows * 3 * max_cp) || mem_.dalloc(&d_p1, rows * 3 * C)) return -1;
-    int wrows = 0;
-    if (upload_conv_w_split(hw.stem_w.data(), C, hdr.in_channels, 3, &stem_w, &wrows)) return -1;
-    if (upload_f32(hw.stem_b.data(), C, 256, &stem_b)) return -1;
-    if (conv_layer_init(&stem_conv, d_in_h, batch_cap, 3 * cin_pad, stem_w, wrows, C, 3, stem_b, hdr.stem_act, nullptr, 0, nullptr, d_xf[0], C,
-                        conv_layer_choose_bn(batch, C)))
+    if (build_conv(&stem_conv, hw.stem_w, hw.stem_b, C, hdr.in_channels, 3, hdr.stem_act,
+                   {.act = d_in_h, .out_f = d_xf[0], .out_s = d_xs[0], .ldo = C, .split_cs = C}))
         return -1;
-    conv_layer_set_precise(&stem_conv, nullptr, 0, d_xs[0], C);
     if (max_m_ > 0) {
         const size_t ms = round_up(max_m_, 64);
         if (mem_.dalloc(&d_yf, rows * max_m_) || mem_.dalloc(&d_qkvf, rows * 3 * max_m_) || mem_.dalloc(&d_zf, rows * max_ca_) ||
@@ -450,11 +439,7 @@ int Net::build_precise(const HostWeights& hw) {
                 return -1;
         }
         // conv1 1x1 256 -> c_op, ReLU: split X -> fp32 H1
-        if (upload_conv_w_split(hb.w1.data(), bd.c_op, C, 1, &w.w1, &wrows)) return -1;
-        if (upload_f32(hb.b1.data(), bd.c_op, round_up(bd.c_op, 256), &w.b1)) return -1;
-        if (conv_layer_init(&w.conv1, d_xs[in], batch_cap, 3 * C, w.w1, wrows, bd.c_op, 1, w.b1, 1, nullptr, 0, nullptr, d_h1f,
-                            bd.c_op, conv_layer_choose_bn(batch, bd.c_op)))
-            return -1;
+        if (build_conv(&w.conv1, hb.w1, hb.b1, bd.c_op, C, 1, 1, {.act = d_xs[in], .out_f = d_h1f, .ldo = bd.c_op})) return -1;
         // depthwise k x k: blob [c_op][k][k] -> device [k*k][c_op]
         const int kk = bd.kernel * bd.kernel;
         t2.assign(static_cast<size_t>(kk) * bd.c_op, 0.f);
@@ -463,24 +448,12 @@ int Net::build_precise(const HostWeights& hw) {
         if (upload_f32(t2.data(), t2.size(), t2.size(), &w.wd)) return -1;
         if (upload_f32(hb.bd.data(), bd.c_op, cp, &w.bd)) return -1;
         // conv2 1x1 c_op -> 256 + fp32 residual: split H2 [.., 3*cp] -> fp32 X' and split X'
-        if (upload_conv_w_split(hb.w2.data(), C, bd.c_op, 1, &w.w2, &wrows)) return -1;
-        if (upload_f32(hb.b2.data(), C, 256, &w.b2)) return -1;
-        if (conv_layer_init(&w.conv2, d_h2s, batch_cap, 3 * cp, w.w2, wrows, C, 1, w.b2, 0, nullptr, 0, nullptr, d_xf[out], C,
-                            conv_layer_choose_bn(batch, C)))
+        if (build_conv(&w.conv2, hb.w2, hb.b2, C, bd.c_op, 1, 0,
+                       {.act = d_h2s, .res_f = d_xf[in], .ldr = C, .out_f = d_xf[out], .out_s = d_xs[out], .ldo = C, .split_cs = C}))
             return -1;
-        conv_layer_set_precise(&w.conv2, d_xf[in], C, d_xs[out], C);
     }
-    const int fin = hdr.n_blocks & 1;
-    if (upload_conv_w_split(hw.pol_w1.data(), C, C, 3, &pol_w1, &wrows)) return -1;
-    if (upload_f32(hw.pol_b1.data(), C, 256, &pol_b1)) return -1;
-    if (conv_layer_init(&pol_conv1, d_xs[fin], batch_cap, 3 * C, pol_w1, wrows, C, 3, pol_b1, 1, nullptr, 0, nullptr, nullptr, C,
-                        conv_layer_choose_bn(batch, C)))
-        return -1;
-    conv_layer_set_precise(&pol_conv1, nullptr, 0, d_p1, C);
-    if (upload_conv_w_split(hw.pol_w2.data(), hdr.policy_channels, C, 3, &pol_w2, &wrows)) return -1;
-    if (upload_policy_bias(hw, wrows)) return -1;
-    if (conv_layer_init(&pol_conv2, d_p1, batch_cap, 3 * C, pol_w2, wrows, hdr.policy_channels, 3, pol_b2, 0, nullptr, 0, nullptr,
-                        d_logits, ldp, conv_layer_choose_bn(batch, hdr.policy_channels)))
+    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_xs[hdr.n_blocks & 1], .out_s = d_p1, .ldo = C, .split_cs = C}) ||
+        build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp}))
         return -1;
     ARA_CUDA_OK(cudaFuncSetAttribute(value_head_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      value_head_smem<float>()));
@@ -494,31 +467,17 @@ int Net::build_ntb_precise(const BlockDesc& bd, const HostBlock& hb, int in, int
     const int M = bd.ntb_m, Ca = bd.ntb_ca, H = bd.ntb_h, ms = round_up(M, 64);
     std::vector<float> qkv_w, qkv_b, gc;
     ntb_device_weights(bd, hb, &qkv_w, &qkv_b, &gc);
-    // one conv_gemm layer on split operands (cin = the channels of one part, 3 cw columns of act): fp32 out[:, 0 .. n_end)
-    // of rows ldo apart and / or the split output of part pitch split_cs, fp32 residual of rows ldr apart
-    auto layer = [&](ConvLayer* c, const std::vector<float>& w, const std::vector<float>* b, int n_out, int cin, int k,
-                     const __half* act, int relu, const float* res, int ldr, float* out_f, int ldo, int n_end, __half* out_s,
-                     int split_cs) {
-        __half* dw = nullptr;
-        float* db = nullptr;
-        int wrows = 0;
-        if (upload_conv_w_split(w.data(), n_out, cin, k, &dw, &wrows)) return -1;
-        if (b != nullptr && upload_f32(b->data(), b->size(), round_up(n_out, 256), &db)) return -1;
-        if (conv_layer_init(c, act, batch_cap, 3 * round_up(cin, 64), dw, wrows, n_out, k, db, relu, nullptr, 0, nullptr, out_f, ldo,
-                            conv_layer_choose_bn(batch, n_out)))
-            return -1;
-        conv_layer_set_precise(c, res, ldr, out_s, split_cs);
-        c->args.n_end = n_end;
-        return 0;
-    };
-    if (layer(&L->pe, hb.pe_w, &hb.pe_b, M, 256, 1, d_xs[in], 0, nullptr, 0, d_yf, M, M, d_ys, ms) ||
-        layer(&L->qkv, qkv_w, &qkv_b, 3 * M, M, 1, d_ys, 0, nullptr, 0, d_qkvf, 3 * M, 3 * M, nullptr, 0) ||
-        layer(&L->proj, hb.proj_w, &hb.proj_b, M, M, 1, d_atts, 0, d_yf, M, d_x2f, 256, M, d_ys, ms) ||
-        layer(&L->prj, hb.prj_w, &hb.prj_b, Ca, M, 1, d_ys, 0, nullptr, 0, d_zf, Ca, Ca, d_zs, 64) ||
-        layer(&L->gc, gc, &hb.gc_b, Ca, Ca, 3, d_zs, 1, nullptr, 0, nullptr, Ca, Ca, d_gs, 64) ||
-        layer(&L->mh, hb.mh_w, nullptr, Ca, Ca, 1, d_gs, 0, d_zf, Ca, d_x2f + M, 256, Ca, nullptr, 0) ||
-        layer(&L->mlp1, hb.mlp1_w, &hb.mlp1_b, H, 256, 1, d_x2s, 1, nullptr, 0, nullptr, H, H, d_hs, H) ||
-        layer(&L->mlp2, hb.mlp2_w, &hb.mlp2_b, 256, H, 1, d_hs, 0, d_x2f, 256, d_xf[out], 256, 256, d_xs[out], 256))
+    if (build_conv(&L->pe, hb.pe_w, hb.pe_b, M, 256, 1, 0, {.act = d_xs[in], .out_f = d_yf, .out_s = d_ys, .ldo = M, .split_cs = ms}) ||
+        build_conv(&L->qkv, qkv_w, qkv_b, 3 * M, M, 1, 0, {.act = d_ys, .out_f = d_qkvf, .ldo = 3 * M}) ||
+        build_conv(&L->proj, hb.proj_w, hb.proj_b, M, M, 1, 0,
+                   {.act = d_atts, .res_f = d_yf, .ldr = M, .out_f = d_x2f, .out_s = d_ys, .ldo = 256, .n_end = M, .split_cs = ms}) ||
+        build_conv(&L->prj, hb.prj_w, hb.prj_b, Ca, M, 1, 0, {.act = d_ys, .out_f = d_zf, .out_s = d_zs, .ldo = Ca, .split_cs = 64}) ||
+        build_conv(&L->gc, gc, hb.gc_b, Ca, Ca, 3, 1, {.act = d_zs, .out_s = d_gs, .ldo = Ca, .split_cs = 64}) ||
+        build_conv(&L->mh, hb.mh_w, {}, Ca, Ca, 1, 0,
+                   {.act = d_gs, .res_f = d_zf, .ldr = Ca, .out_f = d_x2f + M, .ldo = 256, .n_end = Ca}) ||
+        build_conv(&L->mlp1, hb.mlp1_w, hb.mlp1_b, H, 256, 1, 1, {.act = d_x2s, .out_s = d_hs, .ldo = H, .split_cs = H}) ||
+        build_conv(&L->mlp2, hb.mlp2_w, hb.mlp2_b, 256, H, 1, 0,
+                   {.act = d_hs, .res_f = d_x2f, .ldr = 256, .out_f = d_xf[out], .out_s = d_xs[out], .ldo = 256, .split_cs = 256}))
         return -1;
     return 0;
 }
@@ -585,13 +544,10 @@ int Net::enable_second_io() {
 }
 
 int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, int io) {
-    if (from_f32) {
-        ARA_CUDA_OK(launch_pdl(nchw_f32_to_nhwc_split_kernel, dim3(n), dim3(256), hdr.in_channels * 65 * 4, s, d_in_f32, io_in_h[io],
-                               hdr.in_channels, cin_pad));
-        ++launches;
-    }
-    if (conv_layer_launch(io ? &stem_conv2 : &stem_conv, n, s, cnt)) return -1;
-    ++launches;
+    if (from_f32 && launch(nchw_f32_to_nhwc_split_kernel, dim3(n), dim3(256), hdr.in_channels * 65 * 4, s, d_in_f32, io_in_h[io],
+                           hdr.in_channels, cin_pad))
+        return -1;
+    if (launch_conv(io ? stem_conv2 : stem_conv, n, s, cnt)) return -1;
     for (int i = 0, k = 0; i < hdr.n_blocks; ++i) {
         const BlockDesc& bd = blocks[i];
         PreciseBlock& w = pb_[i];
@@ -600,29 +556,24 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
             if (enqueue_ntb_precise(bd, ntbs_[k++], n, s, cnt)) return -1;
             continue;
         }
-        if (bd.se_type != 0) {
-            ARA_CUDA_OK(launch_pdl(se_f32_kernel, dim3(n), dim3(256), 0, s, d_xf[in], d_xs[in], w.se_w1t, w.se_w2t, w.se_b, w.se_b1,
-                                   bd.se_type, bd.gate, (bd.flags & kBlobShortcutPreSe) ? 1 : 0));
-            ++launches;
-        }
-        if (conv_layer_launch(&w.conv1, n, s)) return -1;
+        if (bd.se_type != 0 && launch(se_f32_kernel, dim3(n), dim3(256), 0, s, d_xf[in], d_xs[in], w.se_w1t, w.se_w2t, w.se_b, w.se_b1,
+                                      bd.se_type, bd.gate, (bd.flags & kBlobShortcutPreSe) ? 1 : 0))
+            return -1;
+        if (launch_conv(w.conv1, n, s)) return -1;
         const long long total = static_cast<long long>(n) * 64 * bd.c_op;
         const int grid = static_cast<int>((total + 255) / 256);
         const int cp = round_up(bd.c_op, 64);
-        if (bd.kernel == 3)
-            ARA_CUDA_OK(launch_pdl(dwconv_f32_kernel<3>, dim3(grid), dim3(256), 0, s, d_h1f, w.wd, w.bd, d_h2s, n, bd.c_op, cp));
-        else
-            ARA_CUDA_OK(launch_pdl(dwconv_f32_kernel<5>, dim3(grid), dim3(256), 0, s, d_h1f, w.wd, w.bd, d_h2s, n, bd.c_op, cp));
-        if (conv_layer_launch(&w.conv2, n, s)) return -1;
-        launches += 3;
+        if (launch(bd.kernel == 3 ? dwconv_f32_kernel<3> : dwconv_f32_kernel<5>, dim3(grid), dim3(256), 0, s, d_h1f, w.wd, w.bd, d_h2s, n,
+                   bd.c_op, cp))
+            return -1;
+        if (launch_conv(w.conv2, n, s)) return -1;
     }
     const float* xfinal = d_xf[hdr.n_blocks & 1];
     ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
-    ARA_CUDA_OK(launch_pdl(value_head_kernel<float>, dim3(n), dim3(256), value_head_smem<float>(), s, xfinal, vw, io_value[io], io_aux[io], cnt));
-    if (conv_layer_launch(&pol_conv1, n, s, cnt)) return -1;
-    if (conv_layer_launch(&pol_conv2, n, s, cnt)) return -1;
-    ARA_CUDA_OK(launch_pdl(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt));
-    launches += 4;
+    if (launch(value_head_kernel<float>, dim3(n), dim3(256), value_head_smem<float>(), s, xfinal, vw, io_value[io], io_aux[io], cnt) ||
+        launch_conv(pol_conv1, n, s, cnt) || launch_conv(pol_conv2, n, s, cnt) ||
+        launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt))
+        return -1;
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -630,27 +581,24 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
 // y = patch_embed(x); q|k|v; attention; y1 = y + proj(attention); z = projection(y1); z2 = z + conv1x1(relu(group
 // conv(z))); x' = x2 + mlp2(relu(mlp1(x2))) with x2 = y1 | z2 -- 9 launches, next_vit_official_modules.py:321-335
 int Net::enqueue_ntb_half(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* cnt) {
-    if (conv_layer_launch(&L.pe, n, s, cnt) || conv_layer_launch(&L.qkv, n, s, cnt)) return -1;
-    ARA_CUDA_OK(launch_pdl(ntb_attention_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(128), 0, s, d_qkv, d_att, bd.ntb_m, cnt));
-    if (conv_layer_launch(&L.proj, n, s, cnt) || conv_layer_launch(&L.prj, n, s, cnt) || conv_layer_launch(&L.gc, n, s, cnt) ||
-        conv_layer_launch(&L.mh, n, s, cnt) || conv_layer_launch(&L.mlp1, n, s, cnt) || conv_layer_launch(&L.mlp2, n, s, cnt))
+    if (launch_conv(L.pe, n, s, cnt) || launch_conv(L.qkv, n, s, cnt) ||
+        launch(ntb_attention_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(128), 0, s, d_qkv, d_att, bd.ntb_m, cnt) ||
+        launch_conv(L.proj, n, s, cnt) || launch_conv(L.prj, n, s, cnt) || launch_conv(L.gc, n, s, cnt) || launch_conv(L.mh, n, s, cnt) ||
+        launch_conv(L.mlp1, n, s, cnt) || launch_conv(L.mlp2, n, s, cnt))
         return -1;
-    launches += 9;
     return 0;
 }
 
 // the same in split form: fp32 activations, the split operand of every GEMM in its own buffer, one fp32 -> split
 // conversion of x2 -- 10 launches
 int Net::enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* cnt) {
-    if (conv_layer_launch(&L.pe, n, s, cnt) || conv_layer_launch(&L.qkv, n, s, cnt)) return -1;
-    ARA_CUDA_OK(launch_pdl(ntb_attention_f32_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(64), 0, s, d_qkvf, d_atts, bd.ntb_m,
-                           round_up(bd.ntb_m, 64), cnt));
-    if (conv_layer_launch(&L.proj, n, s, cnt) || conv_layer_launch(&L.prj, n, s, cnt) || conv_layer_launch(&L.gc, n, s, cnt) ||
-        conv_layer_launch(&L.mh, n, s, cnt))
+    if (launch_conv(L.pe, n, s, cnt) || launch_conv(L.qkv, n, s, cnt) ||
+        launch(ntb_attention_f32_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(64), 0, s, d_qkvf, d_atts, bd.ntb_m, round_up(bd.ntb_m, 64),
+               cnt) ||
+        launch_conv(L.proj, n, s, cnt) || launch_conv(L.prj, n, s, cnt) || launch_conv(L.gc, n, s, cnt) || launch_conv(L.mh, n, s, cnt) ||
+        launch(f32_to_split256_kernel, dim3(n * 64), dim3(256), 0, s, d_x2f, d_x2s, cnt) || launch_conv(L.mlp1, n, s, cnt) ||
+        launch_conv(L.mlp2, n, s, cnt))
         return -1;
-    ARA_CUDA_OK(launch_pdl(f32_to_split256_kernel, dim3(n * 64), dim3(256), 0, s, d_x2f, d_x2s, cnt));
-    if (conv_layer_launch(&L.mlp1, n, s, cnt) || conv_layer_launch(&L.mlp2, n, s, cnt)) return -1;
-    launches += 10;
     return 0;
 }
 
@@ -662,29 +610,21 @@ int Net::stem_device(int n, cudaStream_t s, const int* cnt, int io) {
 
 int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, bool stem_done) {
     if (precision == 1) return enqueue_precise(n, s, from_f32, cnt, io);
-    if (from_f32) {
-        ARA_CUDA_OK(launch_pdl(nchw_f32_to_nhwc_f16_kernel, dim3(n), dim3(256), hdr.in_channels * 65 * 4, s, d_in_f32, io_in_h[io], hdr.in_channels, cin_pad));
-        ++launches;
-    }
-    if (!stem_done) {
-        if (conv_layer_launch(io ? &stem_conv2 : &stem_conv, n, s, cnt)) return -1;
-        ++launches;
-    }
+    if (from_f32 && launch(nchw_f32_to_nhwc_f16_kernel, dim3(n), dim3(256), hdr.in_channels * 65 * 4, s, d_in_f32, io_in_h[io],
+                           hdr.in_channels, cin_pad))
+        return -1;
+    if (!stem_done && launch_conv(io ? stem_conv2 : stem_conv, n, s, cnt)) return -1;
     {   // two input / output sets = a search with Threads = 2: the tower is the first kernel of this stream's chain and
         // must not sit on its SMs waiting for the tree stream's event (see PdlSuspend); the small kernels behind it keep
         // their programmatic launches (the tower triggers them at its last block)
         PdlSuspend no_pdl(io_in_h[1] != nullptr);
-        if (rise_trunk_launch(trunks_[0].get(), n, s, cnt, (io == 1 && d_x0_alt != nullptr) ? d_x0_alt : nullptr)) return -1;
+        if (launch_tower(0, n, s, cnt, (io == 1 && d_x0_alt != nullptr) ? d_x0_alt : nullptr)) return -1;
     }
-    ++launches;
     // AlphaVile: NTB, tower segment, NTB, ... (the blob reader refuses an NTB at block 0)
     for (size_t seg = 1, k = 0, i = 0; i < blocks.size(); ++i) {
         if (!blocks[i].ntb) continue;
         if (enqueue_ntb_half(blocks[i], ntbs_[k++], n, s, cnt)) return -1;
-        if (i + 1 < blocks.size() && !blocks[i + 1].ntb) {
-            if (rise_trunk_launch(trunks_[seg++].get(), n, s, cnt)) return -1;
-            ++launches;
-        }
+        if (i + 1 < blocks.size() && !blocks[i + 1].ntb && launch_tower(seg++, n, s, cnt)) return -1;
     }
     __half* xfinal = d_x[1];
     ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
@@ -692,12 +632,12 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
     ARA_CUDA_OK(cudaEventRecord(ev_fork, s));
     ARA_CUDA_OK(cudaStreamWaitEvent(head_stream, ev_fork, 0));
     value_head_kernel<__half><<<dim3(n), dim3(256), value_head_smem<__half>(), head_stream>>>(xfinal, vw, io_value[io], io_aux[io], cnt);
+    ++launches;
     ARA_CUDA_OK(cudaEventRecord(ev_join, head_stream));
-    if (conv_layer_launch(&pol_conv1, n, s, cnt)) return -1;
-    if (conv_layer_launch(&pol_conv2, n, s, cnt)) return -1;
-    ARA_CUDA_OK(launch_pdl(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt));
+    if (launch_conv(pol_conv1, n, s, cnt) || launch_conv(pol_conv2, n, s, cnt) ||
+        launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt))
+        return -1;
     ARA_CUDA_OK(cudaStreamWaitEvent(s, ev_join, 0));
-    launches += 4;
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -717,7 +657,7 @@ int Net::forward_device(int n, cudaStream_t s, const int* cnt, int io, bool stem
     const int gk = stem_done ? 4 + io : (io == 1 ? 3 : (cnt != nullptr ? 2 : 0));
     const int*& baked = baked_[gk];
     if ((gk >= 3 || cnt != nullptr) && cnt != baked) {  // graphs captured with another counter are of no use
-        for (auto& g : graphs_[gk]) cudaGraphExecDestroy(g.second);
+        for (auto& g : graphs_[gk]) cudaGraphExecDestroy(g.second.exec);
         graphs_[gk].clear();
         baked = cnt;
     }
@@ -730,7 +670,7 @@ int Net::forward_from_f32_device(int n, cudaStream_t s) {
 }
 
 // The forward as one launch of graph family `family`'s graph for n boards.  The first forward of a size runs eagerly as a
-// warm-up and is then captured; the launches of the capture are not counted.
+// warm-up and is then captured; the launches the capture enqueued are counted at each replay instead.
 int Net::launch_graph(int family, int n, cudaStream_t s, bool from_f32, const int* cnt, int io, bool stem_done) {
     auto& graphs = graphs_[family];
     auto it = graphs.find(n);
@@ -740,12 +680,13 @@ int Net::launch_graph(int family, int n, cudaStream_t s, bool from_f32, const in
         const long long before = launches;
         cudaGraphExec_t ge;
         const int rc = capture_graph(s, &ge, [&] { return enqueue(n, s, from_f32, cnt, io, stem_done); });
+        const long long captured = launches - before;
         launches = before;
         if (rc) return -1;
-        it = graphs.emplace(n, ge).first;
+        it = graphs.emplace(n, Captured{ge, captured}).first;
     }
-    ARA_CUDA_OK(cudaGraphLaunch(it->second, s));
-    launches += kernels_per_forward(from_f32) - (stem_done ? 1 : 0);
+    ARA_CUDA_OK(cudaGraphLaunch(it->second.exec, s));
+    launches += it->second.launches;
     return 0;
 }
 
@@ -755,19 +696,6 @@ int Net::trunk_cycles(unsigned long long* out32) {
     ARA_CUDA_OK(cudaStreamSynchronize(stream));
     ARA_CUDA_OK(cudaMemcpy(out32, trunks_[0]->d_prof, 32 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return 0;
-}
-
-int Net::kernels_per_forward(bool from_f32) const {
-    int k = from_f32 ? 1 : 0;
-    k += 1;  // stem
-    if (precision == 0) {
-        k += static_cast<int>(trunks_.size());  // the tower kernel per segment
-        for (const auto& b : blocks) k += b.ntb ? 9 : 0;
-    } else {
-        for (const auto& b : blocks) k += b.ntb ? 10 : 3 + (b.se_type != 0 ? 1 : 0);
-    }
-    k += 4;  // value head, policy conv x2, softmax
-    return k;
 }
 
 int Net::predict(const float* planes_host, int n, float* value_host, float* prob_host, float* aux_host) {

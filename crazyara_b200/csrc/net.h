@@ -46,9 +46,24 @@ struct NtbLayers {
 // Precision float32: one bottleneck block as separate launches on fp32 activations (net.cu, conv_gemm.cuh)
 struct PreciseBlock {
     float *se_w1t = nullptr, *se_w2t = nullptr, *se_b = nullptr, *se_b1 = nullptr;
-    __half *w1 = nullptr, *w2 = nullptr;  // operand-split weights [rows][3 * cw] per tap: hi | lo | hi
-    float *b1 = nullptr, *wd = nullptr, *bd = nullptr, *b2 = nullptr;
+    float *wd = nullptr, *bd = nullptr;
     ConvLayer conv1, conv2;
+};
+
+// Where one conv_gemm layer (conv_gemm.cuh) reads and writes.  act: the activations, rows act_pitch channels apart (0:
+// act_cin); float16 reads channels 0 .. act_cin (0: the layer's cin), float32 the split [.., 3 * ceil64(cin)].  The
+// epilogue adds the fp16 or fp32 residual (rows ldr apart) and writes columns 0 .. n_end (0: ldo) of the fp16, fp32 and /
+// or split outputs (rows ldo apart, split parts split_cs wide).
+struct ConvIo {
+    const __half* act = nullptr;
+    int act_cin = 0, act_pitch = 0;
+    const __half* res_h = nullptr;
+    const float* res_f = nullptr;
+    int ldr = 0;
+    __half* out_h = nullptr;
+    float* out_f = nullptr;
+    __half* out_s = nullptr;
+    int ldo = 0, n_end = 0, split_cs = 0;
 };
 
 // the tensors of a weight blob, host side, in blob order (weights.py)
@@ -105,7 +120,6 @@ class Net {
     int ldp = 0;  // padded policy channels (multiple of 32)
     int n_labels() const { return hdr.policy_channels * 64; }
     int n_aux() const { return hdr.wdl_mode ? 4 : 0; }
-    int kernels_per_forward(bool from_f32) const;
     int trunk_cycles(unsigned long long* out32);  // -DARA_TRUNK_PROF builds: per-role cycle counters of CTA 0 (first segment)
     cudaStream_t stream = nullptr;
     // the value head runs beside the policy head: forked side stream, joined before the forward ends
@@ -142,8 +156,14 @@ class Net {
     int read_blob(const char* blob_path, HostWeights* hw);
     int build_half(const HostWeights& hw);
     int build_precise(const HostWeights& hw);
+    int build_conv(ConvLayer* L, const std::vector<float>& w, const std::vector<float>& bias, int n_out, int cin, int ksize,
+                   int relu, const ConvIo& io);
     int upload_value_head(const HostWeights& hw);
-    int upload_policy_bias(const HostWeights& hw, int rows);
+    // the kernel launches of a forward, each counted in `launches`
+    template <typename... KArgs, typename... Args>
+    int launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args);
+    int launch_conv(const ConvLayer& L, int n, cudaStream_t s, const int* boards_dev = nullptr);
+    int launch_tower(size_t segment, int n, cudaStream_t s, const int* boards_dev, const __half* x_in = nullptr);
     int enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io);
     int launch_graph(int family, int n, cudaStream_t s, bool from_f32, const int* boards_dev, int io, bool stem_done);
     int build_ntb_half(const BlockDesc& bd, const HostBlock& hb, NtbLayers* L);
@@ -152,8 +172,6 @@ class Net {
     int enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* boards_dev);
     DeviceBuffers mem_;
     int max_cop_ = 0;
-    __half* stem_w = nullptr;
-    float* stem_b = nullptr;
     ConvLayer stem_conv;
     ConvLayer stem_conv2;  // the stem reading the second input set
     std::vector<PreciseBlock> pb_;
@@ -168,13 +186,14 @@ class Net {
     __half *d_ys = nullptr, *d_atts = nullptr, *d_zs = nullptr, *d_gs = nullptr, *d_x2s = nullptr, *d_hs = nullptr;
     float *vh_wv = nullptr, *vh_bv = nullptr, *vh_w1t = nullptr, *vh_b1 = nullptr, *vh_w2 = nullptr, *vh_b2 = nullptr;
     float *vh_wdl_w = nullptr, *vh_wdl_b = nullptr, *vh_plys_w = nullptr, *vh_plys_b = nullptr;
-    __half *pol_w1 = nullptr, *pol_w2 = nullptr;
-    float *pol_b1 = nullptr, *pol_b2 = nullptr;
     ConvLayer pol_conv1, pol_conv2;
-    std::map<int, cudaGraphExec_t> graphs_[6];  // plain, from fp32 input, with a device-side count (io 0), the same for io 1
-    const int* baked_[6] = {};                  // the counter pointer each graph family was captured with
-    int upload_conv_w(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows);
-    int upload_conv_w_split(const float* w, int n_out, int cin, int ksize, __half** dst, int* rows);
+    struct Captured {
+        cudaGraphExec_t exec;
+        long long launches;  // the kernel launches the capture enqueued
+    };
+    std::map<int, Captured> graphs_[6];  // plain, from fp32 input, with a device-side count (io 0), the same for io 1
+    const int* baked_[6] = {};           // the counter pointer each graph family was captured with
+    int upload_conv_w(const float* w, int n_out, int cin, int ksize, int parts, __half** dst);
     int upload_f32(const float* src, size_t count, size_t padded, float** dst);
 };
 

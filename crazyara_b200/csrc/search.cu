@@ -360,6 +360,7 @@ class Search {
     // one iteration as a CUDA graph
     bool iter_warm_ = false;
     cudaGraphExec_t iter_graph_ = nullptr;
+    long long iter_net_launches_ = 0;  // the network's kernel launches inside iter_graph_
     cudaStream_t side_stream_ = nullptr;  // second branch of an iteration (value backups)
     cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
     int enqueue_iteration(bool with_events);
@@ -803,12 +804,15 @@ int Search::iterate(int count) {
     for (int it = 0; it < count; ++it) {
         if (!profile && iter_graph_ != nullptr) {
             ARA_CUDA_OK(cudaGraphLaunch(iter_graph_, stream_));
-            if (net_) net_->launches += net_->kernels_per_forward(false);
+            if (net_) net_->launches += iter_net_launches_;
         } else if (!profile && iter_warm_) {
             // second iteration of the handle's life (the first one ran eagerly and warmed the network's graph up)
             const long long net_before = net_ ? net_->launches : 0;
             const int rc = capture_graph(stream_, &iter_graph_, [&] { return enqueue_iteration(false); });
-            if (net_) net_->launches = net_before;
+            if (net_) {
+                iter_net_launches_ = net_->launches - net_before;
+                net_->launches = net_before;
+            }
             if (rc) return -1;
             --it;  // nothing ran yet: launch the graph in the next pass
             continue;

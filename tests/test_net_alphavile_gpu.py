@@ -143,7 +143,8 @@ def test_alphavile_packed_two_tree_search_equals_single_tree_searches(av_net):
 @pytest.mark.parametrize("precision", ["float16", "float32"])
 def test_alphavile_launch_bookkeeping_matches_the_launches(av_net, precision):
     """The first forward of a size runs eagerly (every launch counted) before it is captured; a graph replay then adds
-    kernels_per_forward.  Both must agree: per NTB 9 launches in float16 (10 in float32), one tower launch per segment."""
+    the launches its capture enqueued.  Both must agree with the layer plan: per NTB 9 launches in float16 (10 in
+    float32), one tower launch per segment."""
     net, arch, _ = av_net("normal", 4, precision)
     x = golden_input(arch, n=4, seed=25)
     _predict(net, arch, x, 4)

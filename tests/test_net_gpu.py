@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from oracle import net as onet
+from oracle import net_mx
 from tests.golden.gen_net_golden import golden_input
 
 VALUE_ATOL = 4e-3
@@ -92,6 +93,35 @@ def test_net_predict_float32_within_1e4_of_oracle(tmp_path, name, cin, pch, batc
     net.predict(xin, value2, prob2, None, n=n)
     assert np.array_equal(value2[:n], value[:n]) and np.array_equal(prob2[:n], prob[:n])
     net.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["float16", "float32"])
+@pytest.mark.parametrize("name", ["risev33", "mx_risev2"])
+def test_launch_bookkeeping_matches_the_launches(tmp_path, name, precision):
+    """The first forward of a size runs eagerly (every launch counted) before it is captured; a graph replay then adds
+    the launches its capture enqueued.  Both must agree with the layer plan: input conversion, stem, the tower kernel
+    (float16) or per block the squeeze-excitation if any, conv1, depthwise and conv2 (float32), value head, two policy
+    convolutions, softmax.  (AlphaVile: tests/test_net_alphavile_gpu.py)"""
+    from crazyara_b200.nn import NeuralNetAPI
+    from crazyara_b200.weights import export_mx_blob
+    if name == "risev33":
+        arch = onet.arch_risev33(52, 76, True)
+        net, _ = _make_net(tmp_path, arch, 4, 30, precision)
+    else:
+        arch = net_mx.arch_mx_risev2(34, 81)
+        blob = export_mx_blob(net_mx.make_mx_params(arch, 7), arch, str(tmp_path / f"{name}.arab"), input_version=10)
+        net = NeuralNetAPI("gpu", 0, 4, blob, precision=precision)
+    x = golden_input(arch, n=4, seed=25)
+    v, p = np.zeros(4, np.float32), np.zeros((4, arch["policy_channels"] * 64), np.float32)
+    net.predict(x, v, p, None, n=4)
+    first = net.launch_count()
+    net.predict(x, v, p, None, n=4)
+    per_forward = net.launch_count() - first
+    net.close()
+    assert first == 2 * per_forward
+    tower = 1 if precision == "float16" else sum(3 + (se is not None) for se in arch["se_types"])
+    assert per_forward == 1 + 1 + tower + 4
 
 
 @pytest.mark.gpu
