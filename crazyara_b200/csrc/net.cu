@@ -604,8 +604,7 @@ int Net::enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cud
 
 int Net::stem_device(int n, cudaStream_t s, const int* cnt, int io) {
     if (!stem_splittable() || io < 0 || io > 1) return set_error("stem_device: needs Precision float16 and two input / output sets");
-    if (conv_layer_launch(io ? &stem_conv2 : &stem_conv, n, s, cnt)) return -1;
-    return 0;  // (the caller counts the launch: it may sit in a captured graph)
+    return launch_conv(io ? stem_conv2 : stem_conv, n, s, cnt);
 }
 
 int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, bool stem_done) {

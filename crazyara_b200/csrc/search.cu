@@ -9,7 +9,7 @@
 //   network  wgmma conv stack (CUDA graph), or the hash-derived fake backend for search-parity tests
 //   update   scatter priors / values into the new nodes, prepare their next children, backups, collision reverts
 // Threads = 1: all on one stream.  Threads = 2: the two logical threads' tree kernels on one stream in the fixed schedule
-// of oracle/mcts.h, their forwards on a second stream (enqueue_slot).  The host only looks at the per-tree `done` flag
+// of oracle/mcts.h, their forwards on a second stream (enqueue_turn).  The host only looks at the per-tree `done` flag
 // once per chunk of iterations.
 // This translation unit is compiled with -fmad=false: the PUCT / Q arithmetic must round exactly like the
 // reference's (and the oracle's) scalar C++ code.
@@ -332,15 +332,14 @@ class Search {
     ~Search();
     int init(Net* net, const SearchParams& sp, int device, int n_trees, int max_nodes);
     int set_position(int tree, const Board& root, const uint64_t* hist_keys, const int16_t* hist_reps, int hist_len);
+    int set_limits(int tree, unsigned simulations, unsigned nodes);
     int go();
-    int apply_move(int tree, unsigned short move);
-    void request_stop() { stop_requested_.store(true, std::memory_order_relaxed); }
-    int fetch_results();
     int begin();
     int step(int n_batches);
-    int poll_running();
+    int fetch_results();
+    int apply_move(int tree, unsigned short move);
     int node_view(int tree, int node_id, NodeView* out);
-    NodeView* d_node_view_ = nullptr;
+    void request_stop() { stop_requested_.store(true, std::memory_order_relaxed); }
     int debug_cycles(int tree, unsigned long long* out8) {
         TreeState st;
         ARA_CUDA_OK(cudaMemcpy(&st, d_states_[tree], sizeof(st), cudaMemcpyDeviceToHost));
@@ -350,68 +349,38 @@ class Search {
     SearchParams sp{};
     int n_trees = 0;
     std::vector<SearchResult> results;
-    long long launches = 0;
+    long long launches = 0;  // kernels launched so far, each counted by launch() (bench bookkeeping)
+    long long compactions = 0;
+    long long net_forwards = 0;
     double last_go_ms = 0.0;
     double movetime_ms = 0.0;  // > 0: stop issuing iterations once this much wall time has passed (UCI `go movetime`)
     // ThreadManager heuristics (time_manager.h): parameters, and what happened in the last go
     bool use_tc = false;
     ara_time_control_t tc{};
     ara_time_report_t tr{};
-    // one iteration as a CUDA graph
-    bool iter_warm_ = false;
-    cudaGraphExec_t iter_graph_ = nullptr;
-    long long iter_net_launches_ = 0;  // the network's kernel launches inside iter_graph_
-    cudaStream_t side_stream_ = nullptr;  // second branch of an iteration (value backups)
-    cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
-    int enqueue_iteration(bool with_events);
-    // ---- Threads = 2 (sp.threads): two logical search threads per tree, each with its own batch state ("slot": views
-    // of the trees with their own new-leaf / trajectory arrays, their own rows of the network's second input / output
-    // set).  The tree kernels of both threads run on stream_ in the fixed order
-    //     S0 S1 | U0 S0 U1 S1 | U0 S0 ...     (S = select + pack + expand, U = scatter + prepare || backup)
-    // and each thread's network forward on net_stream_, between its S and its next U: while one thread's batch is at
-    // the network the other thread selects.  (oracle/mcts.h describes the schedule; tests compare all three.)
-    int threads_ = 1;
-    bool eps_ = false;  // epsilon-greedy / epsilon-check exploration on: the select_kernel<true> instantiation
-    bool wave_ = false;  // few trees: select_wave_kernel (several warps per tree) instead of one warp per tree
-    void launch_select(const TreeDev* trees, int* count = nullptr) {
-        if (eps_) select_kernel<true><<<n_trees, 32, 0, stream_>>>(trees, sp, count);
-        else if (wave_) select_wave_kernel<<<n_trees, 32 * kWaveWarps, kWaveSmemBytes, stream_>>>(trees, sp, count);
-        else select_kernel<false><<<n_trees, 32, 0, stream_>>>(trees, sp, count);
-    }
-    bool primed_ = false;                  // S0 S1 of the current go have been enqueued
-    TreeDev* d_trees_slot_[2] = {nullptr, nullptr};
-    std::vector<TreeDev> h_trees1_;        // slot 1 views (h_trees_ = slot 0); their batch arrays are slot 1's own
-    // node-pool compaction: the second set of pools per tree (allocated at the first compaction), scan scratch
-    std::vector<TreeDev> shadow_;
-    std::vector<char> advanced_;           // ara_search_apply_move since the last go
-    CompactInfo* d_cinfo_ = nullptr;
-    int* d_keep_n_ = nullptr;
-    int* d_keep_e_ = nullptr;
-    int* d_ctotal_ = nullptr;
-    long long compactions = 0;
-    int compact_pools();
-    int* d_count_slot_[2] = {nullptr, nullptr};
-    float *d_values_slot_[2] = {nullptr, nullptr}, *d_probs_slot_[2] = {nullptr, nullptr};  // fake backend, per slot
-    cudaStream_t net_stream_ = nullptr;
-    cudaEvent_t ev_sel_[2] = {nullptr, nullptr}, ev_net_[2] = {nullptr, nullptr};
-    cudaGraphExec_t slot_graph_[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [slot][with update]
-    bool slot_warm_ = false;
-    int enqueue_slot(int slot, bool with_update);
-    int enqueue_slot_tree_ops(int slot, bool with_update);
-    int iterate2(int cycles);
-    std::vector<uint2> h_limits_;  // per tree {simulations, nodes} of the next go
-    uint2* d_limits_ = nullptr;
-    int set_limits(int tree, unsigned simulations, unsigned nodes);
-    int* d_count_ = nullptr;  // multi-tree searches: rows of the network batch in use (written by pack_kernel)
-    RootTimeStats* d_tstats_ = nullptr;
-    RootTimeStats* h_tstats_ = nullptr;  // pinned
-    int read_time_stats(RootStatsHost* out);
     // per-phase device times of the last go (CUDA events on the search stream), filled when profile is on
     bool profile = false;
     double select_ms = 0.0, net_ms = 0.0, apply_ms = 0.0;
-    long long net_forwards = 0;
 
    private:
+    // One logical search thread: its views of the trees (with their own new-leaf / trajectory arrays), the row count of
+    // its batch, and where that batch goes: a network input / output set, or the fake backend's buffers.  Threads = 1
+    // uses slot 0 only.
+    struct Slot {
+        std::vector<TreeDev> h_trees;  // slot 0: the trees; slot 1: the same pools with its own batch arrays
+        TreeDev* d_trees = nullptr;
+        int* d_count = nullptr;  // rows of the network batch in use (pack_kernel; Threads = 2 with one tree: select)
+        __half* in_h = nullptr;  // the network's input rows (nullptr: fake backend)
+        float *values = nullptr, *probs = nullptr;
+        int io = 0;  // the network's input / output set
+        cudaEvent_t ev_sel = nullptr, ev_net = nullptr;  // Threads = 2: batch selected (tree stream), evaluated (network stream)
+    };
+    // a captured iteration or turn, and the launches its capture enqueued
+    struct Captured {
+        cudaGraphExec_t exec = nullptr;
+        long long search_launches = 0, net_launches = 0;
+    };
+
     // The arrays of TreeDev, listed once: f(member, length) for each.  A tree's node, edge and prepared-child pools
     // (the compaction swaps them for its second set) ...
     template <typename F>
@@ -440,18 +409,74 @@ class Search {
         for_each_batch_array([&](auto m, size_t n) { rc = rc ? rc : mem_.dalloc(&(t.*m), n); });
         return rc;
     }
+    // a plain kernel launch (the graph node `<<<>>>` makes), counted in `launches`
+    template <typename... KArgs, typename... Args>
+    int launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
+        const cudaLaunchConfig_t cfg = {grid, block, smem, s, nullptr, 0};
+        ARA_CUDA_OK(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
+        ++launches;
+        return 0;
+    }
+    int launch_select(const Slot& s, int* count) {
+        if (eps_) return launch(select_kernel<true>, n_trees, 32, 0, stream_, s.d_trees, sp, count);
+        if (wave_) return launch(select_wave_kernel, n_trees, 32 * kWaveWarps, kWaveSmemBytes, stream_, s.d_trees, sp, count);
+        return launch(select_kernel<false>, n_trees, 32, 0, stream_, s.d_trees, sp, count);
+    }
+    // the new leaves of slot s: (many trees) packed into consecutive rows, then expanded, their planes in its input rows
+    int pack_expand(const Slot& s) {
+        const int B = sp.batch_size;
+        if (n_trees > 1 && launch(pack_kernel, 1, 32, 0, stream_, s.d_trees, n_trees, s.d_count)) return -1;
+        return launch(expand_kernel, n_trees * B, 32, 0, stream_, s.d_trees, sp, B, s.in_h, cin_pad_, split_);
+    }
+    int evaluate(const Slot& s, int rows, cudaStream_t stream, const int* count, bool stem_done);
+    template <typename F>
+    int run_captured(Captured& g, F&& enqueue);
+    int enqueue_iteration(bool with_events);
+    int enqueue_turn_tree_ops(const Slot& s, bool with_update);
+    int enqueue_turn(int k, bool with_update);
     int iterate(int count);
+    int compact_pools();
+    int poll_running();
+    int read_time_stats(RootStatsHost* out);
+    cudaEvent_t prof_event();
+    int prof_collect();
+
     Net* net_ = nullptr;
+    int device_ = 0;
+    int threads_ = 1;
+    bool eps_ = false;   // epsilon-greedy / epsilon-check exploration on: the select_kernel<true> instantiation
+    bool wave_ = false;  // few trees: select_wave_kernel (several warps per tree) instead of one warp per tree
     bool searched_ = false;  // a go has run: the device holds trees that apply_move may keep
     // UCI `stop` (SearchThread::stop): set from another host thread while go() runs; go() leaves its loop at the next poll
     std::atomic<bool> stop_requested_{false};
-    int device_ = 0;
+    int max_nodes_ = 0, max_edges_ = 0, n_labels_ = 0, hist_cap_ = 512;
+    int cin_pad_ = 0, split_ = 0;  // the network input's rows (expand_kernel)
+    DeviceBuffers mem_;
+    Slot slots_[2];
     cudaStream_t stream_ = nullptr;
     bool own_stream_ = false;
-    int max_nodes_ = 0, max_edges_ = 0, n_labels_ = 0, hist_cap_ = 512;
-    DeviceBuffers mem_;
-    std::vector<TreeDev> h_trees_;
-    TreeDev* d_trees_ = nullptr;
+    // ---- Threads = 2 (sp.threads): two logical search threads per tree, each with its own slot.  The tree kernels of
+    // both threads run on stream_ in the fixed order
+    //     S0 S1 | U0 S0 U1 S1 | U0 S0 ...     (S = select + pack + expand, U = scatter + prepare || backup)
+    // and each thread's network forward on net_stream_, between its S and its next U: while one thread's batch is at
+    // the network the other thread selects.  (oracle/mcts.h describes the schedule; tests compare all three.)
+    cudaStream_t net_stream_ = nullptr;
+    bool primed_ = false;  // S0 S1 of the current go have been enqueued
+    // Threads = 1 with one tree: the second branch of an iteration (value backups)
+    cudaStream_t side_stream_ = nullptr;
+    cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
+    bool warm_ = false;  // iterations and turns may be captured from now on (run_captured)
+    Captured iter_graph_;        // Threads = 1: an iteration
+    Captured turn_graph_[2][2];  // Threads = 2: a turn [slot][with update]
+    // node-pool compaction: the second set of pools per tree (allocated at the first compaction), scan scratch
+    std::vector<TreeDev> shadow_;
+    std::vector<char> advanced_;  // ara_search_apply_move since the last go
+    CompactInfo* d_cinfo_ = nullptr;
+    int* d_keep_n_ = nullptr;
+    int* d_keep_e_ = nullptr;
+    int* d_ctotal_ = nullptr;
+    std::vector<uint2> h_limits_;  // per tree {simulations, nodes} of the next go
+    uint2* d_limits_ = nullptr;
     Board* d_roots_ = nullptr;
     std::vector<Board> h_roots_;
     std::vector<TreeState*> d_states_;
@@ -459,14 +484,14 @@ class Search {
     std::vector<int16_t*> d_hist_reps_;
     float* d_lut_ = nullptr;
     double* d_sqrt_lut_ = nullptr;
-    float *d_values_ = nullptr, *d_probs_ = nullptr;  // fake backend buffers
     SearchResult* d_results_ = nullptr;
+    NodeView* d_node_view_ = nullptr;
+    RootTimeStats* d_tstats_ = nullptr;
+    RootTimeStats* h_tstats_ = nullptr;  // pinned
     int* h_done_ = nullptr;  // pinned
     cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
     std::vector<cudaEvent_t> prof_events_;
     size_t prof_used_ = 0;
-    cudaEvent_t prof_event();
-    int prof_collect();
 };
 
 cudaEvent_t Search::prof_event() {
@@ -509,15 +534,15 @@ Search::~Search() {
     if (stream_) cudaStreamSynchronize(stream_);
     if (h_done_) cudaFreeHost(h_done_);
     if (h_tstats_) cudaFreeHost(h_tstats_);
-    if (iter_graph_) cudaGraphExecDestroy(iter_graph_);
-    for (auto& a : slot_graph_)
-        for (auto g : a)
-            if (g) cudaGraphExecDestroy(g);
+    if (iter_graph_.exec) cudaGraphExecDestroy(iter_graph_.exec);
+    for (auto& a : turn_graph_)
+        for (auto& g : a)
+            if (g.exec) cudaGraphExecDestroy(g.exec);
     if (net_stream_) cudaStreamDestroy(net_stream_);
-    for (cudaEvent_t e : ev_sel_)
-        if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : ev_net_)
-        if (e) cudaEventDestroy(e);
+    for (Slot& s : slots_) {
+        if (s.ev_sel) cudaEventDestroy(s.ev_sel);
+        if (s.ev_net) cudaEventDestroy(s.ev_net);
+    }
     if (side_stream_) cudaStreamDestroy(side_stream_);
     if (ev_fork_) cudaEventDestroy(ev_fork_);
     if (ev_join_) cudaEventDestroy(ev_join_);
@@ -557,6 +582,7 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     if (wave_)
         ARA_CUDA_OK(cudaFuncSetAttribute(select_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kWaveSmemBytes)));
     n_labels_ = (sp.mode == MODE_CRAZYHOUSE ? 81 : (sp.mode == MODE_CHESS ? 76 : 84)) * 64;
+    Slot& s0 = slots_[0];
     if (net_ != nullptr) {
         if (net_->batch < n_trees * sp.batch_size)
             return set_error("ara_search_create: network batch %d < trees %d x Batch_Size %d", net_->batch, n_trees, sp.batch_size);
@@ -564,11 +590,13 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
             return set_error("ara_search_create: network shape (C=%d, L=%d) does not match mode/version (C=%d, L=%d)",
                              net_->hdr.in_channels, net_->n_labels(), planes_channels(sp.mode, sp.input_version), n_labels_);
         stream_ = net_->stream;
+        cin_pad_ = net_->cin_pad;
+        split_ = net_->precision;
     } else {
         ARA_CUDA_OK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
         own_stream_ = true;
-        if (mem_.dalloc(&d_values_, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
-        if (mem_.dalloc(&d_probs_, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
+        if (mem_.dalloc(&s0.values, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
+        if (mem_.dalloc(&s0.probs, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
     }
     if (max_nodes <= 0) {
         const unsigned budget = sp.simulations ? sp.simulations : (sp.nodes ? sp.nodes * 2 : 0);
@@ -598,14 +626,14 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         for (int i = 0; i < len; ++i) sq[i] = sqrt(static_cast<double>(i));
         if (mem_.dalloc(&d_sqrt_lut_, sq.size())) return -1;
         ARA_CUDA_OK(cudaMemcpy(d_sqrt_lut_, sq.data(), sq.size() * 8, cudaMemcpyHostToDevice));
-        h_trees_.resize(n_trees);
-        for (auto& t : h_trees_) t.cput_lut_len = len;
+        s0.h_trees.resize(n_trees);
+        for (auto& t : s0.h_trees) t.cput_lut_len = len;
     }
     d_states_.resize(n_trees);
     d_hist_keys_.resize(n_trees);
     d_hist_reps_.resize(n_trees);
     for (int i = 0; i < n_trees; ++i) {
-        TreeDev& t = h_trees_[i];
+        TreeDev& t = s0.h_trees[i];
         if (alloc_pools(t) || alloc_batch_arrays(t) || mem_.dalloc(&t.st, 1)) return -1;
         if (mem_.dalloc(&d_hist_keys_[i], hist_cap_) || mem_.dalloc(&d_hist_reps_[i], hist_cap_)) return -1;
         t.hist_keys = d_hist_keys_[i];
@@ -618,8 +646,8 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         t.slot_base = i * B;
         d_states_[i] = t.st;
     }
-    if (mem_.dalloc(&d_trees_, n_trees) || mem_.dalloc(&d_roots_, n_trees) || mem_.dalloc(&d_results_, n_trees) || mem_.dalloc(&d_limits_, n_trees) ||
-        mem_.dalloc(&d_tstats_, 1) || mem_.dalloc(&d_count_, 1) || mem_.dalloc(&d_node_view_, 1))
+    if (mem_.dalloc(&s0.d_trees, n_trees) || mem_.dalloc(&d_roots_, n_trees) || mem_.dalloc(&d_results_, n_trees) || mem_.dalloc(&d_limits_, n_trees) ||
+        mem_.dalloc(&d_tstats_, 1) || mem_.dalloc(&s0.d_count, 1) || mem_.dalloc(&d_node_view_, 1))
         return -1;
     h_limits_.assign(n_trees, make_uint2(sp.simulations, sp.nodes));
     for (int i = 0; i < n_trees; ++i) {  // the trees' Dirichlet generators (TreeState::rng)
@@ -630,35 +658,42 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         ARA_CUDA_OK(cudaMemcpy(d_states_[i]->crand_r, tmp.crand_r, sizeof(tmp.crand_r), cudaMemcpyHostToDevice));
         ARA_CUDA_OK(cudaMemcpy(&d_states_[i]->crand_f, &tmp.crand_f, sizeof(tmp.crand_f), cudaMemcpyHostToDevice));
     }
-    d_trees_slot_[0] = d_trees_;
     if (threads_ == 2) {
-        h_trees1_.resize(n_trees);
-        for (auto& t : h_trees1_)
+        Slot& s1 = slots_[1];
+        s1.io = 1;
+        s1.h_trees.resize(n_trees);
+        for (auto& t : s1.h_trees)
             if (alloc_batch_arrays(t)) return -1;
-        if (mem_.dalloc(&d_trees_slot_[1], n_trees)) return -1;
+        if (mem_.dalloc(&s1.d_trees, n_trees)) return -1;
         if (net_ != nullptr) {
             if (net_->enable_second_io()) return -1;
         } else {
-            d_values_slot_[0] = d_values_, d_probs_slot_[0] = d_probs_;
-            if (mem_.dalloc(&d_values_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
-            if (mem_.dalloc(&d_probs_slot_[1], static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
+            if (mem_.dalloc(&s1.values, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
+            if (mem_.dalloc(&s1.probs, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
         }
         // the network stream has the same (default) priority as the tree stream: neither yields to the other
         ARA_CUDA_OK(cudaStreamCreateWithFlags(&net_stream_, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; ++k) {
-            ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_sel_[k], cudaEventDisableTiming));
-            ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_net_[k], cudaEventDisableTiming));
+        for (Slot& s : slots_) {
+            ARA_CUDA_OK(cudaEventCreateWithFlags(&s.ev_sel, cudaEventDisableTiming));
+            ARA_CUDA_OK(cudaEventCreateWithFlags(&s.ev_net, cudaEventDisableTiming));
         }
-        if (mem_.dalloc(&d_count_slot_[1], 1)) return -1;
+        if (mem_.dalloc(&s1.d_count, 1)) return -1;
+    } else if (n_trees == 1) {
+        ARA_CUDA_OK(cudaStreamCreateWithFlags(&side_stream_, cudaStreamNonBlocking));
+        ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
+        ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_join_, cudaEventDisableTiming));
     }
+    if (net_ != nullptr)
+        for (int k = 0; k < threads_; ++k) {  // (set 0 is the network's own d_in_h / d_value / d_prob)
+            Slot& s = slots_[k];
+            s.in_h = net_->io_in_h[s.io];
+            s.values = net_->io_value[s.io];
+            s.probs = net_->io_prob[s.io];
+        }
     h_roots_.resize(n_trees);
     results.resize(n_trees);
     ARA_CUDA_OK(cudaMallocHost(&h_done_, sizeof(int) * n_trees));
     ARA_CUDA_OK(cudaMallocHost(&h_tstats_, sizeof(RootTimeStats)));
-    d_count_slot_[0] = d_count_;
-    ARA_CUDA_OK(cudaStreamCreateWithFlags(&side_stream_, cudaStreamNonBlocking));
-    ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
-    ARA_CUDA_OK(cudaEventCreateWithFlags(&ev_join_, cudaEventDisableTiming));
     ARA_CUDA_OK(cudaEventCreate(&ev0_));
     ARA_CUDA_OK(cudaEventCreate(&ev1_));
     return 0;
@@ -676,159 +711,135 @@ int Search::set_position(int tree, const Board& root, const uint64_t* hist_keys,
         ARA_CUDA_OK(cudaMemcpyAsync(d_hist_keys_[tree], hist_keys + skip, sizeof(uint64_t) * len, cudaMemcpyHostToDevice, stream_));
         ARA_CUDA_OK(cudaMemcpyAsync(d_hist_reps_[tree], hist_reps + skip, sizeof(int16_t) * len, cudaMemcpyHostToDevice, stream_));
     }
-    h_trees_[tree].hist_len = len;
+    slots_[0].h_trees[tree].hist_len = len;
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
+    return 0;
+}
+
+// The batch of slot s on `stream`: the network's forward of `rows` rows (count: their device-side number, or nullptr), or
+// the fake backend's values and priors of the new leaves.
+int Search::evaluate(const Slot& s, int rows, cudaStream_t stream, const int* count, bool stem_done) {
+    if (net_) return net_->forward_device(rows, stream, count, s.io, stem_done);
+    const int B = sp.batch_size;
+    return launch(fake_eval_kernel, n_trees * B, 128, 0, stream, s.d_trees, n_trees, B, s.values, s.probs, n_labels_);
+}
+
+// The tree kernels of one iteration (Threads = 1) or turn (Threads = 2) on stream_, enqueue().  They never change (same
+// pointers, same grids): outside profiling runs, once the handle is warm, they are captured at the first need and run as
+// ONE graph launch from then on -- a network forward among them becomes part of the graph, and the dependent-launch gaps
+// shrink to graph-edge latency.  Each replay counts the launches its capture enqueued, the search's and the network's.
+template <typename F>
+int Search::run_captured(Captured& g, F&& enqueue) {
+    if (profile || !warm_) return enqueue();
+    if (g.exec == nullptr) {
+        const long long search_before = launches, net_before = net_ ? net_->launches : 0;
+        const int rc = capture_graph(stream_, &g.exec, enqueue);
+        g.search_launches = launches - search_before;
+        launches = search_before;
+        if (net_) {
+            g.net_launches = net_->launches - net_before;
+            net_->launches = net_before;
+        }
+        if (rc) return -1;
+    }
+    ARA_CUDA_OK(cudaGraphLaunch(g.exec, stream_));
+    launches += g.search_launches;
+    if (net_) net_->launches += g.net_launches;
     return 0;
 }
 
 // One search iteration on the stream: select -> (pack) -> expand -> network -> scatter -> backup -> prepare.
 int Search::enqueue_iteration(bool with_events) {
-    __half* in_h = net_ ? net_->d_in_h : nullptr;
-    const int cpad = net_ ? net_->cin_pad : 0;
+    const Slot& s = slots_[0];
     const int B = sp.batch_size;
-    const float* values = net_ ? net_->d_value : d_values_;
-    const float* probs = net_ ? net_->d_prob : d_probs_;
     if (with_events) prof_event();
-    launch_select(d_trees_);
-    if (n_trees > 1) pack_kernel<<<1, 32, 0, stream_>>>(d_trees_, n_trees, d_count_);
-    expand_kernel<<<n_trees * B, 32, 0, stream_>>>(d_trees_, sp, B, in_h, cpad, net_ ? net_->precision : 0);
+    if (launch_select(s, nullptr) || pack_expand(s)) return -1;
     if (with_events) prof_event();
-    if (net_) {
-        if (net_->forward_device(n_trees * B, stream_, n_trees > 1 ? d_count_ : nullptr)) return -1;
-    } else {
-        fake_eval_kernel<<<n_trees * B, 128, 0, stream_>>>(d_trees_, n_trees, B, d_values_, d_probs_, n_labels_);
-    }
+    if (evaluate(s, n_trees * B, stream_, n_trees > 1 ? s.d_count : nullptr, false)) return -1;
     if (with_events) prof_event();
     // the value backups (one warp per tree, a latency chain) run beside scatter -> prepare: neither reads what the
     // other writes (backup_results); a second branch of the iteration graph
     if (n_trees > 1) {
-        update_kernel<<<n_trees + n_trees * 4 * B, 32, 0, stream_>>>(d_trees_, sp, n_trees, B, 4 * B, values, probs, n_labels_);
+        if (launch(update_kernel, n_trees + n_trees * 4 * B, 32, 0, stream_, s.d_trees, sp, n_trees, B, 4 * B, s.values, s.probs,
+                   n_labels_))
+            return -1;
     } else {
         // (one tree, one thread: measured 2 % faster with the backup warp as a kernel of its own on a second branch of the
         // iteration graph than inside the scatter / prepare grid)
         ARA_CUDA_OK(cudaEventRecord(ev_fork_, stream_));
         ARA_CUDA_OK(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
-        backup_kernel<<<n_trees, 32, 0, side_stream_>>>(d_trees_, sp, 0, values);
+        if (launch(backup_kernel, n_trees, 32, 0, side_stream_, s.d_trees, sp, 0, s.values)) return -1;
         ARA_CUDA_OK(cudaEventRecord(ev_join_, side_stream_));
-        scatter_prepare_kernel<<<n_trees * 4 * B, 32, 0, stream_>>>(d_trees_, sp, B, 4 * B, values, probs, n_labels_);
+        if (launch(scatter_prepare_kernel, n_trees * 4 * B, 32, 0, stream_, s.d_trees, sp, B, 4 * B, s.values, s.probs, n_labels_))
+            return -1;
         ARA_CUDA_OK(cudaStreamWaitEvent(stream_, ev_join_, 0));
     }
     if (with_events) prof_event();
     return 0;
 }
 
-// `count` iterations.  Outside profiling runs an iteration is ONE graph launch: the kernels of an iteration never
-// change (same pointers, same grids), so the sequence is captured once per handle -- the network's own graph becomes a
-// child node -- and the dependent-launch gaps between the seven search kernels shrink to graph-edge latency.
-// Threads = 2: the tree kernels of one turn of logical thread `slot` -- U (the backups and the scatter / prepare step of
-// its previous batch) then S (its next select, pack, expand) -- on stream_.
-int Search::enqueue_slot_tree_ops(int slot, bool with_update) {
+// Threads = 2: the tree kernels of one turn of logical thread s -- U (the backups and the scatter / prepare step of its
+// previous batch) then S (its next select, pack, expand) -- on stream_.
+int Search::enqueue_turn_tree_ops(const Slot& s, bool with_update) {
     const int B = sp.batch_size;
-    TreeDev* trees = d_trees_slot_[slot];
-    const float* values = net_ ? net_->io_value[slot] : d_values_slot_[slot];
-    const float* probs = net_ ? net_->io_prob[slot] : d_probs_slot_[slot];
-    if (with_update) {
-        update_kernel<<<n_trees + n_trees * 4 * B, 32, 0, stream_>>>(trees, sp, n_trees, B, 4 * B, values, probs, n_labels_);
-    }
-    if (n_trees == 1) {  // (one tree: its rows start at 0, the select kernel itself leaves the count)
-        launch_select(trees, d_count_slot_[slot]);
-    } else {
-        launch_select(trees);
-        pack_kernel<<<1, 32, 0, stream_>>>(trees, n_trees, d_count_slot_[slot]);
-    }
-    expand_kernel<<<n_trees * B, 32, 0, stream_>>>(trees, sp, B, net_ ? net_->io_in_h[slot] : nullptr, net_ ? net_->cin_pad : 0,
-                                                    net_ ? net_->precision : 0);
+    if (with_update &&
+        launch(update_kernel, n_trees + n_trees * 4 * B, 32, 0, stream_, s.d_trees, sp, n_trees, B, 4 * B, s.values, s.probs, n_labels_))
+        return -1;
+    // (one tree: its rows start at 0, the select kernel itself leaves the count)
+    if (launch_select(s, n_trees == 1 ? s.d_count : nullptr) || pack_expand(s)) return -1;
     // the stem convolution of the new batch right here, on the tree stream (which has the slack): the network stream's
     // chain starts at the tower
-    if (net_ && net_->stem_splittable() && net_->stem_device(n_trees * B, stream_, d_count_slot_[slot], slot)) return -1;
+    if (net_ && net_->stem_splittable() && net_->stem_device(n_trees * B, stream_, s.d_count, s.io)) return -1;
     return 0;
 }
 
-// one turn of logical thread `slot`: wait for its batch at the network, U + S on the tree stream, then hand the new batch
-// to the network stream
-int Search::enqueue_slot(int slot, bool with_update) {
-    const int B = sp.batch_size;
-    if (with_update) ARA_CUDA_OK(cudaStreamWaitEvent(stream_, ev_net_[slot], 0));
-    cudaGraphExec_t& ge = slot_graph_[slot][with_update ? 1 : 0];
+// one turn of logical thread k: wait for its batch at the network, U + S on the tree stream, then hand the new batch to
+// the network stream
+int Search::enqueue_turn(int k, bool with_update) {
+    Slot& s = slots_[k];
+    if (with_update) ARA_CUDA_OK(cudaStreamWaitEvent(stream_, s.ev_net, 0));
     if (profile) prof_event();
-    if (!profile && ge != nullptr) {
-        ARA_CUDA_OK(cudaGraphLaunch(ge, stream_));
-    } else if (!profile && slot_warm_) {
-        if (capture_graph(stream_, &ge, [&] { return enqueue_slot_tree_ops(slot, with_update); })) return -1;
-        ARA_CUDA_OK(cudaGraphLaunch(ge, stream_));
-    } else {
-        if (enqueue_slot_tree_ops(slot, with_update)) return -1;
-    }
+    if (run_captured(turn_graph_[k][with_update ? 1 : 0], [&] { return enqueue_turn_tree_ops(s, with_update); })) return -1;
     if (profile) prof_event();
-    launches += (n_trees == 1 ? 2 : 3) + (with_update ? 1 : 0);
-    if (net_ && net_->stem_splittable()) ++net_->launches;  // (the stem ran with the tree kernels, possibly from their graph)
-    ARA_CUDA_OK(cudaEventRecord(ev_sel_[slot], stream_));
-    ARA_CUDA_OK(cudaStreamWaitEvent(net_stream_, ev_sel_[slot], 0));
+    ARA_CUDA_OK(cudaEventRecord(s.ev_sel, stream_));
+    ARA_CUDA_OK(cudaStreamWaitEvent(net_stream_, s.ev_sel, 0));
     if (profile) {
         cudaEvent_t e = prof_event();  // (recorded on stream_; re-record it on the network stream)
         ARA_CUDA_OK(cudaEventRecord(e, net_stream_));
     }
-    if (net_) {
-        if (net_->forward_device(n_trees * B, net_stream_, d_count_slot_[slot], slot, net_->stem_splittable())) return -1;
-    } else {
-        fake_eval_kernel<<<n_trees * B, 128, 0, net_stream_>>>(d_trees_slot_[slot], n_trees, B, d_values_slot_[slot],
-                                                               d_probs_slot_[slot], n_labels_);
-        ++launches;
-    }
+    if (evaluate(s, n_trees * sp.batch_size, net_stream_, s.d_count, net_ && net_->stem_splittable())) return -1;
     if (profile) {
         cudaEvent_t e = prof_event();
         ARA_CUDA_OK(cudaEventRecord(e, net_stream_));
     }
-    ARA_CUDA_OK(cudaEventRecord(ev_net_[slot], net_stream_));
+    ARA_CUDA_OK(cudaEventRecord(s.ev_net, net_stream_));
     ++net_forwards;
     return 0;
 }
 
-// `cycles` turns of both logical threads (two mini-batches each cycle)
-int Search::iterate2(int cycles) {
-    if (!primed_) {  // S0 S1: nothing to back up yet (the root's batch was applied by the root phase)
-        if (enqueue_slot(0, false) || enqueue_slot(1, false)) return -1;
-        primed_ = true;
-        slot_warm_ = true;
-        --cycles;
-    }
-    for (int c = 0; c < cycles; ++c)
-        if (enqueue_slot(0, true) || enqueue_slot(1, true)) return -1;
-    ARA_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
+// `count` iterations.  Threads = 2: (count + 1) / 2 cycles of a turn of each logical thread, the first cycle of a go
+// S0 S1 (nothing to back up yet: the root's batch was applied by the root phase).  The handle is warm after its first
+// iteration (which warmed the network's graph up) or its first S0 S1.
 int Search::iterate(int count) {
-    if (threads_ == 2) return iterate2((count + 1) / 2);
-    const int search_kernels = 4 + (net_ ? 0 : 1);  // (one tree: select, expand, scatter+prepare, backup; many: + pack, one update launch)
-    for (int it = 0; it < count; ++it) {
-        if (!profile && iter_graph_ != nullptr) {
-            ARA_CUDA_OK(cudaGraphLaunch(iter_graph_, stream_));
-            if (net_) net_->launches += iter_net_launches_;
-        } else if (!profile && iter_warm_) {
-            // second iteration of the handle's life (the first one ran eagerly and warmed the network's graph up)
-            const long long net_before = net_ ? net_->launches : 0;
-            const int rc = capture_graph(stream_, &iter_graph_, [&] { return enqueue_iteration(false); });
-            if (net_) {
-                iter_net_launches_ = net_->launches - net_before;
-                net_->launches = net_before;
-            }
-            if (rc) return -1;
-            --it;  // nothing ran yet: launch the graph in the next pass
-            continue;
-        } else {
-            if (enqueue_iteration(profile)) return -1;
-            iter_warm_ = true;
+    if (threads_ == 2) {
+        for (int c = 0; c < (count + 1) / 2; ++c) {
+            if (enqueue_turn(0, primed_) || enqueue_turn(1, primed_)) return -1;
+            primed_ = warm_ = true;
         }
-        ++net_forwards;
-        launches += search_kernels;
+    } else {
+        for (int it = 0; it < count; ++it) {
+            if (run_captured(iter_graph_, [&] { return enqueue_iteration(profile); })) return -1;
+            warm_ = true;
+            ++net_forwards;
+        }
     }
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 // Before a go that may continue on a kept subtree: where the pools have no room for another search, the subtree moves to
-// the front of the tree's second set of pools (see compact_decide_kernel).  h_trees_ is updated; the caller uploads it.
+// the front of the tree's second set of pools (see compact_decide_kernel).  Slot 0's views are updated; the caller
+// uploads them.
 int Search::compact_pools() {
     bool any = false;
     for (char a : advanced_) any = any || a != 0;
@@ -841,37 +852,37 @@ int Search::compact_pools() {
         shadow_.resize(n_trees);
         for (auto& t : shadow_) t.hdr = nullptr;
     }
-    compact_decide_kernel<<<n_trees, 32, 0, stream_>>>(d_trees_, sp, d_roots_, d_cinfo_);
+    Slot& s0 = slots_[0];
+    if (launch(compact_decide_kernel, n_trees, 32, 0, stream_, s0.d_trees, sp, d_roots_, d_cinfo_)) return -1;
     std::vector<CompactInfo> info(n_trees);
     ARA_CUDA_OK(cudaMemcpyAsync(info.data(), d_cinfo_, sizeof(CompactInfo) * n_trees, cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
-    ++launches;
     for (int i = 0; i < n_trees; ++i) {
         const CompactInfo& c = info[i];
         if (!c.need || c.n_nodes <= 0) continue;
-        TreeDev& t = h_trees_[i];
-        compact_mark_kernel<<<(c.n_nodes + 255) / 256, 256, 0, stream_>>>(t, c.cand, c.n_nodes, d_keep_n_, d_keep_e_);
-        compact_scan_kernel<<<1, 1024, 0, stream_>>>(d_keep_n_, c.n_nodes, d_ctotal_);
-        compact_scan_kernel<<<1, 1024, 0, stream_>>>(d_keep_e_, c.n_nodes, d_ctotal_ + 1);
+        TreeDev& t = s0.h_trees[i];
+        if (launch(compact_mark_kernel, (c.n_nodes + 255) / 256, 256, 0, stream_, t, c.cand, c.n_nodes, d_keep_n_, d_keep_e_) ||
+            launch(compact_scan_kernel, 1, 1024, 0, stream_, d_keep_n_, c.n_nodes, d_ctotal_) ||
+            launch(compact_scan_kernel, 1, 1024, 0, stream_, d_keep_e_, c.n_nodes, d_ctotal_ + 1))
+            return -1;
         int total[2] = {0, 0};
         ARA_CUDA_OK(cudaMemcpyAsync(total, d_ctotal_, sizeof(total), cudaMemcpyDeviceToHost, stream_));
         ARA_CUDA_OK(cudaStreamSynchronize(stream_));
-        launches += 3;
         if (!pools_have_room(sp, max_nodes_, max_edges_, total[0], total[1])) continue;  // even the subtree alone is too big: new tree
         TreeDev& d = shadow_[i];
         if (d.hdr == nullptr) {
             d = t;
             if (alloc_pools(d)) return -1;
         }
-        compact_gather_kernel<<<(c.n_nodes + 7) / 8, 256, 0, stream_>>>(t, d, c.cand, c.n_nodes, d_keep_n_, d_keep_e_);
-        compact_finish_kernel<<<1, 1, 0, stream_>>>(t.st, total[0], total[1]);
-        launches += 2;
+        if (launch(compact_gather_kernel, (c.n_nodes + 7) / 8, 256, 0, stream_, t, d, c.cand, c.n_nodes, d_keep_n_, d_keep_e_) ||
+            launch(compact_finish_kernel, 1, 1, 0, stream_, t.st, total[0], total[1]))
+            return -1;
         // swap the pools: the tree now lives in what was the second set
         for_each_pool([&](auto m, size_t) { std::swap(t.*m, d.*m); });
         ++compactions;
     }
     ARA_CUDA_OK(cudaGetLastError());
-    ARA_CUDA_OK(cudaMemcpyAsync(d_trees_, h_trees_.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
+    ARA_CUDA_OK(cudaMemcpyAsync(s0.d_trees, s0.h_trees.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
     return 0;
 }
 
@@ -882,43 +893,32 @@ int Search::begin() {
     net_forwards = 0;
     searched_ = true;
     stop_requested_.store(false, std::memory_order_relaxed);
+    const Slot& s = slots_[0];
     ARA_CUDA_OK(cudaEventRecord(ev0_, stream_));
-    ARA_CUDA_OK(cudaMemcpyAsync(d_trees_, h_trees_.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
+    ARA_CUDA_OK(cudaMemcpyAsync(s.d_trees, s.h_trees.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
     ARA_CUDA_OK(cudaMemcpyAsync(d_roots_, h_roots_.data(), sizeof(Board) * n_trees, cudaMemcpyHostToDevice, stream_));
     if (compact_pools()) return -1;
     if (threads_ == 2) {  // the second thread's views of the trees: same pools, its own batch arrays
+        Slot& s1 = slots_[1];
         for (int i = 0; i < n_trees; ++i) {
-            TreeDev v = h_trees_[i];
-            for_each_batch_array([&](auto m, size_t) { v.*m = h_trees1_[i].*m; });
-            h_trees1_[i] = v;
+            TreeDev v = s.h_trees[i];
+            for_each_batch_array([&](auto m, size_t) { v.*m = s1.h_trees[i].*m; });
+            s1.h_trees[i] = v;
             ARA_CUDA_OK(cudaMemsetAsync(v.bs, 0, sizeof(BatchState), stream_));
         }
-        ARA_CUDA_OK(cudaMemcpyAsync(d_trees_slot_[1], h_trees1_.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
+        ARA_CUDA_OK(cudaMemcpyAsync(s1.d_trees, s1.h_trees.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
         primed_ = false;
     }
-    __half* in_h = net_ ? net_->d_in_h : nullptr;
-    const int cpad = net_ ? net_->cin_pad : 0;
     const int B = sp.batch_size;
     // root: create, expand, evaluate (set_root_node_predictions), scatter, prepare_node_for_visits (+ Dirichlet)
     ARA_CUDA_OK(cudaMemcpyAsync(d_limits_, h_limits_.data(), sizeof(uint2) * n_trees, cudaMemcpyHostToDevice, stream_));
-    root_kernel<<<n_trees, 32, 0, stream_>>>(d_trees_, sp, d_roots_, d_limits_);
-    if (n_trees > 1) {
-        pack_kernel<<<1, 32, 0, stream_>>>(d_trees_, n_trees, d_count_);
-        ++launches;
-    }
-    expand_kernel<<<n_trees * B, 32, 0, stream_>>>(d_trees_, sp, B, in_h, cpad, net_ ? net_->precision : 0);
-    if (net_) {
-        // a single-tree search only needs row 0; the new roots of a multi-tree search are packed into the first rows
-        if (net_->forward_device(n_trees == 1 ? 1 : n_trees * B, stream_, n_trees > 1 ? d_count_ : nullptr)) return -1;
-    } else {
-        fake_eval_kernel<<<n_trees * B, 128, 0, stream_>>>(d_trees_, n_trees, B, d_values_, d_probs_, n_labels_);
-        ++launches;
-    }
-    scatter_kernel<<<n_trees * B, 32, 0, stream_>>>(d_trees_, sp, B, net_ ? net_->d_value : d_values_,
-                                                     net_ ? net_->d_prob : d_probs_, n_labels_);
-    backup_kernel<<<n_trees, 32, 0, stream_>>>(d_trees_, sp, 1, net_ ? net_->d_value : d_values_);
-    prepare_kernel<<<n_trees * 4 * B, 32, 0, stream_>>>(d_trees_, sp, 4 * B);
-    launches += 5;
+    if (launch(root_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, d_roots_, d_limits_) || pack_expand(s)) return -1;
+    // a single-tree search only needs row 0; the new roots of a multi-tree search are packed into the first rows
+    if (evaluate(s, n_trees == 1 ? 1 : n_trees * B, stream_, n_trees > 1 ? s.d_count : nullptr, false)) return -1;
+    if (launch(scatter_kernel, n_trees * B, 32, 0, stream_, s.d_trees, sp, B, s.values, s.probs, n_labels_) ||
+        launch(backup_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, 1, s.values) ||
+        launch(prepare_kernel, n_trees * 4 * B, 32, 0, stream_, s.d_trees, sp, 4 * B))
+        return -1;
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -956,8 +956,7 @@ int Search::node_view(int tree, int node_id, NodeView* out) {
     if (tree < 0 || tree >= n_trees) return set_error("ara_search_node: tree %d out of range", tree);
     if (!searched_) return set_error("ara_search_node: no search has been started on this handle");
     ARA_CUDA_OK(cudaSetDevice(device_));
-    node_view_kernel<<<1, 32, 0, stream_>>>(d_trees_, tree, node_id, d_node_view_);
-    ++launches;
+    if (launch(node_view_kernel, 1, 32, 0, stream_, slots_[0].d_trees, tree, node_id, d_node_view_)) return -1;
     ARA_CUDA_OK(cudaMemcpyAsync(out, d_node_view_, sizeof(NodeView), cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
     if (out->node_id < 0) return set_error("ara_search_node: tree %d has no node %d", tree, node_id);
@@ -1054,8 +1053,7 @@ int Search::set_limits(int tree, unsigned simulations, unsigned nodes) {
 }
 
 int Search::read_time_stats(RootStatsHost* out) {
-    time_stats_kernel<<<1, 32, 0, stream_>>>(d_trees_, d_tstats_);
-    ++launches;
+    if (launch(time_stats_kernel, 1, 32, 0, stream_, slots_[0].d_trees, d_tstats_)) return -1;
     ARA_CUDA_OK(cudaMemcpyAsync(h_tstats_, d_tstats_, sizeof(RootTimeStats), cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
     static_assert(sizeof(RootStatsHost) == sizeof(RootTimeStats), "root statistics layout");
@@ -1067,19 +1065,16 @@ int Search::apply_move(int tree, unsigned short move) {
     if (tree < 0 || tree >= n_trees) return set_error("ara_search_apply_move: tree %d out of range", tree);
     ARA_CUDA_OK(cudaSetDevice(device_));
     if (!searched_) return 0;  // nothing to keep before the first search
-    // d_trees_ still holds the descriptors of the last go (pool pointers never change)
-    advance_kernel<<<1, 32, 0, stream_>>>(d_trees_, tree, static_cast<Move>(move));
+    // slot 0's device views still hold the descriptors of the last go (pool pointers never change)
+    if (launch(advance_kernel, 1, 32, 0, stream_, slots_[0].d_trees, tree, static_cast<Move>(move))) return -1;
     if (advanced_.empty()) advanced_.assign(n_trees, 0);
     advanced_[tree] = 1;
-    ++launches;
-    ARA_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 int Search::fetch_results() {
     ARA_CUDA_OK(cudaSetDevice(device_));
-    result_kernel<<<n_trees, 32, 0, stream_>>>(d_trees_, sp, d_results_);
-    ++launches;
+    if (launch(result_kernel, n_trees, 32, 0, stream_, slots_[0].d_trees, sp, d_results_)) return -1;
     ARA_CUDA_OK(cudaMemcpyAsync(results.data(), d_results_, sizeof(SearchResult) * n_trees, cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
     for (const auto& r : results)
