@@ -1,46 +1,35 @@
-"""Weight import from the reference's ONNX artefacts (SURVEY §8 f3): `<prefix>-v<version>[-bsize-<n>].onnx` as written by
-`export_to_onnx` (DeepCrazyhouse/src/training/trainer_agent_pytorch.py:588-650: torch.onnx.export in eval mode, then
-onnx-simplifier -- BatchNorm folded into the convolutions) -> ARAB2001 blob for ara_net_create.
+"""Weight import from the reference's ONNX artefacts (SURVEY §8 f3) -> a blob for ara_net_create: the files
+`export_to_onnx` writes (DeepCrazyhouse/src/training/trainer_agent_pytorch.py:588-650: torch.onnx.export in eval mode,
+then onnx-simplifier, which folds BatchNorm into the convolutions) and the exports of the MXNet symbols
+(`convert_to_onnx.py`).  No `onnx` package is needed: a minimal protobuf wire-format reader takes only the fields used here
+(graph.node: op_type, inputs, outputs, attributes; graph.initializer: dims, data type, raw / float / int64 data).
 
-No `onnx` package is needed (the image has none): the file is read with a minimal protobuf wire-format reader, only the
-fields this import uses (graph.node: op_type, inputs, attributes `group` / `transB`; graph.initializer: dims, data type,
-raw / float / int64 data).  The graph is not executed; the network structure is the RISE family's and is recovered from
-the ORDER of its Conv / Gemm / MatMul nodes (a torch export lists them in execution order):
+The graph is not executed and its node order is not trusted: `_Graph` follows its edges from the stem convolution on the
+graph input, block by block, to the heads, looking through shape-only nodes.
+- BatchNorm folded (RISE; AlphaVile after merge_bn() has folded norm1 / norm2 into q / k / v and mlp.conv1) -> the blob
+  weights.export_blob writes for the same checkpoint, ARAB2001 or ARAB2003.  A block input that feeds a `Mul` with a gate
+  has squeeze-excitation, and the `Mul` output is the block's input and shortcut (builder_util.py:473-475).  A block input
+  that feeds an `Add` starts a bottleneck block (conv1x1, depthwise, conv1x1, traced back from the Add); any other block
+  is a NextViT transformer block (NTB), whose q and k are told apart by the attention-score `MatMul` they feed and v by
+  the one behind the `Softmax`.  The policy head's 3x3 convolution ends the tower.
+- Unfolded `BatchNormalization` nodes (an MXNet export, SE off the shortcut) -> export_mx_blob's ARAB2002 blob.  Each block
+  is the `Add` fed by the block input, traced back through BatchNormalization / Relu / Conv to its first convolution,
+  whose input is the block input or its `Mul` with the gate (`Sigmoid`, or `HardSigmoid` with alpha 0.2).
+Both trace the gate back to `Gemm, Relu, Gemm` (ca_se) or to a 1-D `Conv` over the channels (eca_se).
 
-    stem conv3x3 | per block: [SE: Gemm, Gemm  or  eca Conv1d] conv1x1, depthwise kxk (group = channels), conv1x1 |
-    value head: conv1x1, Gemm(s) | policy head: conv3x3, conv3x3
-
-PARITY UNPINNED: /root/reference holds no .onnx file and the `onnx` / `onnxsim` packages are absent, so this reader is
-checked against files written by tests/onnx_writer.py (same node kinds and tensor layouts as the torch exporter emits for
-these modules), not against an artefact of the reference itself.
-
-A graph exported from the reference's MXNet symbols (`convert_to_onnx.py`) computes another network from the same
-layers (crazyara_b200/weights.py, export_mx_blob).  It is recognised by its unfolded `BatchNormalization` nodes and read by
-graph edges, not node order: from the stem, each block is the `Add` fed by the block input, traced back through
-BatchNormalization / Relu / Conv to its first convolution, whose input is the block input itself or a `Mul` of it with a
-squeeze-excitation gate (`Sigmoid`, or `HardSigmoid` with its alpha; behind it a 1-D `Conv` over the channels for eca_se,
-or two `Gemm` with biases for ca_se).  The layers go, under the names the symbol code gives them, through export_mx_blob
-into an ARAB2002 blob.  PARITY UNPINNED as well: no MXNet export is in either tree; the reader is checked against files
-written by tests/onnx_mx_writer.py.
-
-An AlphaVile export (alpha_vile.py; the trainer calls merge_bn() first, so norm1 / norm2 are folded into q / k / v and
-mlp.conv1) is recognised by the `Concat` of activations in its NextViT transformer blocks (a `Concat` of shape arithmetic,
-which dynamic-batch exports of the RISE networks carry, does not count) and read by graph edges as well: from the stem,
-a block whose input feeds an `Add` is a bottleneck block (conv1x1, depthwise, conv1x1 traced back from that Add), any other
-is an NTB -- patch_embed `Conv`, q / k / v / proj as `MatMul` + `Add` with initialisers (q and k told apart by the
-attention-score `MatMul` they feed, v by the one behind the `Softmax`), projection `Conv`, the group `Conv`, the MHCA
-conv1x1, `Concat`, the two MLP `Conv`s and the closing `Add`.  The result is the ARAB2003 blob weights.export_blob writes
-for the same checkpoint.  PARITY UNPINNED: no `onnx` package is installed and the legacy exporter refuses to run without
-it, so the reader is checked against files written by tests/onnx_alphavile_writer.py.
+PARITY UNPINNED: the reference tree holds no .onnx file and no `onnx` / `onnxsim` package is installed, so the readers are
+checked against files written by tests/onnx_writer.py, tests/onnx_mx_writer.py and tests/onnx_alphavile_writer.py.
 """
 import struct
 from collections import defaultdict
 
 import numpy as np
 
-from .weights import SE_CODE, export_mx_blob, write_blob
+from .weights import export_mx_blob, input_version_of, write_blob
 
-_SHAPE_OPS = ("Reshape", "Flatten", "Squeeze", "Unsqueeze", "Identity", "Transpose")
+_SHAPE_OPS = ("Reshape", "Flatten", "Squeeze", "Unsqueeze", "Identity")
+# a torch export also has the NTB's token transposes and the Expand of the SE gate (x * y.view(b, c, 1, 1).expand_as(x))
+_TORCH_SHAPE_OPS = _SHAPE_OPS + ("Transpose", "Expand")
 
 
 # ---------------------------------------------------------------------------------------------- protobuf wire format
@@ -155,401 +144,310 @@ def read_graph(path):
     return nodes, inits
 
 
+# ---------------------------------------------------------------------------------------------- graph walks
+class _Graph:
+    """One file's nodes, initialisers, producers and consumers, and walks along its edges through the node types `skip`"""
+
+    def __init__(self, path, nodes, inits, skip):
+        self.path, self.nodes, self.inits, self.skip = path, nodes, inits, skip
+        self.prod, self.cons = {}, defaultdict(list)
+        for nd in nodes:
+            for o in nd[2]:
+                self.prod[o] = nd
+            for i in nd[1]:
+                self.cons[i].append(nd)
+
+    def fail(self, what):
+        raise ValueError(f"{self.path}: {what}")
+
+    def back(self, t, *ops):  # the producer of t, skipping shape-only nodes, which must be one of ops
+        nd = self.prod.get(t)
+        while nd is not None and nd[0] in self.skip:
+            nd = self.prod.get(nd[1][0])
+        if nd is None or nd[0] not in ops:
+            self.fail(f"expected {'/'.join(ops)} in front of '{t}', found {nd[0] if nd else 'a graph input'}")
+        return nd
+
+    def fwd(self, t, op, weighted=None):  # the consumers of t of type op, whose second input is an initialiser if weighted
+        out, frontier = [], [t]
+        while frontier:
+            u = frontier.pop()
+            for nd in self.cons[u]:
+                if nd[0] in self.skip:
+                    frontier.append(nd[2][0])
+                elif nd[0] == op and (weighted is None or (len(nd[1]) > 1 and nd[1][1] in self.inits) == weighted):
+                    out.append(nd)
+        return out
+
+    def first(self, t, op):  # the first direct consumer of t of type op, or None
+        return next((nd for nd in self.cons[t] if nd[0] == op), None)
+
+    def one(self, t, op, weighted=None):
+        c = self.fwd(t, op, weighted)
+        if len(c) != 1:
+            self.fail(f"expected one {op} behind '{t}', found {len(c)}")
+        return c[0]
+
+    def downstream(self, t, ops):  # the first node of one of ops reached from tensor t, breadth first
+        seen, frontier = set(), [t]
+        while frontier:
+            nxt = []
+            for u in frontier:
+                for nd in self.cons[u]:
+                    if nd[0] in ops:
+                        return nd
+                    if id(nd) not in seen:
+                        seen.add(id(nd))
+                        nxt += nd[2]
+            frontier = nxt
+        return None
+
+    def weight(self, nd):  # a Conv's weight; a Gemm's or MatMul's as [out, in], the layout of torch.nn.Linear.weight
+        w = self.inits[nd[1][1]]
+        return np.ascontiguousarray(w.T if nd[0] == "MatMul" or (nd[0] == "Gemm" and not nd[3].get("transB", 0)) else w)
+
+    def bias(self, nd):  # a Conv's or Gemm's bias, zeros when it has none
+        has = len(nd[1]) > 2 and nd[1][2] in self.inits
+        return self.inits[nd[1][2]] if has else np.zeros(self.weight(nd).shape[0], np.float32)
+
+    def linear(self, mm):  # MatMul(x, W[in, out]) + Add(bias) -> ([out, in], bias, output tensor)
+        add = self.one(mm[2][0], "Add")
+        b = next((self.inits[i] for i in add[1] if i in self.inits), None)
+        if b is None:
+            self.fail(f"no bias behind MatMul '{mm[2][0]}'")
+        return self.weight(mm), b, add[2][0]
+
+    def stem(self):  # the convolution on the graph input
+        return next((nd for nd in self.nodes if nd[0] == "Conv" and nd[1][0] not in self.prod and nd[1][0] not in self.inits), None)
+
+    def se(self, mul, x, i):  # block i's Mul(x, gate) -> (gate, [Gemm, Gemm] for ca_se or [Conv] for eca_se)
+        if x not in mul[1]:
+            self.fail(f"block {i}: the squeeze-excitation does not act on the block input")
+        gate = self.back(mul[1][1] if mul[1][0] == x else mul[1][0], "Sigmoid", "HardSigmoid")
+        fc = self.back(gate[1][0], "Gemm", "MatMul", "Conv")
+        if fc[0] == "Conv":
+            return gate, [fc]
+        return gate, [self.back(self.back(fc[1][0], "Relu")[1][0], "Gemm", "MatMul"), fc]
+
+
 # ---------------------------------------------------------------------------------------------- graph -> blob
 def import_onnx(onnx_path, blob_path, input_version=None, channels=256):
     nodes, inits = read_graph(onnx_path)
     if any(nd[0] == "BatchNormalization" for nd in nodes):
-        return _import_mxnet_graph(onnx_path, nodes, inits, blob_path, input_version, channels)
-    if _has_data_concat(nodes):
-        return _import_alphavile_graph(onnx_path, nodes, inits, blob_path, input_version)
-    order = []  # convolutions and fully-connected layers in execution order
-    for op, ins, outs, attrs in nodes:
-        if op == "Conv" and len(ins) >= 2 and ins[1] in inits:
-            w = inits[ins[1]]
-            b = inits[ins[2]] if len(ins) > 2 and ins[2] in inits else np.zeros(w.shape[0], np.float32)
-            order.append(("conv", w, b, int(attrs.get("group", 1))))
-        elif op in ("Gemm", "MatMul") and len(ins) >= 2 and ins[1] in inits:
-            w = inits[ins[1]]
-            if op == "MatMul" or not attrs.get("transB", 0):
-                w = w.T  # -> [out, in], the layout of torch.nn.Linear.weight
-            b = inits[ins[2]] if len(ins) > 2 and ins[2] in inits else np.zeros(w.shape[0], np.float32)
-            order.append(("fc", np.ascontiguousarray(w), b, 1))
-    if not order or order[0][0] != "conv" or order[0][1].ndim != 4 or order[0][1].shape[2] != 3:
-        raise ValueError(f"{onnx_path}: does not start with a 3x3 stem convolution")
-    tensors = []
-    put = lambda a: tensors.append(np.ascontiguousarray(a, dtype=np.float32).reshape(-1))
-    stem_w, stem_b = order[0][1], order[0][2]
-    C = stem_w.shape[0]
-    if C != channels:
-        raise ValueError(f"{onnx_path}: {C} trunk channels, this engine builds {channels}")
-    put(stem_w), put(stem_b)
-    i, kernels, se_types, c_ops = 1, [], [], []
-    while True:
-        # squeeze-excitation layers in front of the block (they act on its input)
-        se, j = None, i
-        fcs = []
-        while j < len(order) and (order[j][0] == "fc" or (order[j][0] == "conv" and order[j][1].ndim == 3)):
-            fcs.append(order[j])
-            j += 1
-        # a block = conv1x1 (C -> Cop), depthwise kxk, conv1x1 (Cop -> C)
-        if not (j + 2 < len(order) and order[j][0] == "conv" and order[j][1].ndim == 4 and order[j][1].shape[2] == 1 and
-                order[j + 1][0] == "conv" and order[j + 1][3] == order[j + 1][1].shape[0] and order[j + 1][3] > 1):
-            break
-        if fcs:
-            if len(fcs) == 2 and fcs[0][0] == "fc":
-                se = "ca_se"
-                put(fcs[0][1]), put(fcs[1][1])  # (the reference's SE FCs have no bias, builder_util.py:100-116)
-            elif len(fcs) == 1 and fcs[0][1].ndim == 3:
-                se = "eca_se"
-                wc = fcs[0][1]
-                put(wc[:, :, wc.shape[2] // 2]), put(fcs[0][2])
-            else:
-                raise ValueError(f"{onnx_path}: unrecognised squeeze-excitation pattern in front of block {len(kernels)}")
-        w1, b1, _ = order[j][1:]
-        wd, bd, _ = order[j + 1][1:]
-        w2, b2, _ = order[j + 2][1:]
-        cop, k = w1.shape[0], wd.shape[2]
-        if w1.shape[1] != C or wd.shape[0] != cop or w2.shape[:2] != (C, cop) or k not in (3, 5):
-            raise ValueError(f"{onnx_path}: block {len(kernels)} is not a RISE bottleneck block")
-        put(w1), put(b1), put(wd), put(bd), put(w2), put(b2)
-        kernels.append(int(k)), se_types.append(se), c_ops.append(int(cop))
-        i = j + 3
-    if not kernels:
-        raise ValueError(f"{onnx_path}: no bottleneck block found")
-    # value head: conv1x1 (C -> 8) + FC layers; policy head: conv3x3 (C -> C), conv3x3 (C -> P)
-    rest = order[i:]
-    vconv = [r for r in rest if r[0] == "conv" and r[1].ndim == 4 and r[1].shape[2] == 1]
-    heads = [r for r in rest if r[0] == "conv" and r[1].ndim == 4 and r[1].shape[2] == 3]
-    fcs = [r for r in rest if r[0] == "fc"]
-    if len(vconv) != 1 or vconv[0][1].shape[1] != C:
-        raise ValueError(f"{onnx_path}: value head (one 1x1 convolution) not found behind the tower")
-    if len(heads) != 2 or heads[0][1].shape[:2] != (C, C) or heads[1][1].shape[1] != C:
-        raise ValueError(f"{onnx_path}: policy head (two 3x3 convolutions) not found behind the tower")
-    put(vconv[0][1]), put(vconv[0][2])
-    # value head variants (builder_util.py:246-330): FC 512 -> 256 -> 1 (tanh), or the WDL head FC -> 3 with the plies FC -> 1
-    wdl = len(fcs) == 2 and fcs[0][1].shape[0] == 3
-    if wdl:
-        put(fcs[0][1]), put(fcs[0][2]), put(fcs[1][1]), put(fcs[1][2])
-    elif len(fcs) == 2:
-        put(fcs[0][1]), put(fcs[0][2]), put(fcs[1][1]), put(fcs[1][2])
-    else:
-        raise ValueError(f"{onnx_path}: {len(fcs)} fully-connected layers in the value head (expected 2)")
-    put(heads[0][1]), put(heads[0][2])
-    put(heads[1][1])
-    arch = dict(name=f"rise_{len(kernels)}b", in_channels=int(stem_w.shape[1]), policy_channels=int(heads[1][1].shape[0]),
-                channels=int(C), kernels=kernels, se_types=se_types, c_ops=c_ops, wdl=bool(wdl), value_channels=int(vconv[0][1].shape[0]),
-                value_fc=256)
-    write_blob(blob_path, arch, tensors, _input_version(arch, input_version))
-    return arch
+        return _import_mxnet_graph(_Graph(onnx_path, nodes, inits, _SHAPE_OPS), blob_path, input_version, channels)
+    return _import_folded_graph(_Graph(onnx_path, nodes, inits, _TORCH_SHAPE_OPS), blob_path, input_version, channels)
 
 
-def _input_version(arch, input_version):
-    if input_version is not None:
-        return input_version
-    return {34: 10, 63: 10, 39: 10, 51: 20, 52: 30, 64: 30, 80: 30}.get(arch["in_channels"], 10)
-
-
-def _import_mxnet_graph(onnx_path, nodes, inits, blob_path, input_version, channels):
-    """a graph with unfolded BatchNormalization nodes (an MXNet export), read by its edges -> ARAB2002 blob"""
-    prod, cons = {}, defaultdict(list)
-    for nd in nodes:
-        for o in nd[2]:
-            prod[o] = nd
-        for i in nd[1]:
-            cons[i].append(nd)
-
-    def fail(what):
-        raise ValueError(f"{onnx_path}: {what}")
-
-    def back(t, *ops):  # the producer of t, skipping shape-only nodes, which must be one of ops
-        nd = prod.get(t)
-        while nd is not None and nd[0] in ("Reshape", "Flatten", "Squeeze", "Unsqueeze", "Identity"):
-            nd = prod.get(nd[1][0])
-        if nd is None or nd[0] not in ops:
-            fail(f"expected {'/'.join(ops)} in front of '{t}', found {nd[0] if nd else 'a graph input'}")
-        return nd
-
-    def fwd(t, op):  # the consumer of t with type op, or None
-        return next((nd for nd in cons[t] if nd[0] == op), None)
-
+def _import_mxnet_graph(g, blob_path, input_version, channels):
+    """a graph with unfolded BatchNormalization nodes (an MXNet export) -> ARAB2002 blob"""
     params, eps = {}, {}
 
     def take_bn(nd, name):
         for key, i in (("gamma", 1), ("beta", 2), ("moving_mean", 3), ("moving_var", 4)):
-            params[f"{name}_{key}"] = inits[nd[1][i]]
+            params[f"{name}_{key}"] = g.inits[nd[1][i]]
         eps[name] = float(nd[3].get("epsilon", 1e-5))  # (ONNX's default)
 
     def take(nd, name):  # Conv / Gemm weights and bias under the MXNet layer name
-        w = inits[nd[1][1]]
-        if nd[0] == "Gemm" and not nd[3].get("transB", 0):
-            w = w.T
-        params[name + "_weight"] = np.ascontiguousarray(w)
-        if len(nd[1]) > 2 and nd[1][2] in inits:
-            params[name + "_bias"] = inits[nd[1][2]]
+        params[name + "_weight"] = g.weight(nd)
+        if len(nd[1]) > 2 and nd[1][2] in g.inits:
+            params[name + "_bias"] = g.inits[nd[1][2]]
 
     def conv_bn(t, name):  # t = output of Conv -> BatchNormalization: the Conv node
-        bn = back(t, "BatchNormalization")
-        conv = back(bn[1][0], "Conv")
+        bn = g.back(t, "BatchNormalization")
+        conv = g.back(bn[1][0], "Conv")
         take(conv, name)
         take_bn(bn, name.replace("conv", "bn"))
         return conv
 
-    stem = next((nd for nd in nodes if nd[0] == "Conv" and nd[1][0] not in prod and nd[1][0] not in inits), None)
-    if stem is None or inits[stem[1][1]].shape[0] != channels or inits[stem[1][1]].shape[2] != 3:
-        fail(f"no 3x3 stem convolution with {channels} channels on the graph input")
+    stem = g.stem()
+    if stem is None or g.weight(stem).shape[0] != channels or g.weight(stem).shape[2] != 3:
+        g.fail(f"no 3x3 stem convolution with {channels} channels on the graph input")
     take(stem, "stem_conv0")
-    bn = fwd(stem[2][0], "BatchNormalization")
+    bn = g.first(stem[2][0], "BatchNormalization")
     if bn is None:
-        fail("no BatchNormalization behind the stem")
+        g.fail("no BatchNormalization behind the stem")
     take_bn(bn, "stem_bn0")
-    relu = fwd(bn[2][0], "Relu")
-    x, stem_act = (relu[2][0], True) if relu is not None and fwd(relu[2][0], "Add") is not None else (bn[2][0], False)
+    relu = g.first(bn[2][0], "Relu")
+    x, stem_act = (relu[2][0], True) if relu is not None and g.first(relu[2][0], "Add") is not None else (bn[2][0], False)
     kernels, se_types, se_gates, c_ops, n_eca = [], [], [], [], 0
     while True:
-        add = next((nd for nd in cons[x] if nd[0] == "Add" and len(nd[1]) == 2), None)
+        add = g.first(x, "Add")
         if add is None:
             break
         i, p = len(kernels), f"bc_res_block{len(kernels)}"
-        other = add[1][1] if add[1][0] == x else add[1][0]
-        conv3 = conv_bn(other, p + "_conv3")
-        conv2 = conv_bn(back(conv3[1][0], "Relu")[1][0], p + "_conv2")
-        conv1 = conv_bn(back(conv2[1][0], "Relu")[1][0], p + "_conv1")
+        conv3 = conv_bn(add[1][1] if add[1][0] == x else add[1][0], p + "_conv3")
+        conv2 = conv_bn(g.back(conv3[1][0], "Relu")[1][0], p + "_conv2")
+        conv1 = conv_bn(g.back(conv2[1][0], "Relu")[1][0], p + "_conv1")
         w1, wd = params[p + "_conv1_weight"], params[p + "_conv2_weight"]
         if w1.shape[1] != channels or wd.shape[0] != w1.shape[0] or wd.shape[2] not in (3, 5):
-            fail(f"block {i} is not a RISE bottleneck block")
+            g.fail(f"block {i} is not a RISE bottleneck block")
         se, gate = None, None
         if conv1[1][0] != x:
-            mul = back(conv1[1][0], "Mul")
-            if x not in mul[1]:
-                fail(f"block {i}: the squeeze-excitation does not act on the block input")
-            g = back(mul[1][1] if mul[1][0] == x else mul[1][0], "Sigmoid", "HardSigmoid")
-            if g[0] == "Sigmoid":
-                gate = "sigmoid"
-            elif abs(g[3].get("alpha", 0.2) - 0.2) < 1e-6 and abs(g[3].get("beta", 0.5) - 0.5) < 1e-6:
-                gate = "hard_sigmoid"
-            else:
-                fail(f"block {i}: HardSigmoid alpha {g[3].get('alpha')} beta {g[3].get('beta')}")
-            fc = back(g[1][0], "Gemm", "MatMul", "Conv")
-            if fc[0] == "Conv":
-                se = "eca_se"
-                take(fc, f"convolution{n_eca}")
+            gn, fcs = g.se(g.back(conv1[1][0], "Mul"), x, i)
+            gate, alpha, beta = ("sigmoid" if gn[0] == "Sigmoid" else "hard_sigmoid"), gn[3].get("alpha", 0.2), gn[3].get("beta", 0.5)
+            if gate == "hard_sigmoid" and not (abs(alpha - 0.2) < 1e-6 and abs(beta - 0.5) < 1e-6):
+                g.fail(f"block {i}: HardSigmoid alpha {alpha} beta {beta}")
+            se = "eca_se" if len(fcs) == 1 else "ca_se"
+            if se == "eca_se":
+                take(fcs[0], f"convolution{n_eca}")
                 n_eca += 1
             else:
-                se = "ca_se"
-                take(fc, p + "_se_fc1")
-                take(back(back(fc[1][0], "Relu")[1][0], "Gemm", "MatMul"), p + "_se_fc0")
+                take(fcs[0], p + "_se_fc0"), take(fcs[1], p + "_se_fc1")
         kernels.append(int(wd.shape[2])), se_types.append(se), se_gates.append(gate), c_ops.append(int(w1.shape[0]))
         x = add[2][0]
     if not kernels:
-        fail("no bottleneck block found")
-    heads = [nd for nd in cons[x] if nd[0] == "Conv"]
-    vconv = [nd for nd in heads if inits[nd[1][1]].shape[2] == 1]
-    pconv = [nd for nd in heads if inits[nd[1][1]].shape[2] == 3]
+        g.fail("no bottleneck block found")
+    heads = [nd for nd in g.cons[x] if nd[0] == "Conv"]
+    vconv = [nd for nd in heads if g.weight(nd).shape[2] == 1]
+    pconv = [nd for nd in heads if g.weight(nd).shape[2] == 3]
     if len(vconv) != 1 or len(pconv) != 1:
-        fail("value head (1x1 convolution) and policy head (3x3 convolution) not found behind the tower")
+        g.fail("value head (1x1 convolution) and policy head (3x3 convolution) not found behind the tower")
     take(vconv[0], "value_conv0")
-    take_bn(fwd(vconv[0][2][0], "BatchNormalization"), "value_bn0")
-    g0 = _downstream(cons, vconv[0][2][0], ("Gemm", "MatMul"))
-    g1 = g0 and _downstream(cons, g0[2][0], ("Gemm", "MatMul"))
+    take_bn(g.first(vconv[0][2][0], "BatchNormalization"), "value_bn0")
+    g0 = g.downstream(vconv[0][2][0], ("Gemm", "MatMul"))
+    g1 = g0 and g.downstream(g0[2][0], ("Gemm", "MatMul"))
     if g1 is None:
-        fail("value head: two fully-connected layers not found")
+        g.fail("value head: two fully-connected layers not found")
     take(g0, "value_fc0"), take(g1, "value_fc1")
     take(pconv[0], "policy_conv0")
-    take_bn(fwd(pconv[0][2][0], "BatchNormalization"), "policy_bn0")
-    take(_downstream(cons, pconv[0][2][0], ("Conv",)), "policy_conv1")
-    arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(inits[stem[1][1]].shape[1]),
+    take_bn(g.first(pconv[0][2][0], "BatchNormalization"), "policy_bn0")
+    take(g.downstream(pconv[0][2][0], ("Conv",)), "policy_conv1")
+    arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(g.weight(stem).shape[1]),
                 policy_channels=int(params["policy_conv1_weight"].shape[0]), channels=channels, kernels=kernels,
                 se_types=se_types, se_gates=se_gates, c_ops=c_ops, wdl=False, value_channels=int(params["value_conv0_weight"].shape[0]),
                 value_fc=256, stem_act=stem_act, policy_bias="policy_conv1_bias" in params)
-    export_mx_blob(params, arch, blob_path, _input_version(arch, input_version), eps=eps, fix_gamma=False)
+    export_mx_blob(params, arch, blob_path, input_version_of(arch, input_version), eps=eps, fix_gamma=False)
     return arch
 
 
-def _has_data_concat(nodes):
-    """a Concat of activations (the NTB's y1 | z2, both produced by an Add), as opposed to the shape arithmetic
-    (Shape -> Gather -> Unsqueeze -> Concat -> Reshape) a dynamic-batch export leaves in front of a view()"""
-    prod = {o: nd for nd in nodes for o in nd[2]}
-    return any(nd[0] == "Concat" and len(nd[1]) >= 2 and all(prod.get(i, ("",))[0] in ("Add", "Conv", "Relu") for i in nd[1])
-               for nd in nodes)
-
-
-def _import_alphavile_graph(onnx_path, nodes, inits, blob_path, input_version):
-    """an AlphaVile export (BatchNorms folded, NTB blocks joined by Concat), read by its edges -> ARAB2003 blob"""
-    prod, cons = {}, defaultdict(list)
-    for nd in nodes:
-        for o in nd[2]:
-            prod[o] = nd
-        for i in nd[1]:
-            cons[i].append(nd)
-
-    def fail(what):
-        raise ValueError(f"{onnx_path}: {what}")
-
-    def back(t, *ops):  # the producer of t, skipping shape-only nodes, which must be one of ops
-        nd = prod.get(t)
-        while nd is not None and nd[0] in _SHAPE_OPS:
-            nd = prod.get(nd[1][0])
-        if nd is None or nd[0] not in ops:
-            fail(f"expected {'/'.join(ops)} in front of '{t}', found {nd[0] if nd else 'a graph input'}")
-        return nd
-
-    def fwd(t, op, weighted=None):  # the consumers of t of type op, through shape-only nodes
-        out, frontier = [], [t]
-        while frontier:
-            u = frontier.pop()
-            for nd in cons[u]:
-                if nd[0] in _SHAPE_OPS:
-                    frontier.append(nd[2][0])
-                elif nd[0] == op and (weighted is None or (len(nd[1]) > 1 and nd[1][1] in inits) == weighted):
-                    out.append(nd)
-        return out
-
-    def one(t, op, weighted=None):
-        c = fwd(t, op, weighted)
-        if len(c) != 1:
-            fail(f"expected one {op} behind '{t}', found {len(c)}")
-        return c[0]
-
-    W = lambda nd: inits[nd[1][1]]
-    bias = lambda nd: inits[nd[1][2]] if len(nd[1]) > 2 and nd[1][2] in inits else np.zeros(W(nd).shape[0], np.float32)
+def _import_folded_graph(g, blob_path, input_version, channels):
+    """a BatchNorm-folded export: a RISE network (256-channel trunk) -> ARAB2001 blob, an AlphaVile one -> ARAB2003"""
+    W, bias = g.weight, g.bias
     mat = lambda a: a.reshape(a.shape[0], -1)
-
-    def linear(mm):  # MatMul(x, W[in, out]) + Add(bias) -> ([out, in], bias, output tensor)
-        add = one(mm[2][0], "Add")
-        b = next((inits[i] for i in add[1] if i in inits), None)
-        if b is None:
-            fail(f"no bias behind MatMul '{mm[2][0]}'")
-        return np.ascontiguousarray(W(mm).T), b, add[2][0]
-
-    stem = next((nd for nd in nodes if nd[0] == "Conv" and nd[1][0] not in prod and nd[1][0] not in inits), None)
+    stem = g.stem()
     if stem is None or W(stem).shape[2] != 3:
-        fail("no 3x3 stem convolution on the graph input")
+        g.fail("no 3x3 stem convolution on the graph input")
     C = int(W(stem).shape[0])
     tensors = [W(stem), bias(stem)]
-    x = one(stem[2][0], "Relu")[2][0]
-    kernels, c_ops, ntb, widths = [], [], [], set()
-    while not any(W(nd).shape[2] == 3 for nd in fwd(x, "Conv", True)):  # the policy head's 3x3 convolution ends the tower
-        add = next((nd for nd in cons[x] if nd[0] == "Add" and len(nd[1]) == 2), None)
-        i = len(kernels)
+    x = g.one(stem[2][0], "Relu")[2][0]
+    kernels, se_types, c_ops, ntb, widths = [], [], [], [], set()
+    while not any(W(nd).shape[2] == 3 for nd in g.fwd(x, "Conv", True)):  # the policy head's 3x3 convolution ends the tower
+        i, se = len(kernels), None
+        mul = g.first(x, "Mul")
+        if mul is not None:  # squeeze-excitation (its gate unchecked: ARAB2001 knows only torch's hard sigmoid)
+            _, fcs = g.se(mul, x, i)
+            se, w = ("ca_se" if len(fcs) == 2 else "eca_se"), W(fcs[0])
+            if se == "eca_se" and w.ndim != 3:
+                g.fail(f"block {i}: the eca_se convolution is not 1-D")
+            # (the reference's SE FCs have no bias, builder_util.py:100-116; of the eca_se Conv the centre tap and bias)
+            tensors += [w, W(fcs[1])] if se == "ca_se" else [w[:, :, w.shape[2] // 2], bias(fcs[0])]
+            x = mul[2][0]  # the block's input and its shortcut
+        add = g.first(x, "Add")
         if add is not None:  # bottleneck block: x + conv1x1(relu(depthwise(relu(conv1x1(x)))))
-            c3 = back(add[1][1] if add[1][0] == x else add[1][0], "Conv")
-            c2 = back(back(c3[1][0], "Relu")[1][0], "Conv")
-            c1 = back(back(c2[1][0], "Relu")[1][0], "Conv")
-            w1, wd = W(c1), W(c2)
-            if c1[1][0] != x or w1.shape[1] != C or wd.shape[0] != w1.shape[0] or wd.shape[2] not in (3, 5):
-                fail(f"block {i} is not a RISE bottleneck block")
-            tensors += [w1, bias(c1), wd, bias(c2), W(c3), bias(c3)]
-            kernels.append(int(wd.shape[2])), c_ops.append(int(w1.shape[0])), ntb.append(False)
+            c3 = g.back(add[1][1] if add[1][0] == x else add[1][0], "Conv")
+            c2 = g.back(g.back(c3[1][0], "Relu")[1][0], "Conv")
+            c1 = g.back(g.back(c2[1][0], "Relu")[1][0], "Conv")
+            w1, wd, w3 = W(c1), W(c2), W(c3)
+            if (c1[1][0] != x or w1.shape[1] != C or wd.shape[0] != w1.shape[0] or wd.shape[2] not in (3, 5) or
+                    w3.shape[:2] != (C, w1.shape[0])):
+                g.fail(f"block {i} is not a RISE bottleneck block")
+            tensors += [w1, bias(c1), wd, bias(c2), w3, bias(c3)]
+            kernels.append(int(wd.shape[2])), se_types.append(se), c_ops.append(int(w1.shape[0])), ntb.append(False)
             x = add[2][0]
             continue
-        pe = one(x, "Conv", True)
+        if se is not None:
+            g.fail(f"block {i}: no Add takes the squeeze-excitation's output as the shortcut")
+        pe = g.one(x, "Conv", True)
         y = pe[2][0]
-        lin = {}
-        for mm in fwd(y, "MatMul", True):
-            w, b, t = linear(mm)
-            lin[t] = (w, b)
+        lin = {t: (w, b) for w, b, t in map(g.linear, g.fwd(y, "MatMul", True))}
         if len(lin) != 3:
-            fail(f"block {i}: {len(lin)} q / k / v projections behind the patch embedding (expected 3)")
+            g.fail(f"block {i}: {len(lin)} q / k / v projections behind the patch embedding (expected 3)")
         users = {}  # the attention MatMul each projection feeds: q and k the scores Q K^T, v the product P V
         for t in lin:
-            u = fwd(t, "MatMul", False)
-            if len(u) != 1:
-                fail(f"block {i}: a q / k / v projection feeds {len(u)} attention products")
-            users.setdefault(id(u[0]), (u[0], []))[1].append(t)
+            u = g.one(t, "MatMul", False)
+            users.setdefault(id(u), (u, []))[1].append(t)
         qk = next((nd for nd, ts in users.values() if len(ts) == 2), None)
         if qk is None:
-            fail(f"block {i}: attention scores Q K^T not found")
-        q, k = (back(a, "Add")[2][0] for a in qk[1])
-        sc = fwd(qk[2][0], "Mul") or fwd(qk[2][0], "Div")
-        s = next((float(inits[a].reshape(-1)[0]) for a in sc[0][1] if a in inits), None) if len(sc) == 1 else None
+            g.fail(f"block {i}: attention scores Q K^T not found")
+        q, k = (g.back(a, "Add")[2][0] for a in qk[1])
+        sc = g.fwd(qk[2][0], "Mul") or g.fwd(qk[2][0], "Div")
+        s = next((float(g.inits[a].reshape(-1)[0]) for a in sc[0][1] if a in g.inits), None) if len(sc) == 1 else None
         if s is None or abs((s if sc[0][0] == "Mul" else 1.0 / s) - 32 ** -0.5) > 1e-6:
-            fail(f"block {i}: attention scale {s} (expected 32^-0.5)")
-        sm = one(sc[0][2][0], "Softmax")
-        pv = one(sm[2][0], "MatMul", False)
-        v = back(pv[1][1], "Add")[2][0]
+            g.fail(f"block {i}: attention scale {s} (expected 32^-0.5)")
+        sm = g.one(sc[0][2][0], "Softmax")
+        pv = g.one(sm[2][0], "MatMul", False)
+        v = g.back(pv[1][1], "Add")[2][0]
         if len({q, k, v}) != 3:
-            fail(f"block {i}: q / k / v not told apart")
-        wp, bp, o = linear(one(pv[2][0], "MatMul", True))
-        y1_add = one(o, "Add")
+            g.fail(f"block {i}: q / k / v not told apart")
+        wp, bp, o = g.linear(g.one(pv[2][0], "MatMul", True))
+        y1_add = g.one(o, "Add")
         if y not in y1_add[1]:
-            fail(f"block {i}: the attention output is not added to the patch embedding")
+            g.fail(f"block {i}: the attention output is not added to the patch embedding")
         y1 = y1_add[2][0]
-        prj = one(y1, "Conv", True)
+        prj = g.one(y1, "Conv", True)
         z = prj[2][0]
-        gc = next((nd for nd in fwd(z, "Conv", True) if W(nd).shape[2] == 3), None)  # (one group when Ca = 32)
+        gc = next((nd for nd in g.fwd(z, "Conv", True) if W(nd).shape[2] == 3), None)  # (one group when Ca = 32)
         if gc is None:
-            fail(f"block {i}: no group convolution behind the projection")
-        mh = one(one(gc[2][0], "Relu")[2][0], "Conv", True)
+            g.fail(f"block {i}: no group convolution behind the projection")
+        mh = g.one(g.one(gc[2][0], "Relu")[2][0], "Conv", True)
         if np.any(bias(mh) != 0):
-            fail(f"block {i}: the MHCA conv1x1 has a bias")
-        z2 = one(mh[2][0], "Add")
-        cat = one(y1, "Concat")
+            g.fail(f"block {i}: the MHCA conv1x1 has a bias")
+        z2 = g.one(mh[2][0], "Add")
+        cat = g.one(y1, "Concat")
         if cat[1] != [y1, z2[2][0]] or z not in z2[1]:
-            fail(f"block {i}: the NTB does not concatenate y1 | z2")
-        m1 = one(cat[2][0], "Conv", True)
-        m2 = one(one(m1[2][0], "Relu")[2][0], "Conv", True)
-        out = one(m2[2][0], "Add")
+            g.fail(f"block {i}: the NTB does not concatenate y1 | z2")
+        m1 = g.one(cat[2][0], "Conv", True)
+        m2 = g.one(g.one(m1[2][0], "Relu")[2][0], "Conv", True)
+        out = g.one(m2[2][0], "Add")
         if cat[2][0] not in out[1]:
-            fail(f"block {i}: the MLP output is not added to the concatenation")
+            g.fail(f"block {i}: the MLP output is not added to the concatenation")
         M, Ca, H = int(W(pe).shape[0]), int(W(prj).shape[0]), int(W(m1).shape[0])
         if W(gc).shape[1] != 32 or W(gc).shape[0] != Ca or gc[3].get("group", 1) != Ca // 32:
-            fail(f"block {i}: group convolution {W(gc).shape} (expected heads of 32 channels)")
+            g.fail(f"block {i}: group convolution {W(gc).shape} (expected heads of 32 channels)")
         tensors += [mat(W(pe)), bias(pe), np.concatenate([lin[q][0], lin[k][0], lin[v][0]]),
                     np.concatenate([lin[q][1], lin[k][1], lin[v][1]]), wp, bp, mat(W(prj)), bias(prj), W(gc), bias(gc),
                     mat(W(mh)), mat(W(m1)), bias(m1), mat(W(m2)), bias(m2)]
         widths.add((M, Ca, H))
-        kernels.append(3), c_ops.append(0), ntb.append(True)
+        kernels.append(3), se_types.append(None), c_ops.append(0), ntb.append(True)
         x = out[2][0]
     if not kernels:
-        fail("no block found")
+        g.fail("no block found")
     if len(widths) > 1:
-        fail(f"NTB blocks of different widths {sorted(widths)}")
-    heads = fwd(x, "Conv", True)
+        g.fail(f"NTB blocks of different widths {sorted(widths)}")
+    if not widths and C != channels:
+        g.fail(f"{C} trunk channels, this engine builds {channels}")
+    heads = g.fwd(x, "Conv", True)
     vconv = [nd for nd in heads if W(nd).shape[2] == 1]
     pconv = [nd for nd in heads if W(nd).shape[2] == 3]
     if len(vconv) != 1 or len(pconv) != 1:
-        fail("value head (1x1 convolution) and policy head (3x3 convolution) not found behind the tower")
+        g.fail("value head (1x1 convolution) and policy head (3x3 convolution) not found behind the tower")
     tensors += [W(vconv[0]), bias(vconv[0])]
-    fc = fwd(one(vconv[0][2][0], "Relu")[2][0], "Gemm", True) or fwd(one(vconv[0][2][0], "Relu")[2][0], "MatMul", True)
-    gw = lambda nd: np.ascontiguousarray(W(nd) if nd[0] == "Gemm" and nd[3].get("transB", 0) else W(nd).T)
+    v = g.one(vconv[0][2][0], "Relu")[2][0]
+    fc = g.fwd(v, "Gemm", True) or g.fwd(v, "MatMul", True)
     wdl = len(fc) == 2
     if wdl:
-        fc = sorted(fc, key=lambda nd: -gw(nd).shape[0])  # WDL (3 outputs), then plies (1)
+        fc = sorted(fc, key=lambda nd: -W(nd).shape[0])  # WDL (3 outputs), then plies (1)
     elif len(fc) == 1:
-        fc = [fc[0], _downstream(cons, fc[0][2][0], ("Gemm", "MatMul"))]
+        fc = [fc[0], g.downstream(fc[0][2][0], ("Gemm", "MatMul"))]
         if fc[1] is None:
-            fail("value head: two fully-connected layers not found")
+            g.fail("value head: two fully-connected layers not found")
     else:
-        fail(f"value head: {len(fc)} fully-connected layers behind the convolution")
+        g.fail(f"value head: {len(fc)} fully-connected layers behind the convolution")
     for nd in fc:
-        tensors += [gw(nd), bias(nd)]
-    p2 = _downstream(cons, pconv[0][2][0], ("Conv",))
+        tensors += [W(nd), bias(nd)]
+    p2 = g.downstream(pconv[0][2][0], ("Conv",))
     if p2 is None:
-        fail("policy head: second convolution not found")
+        g.fail("policy head: second convolution not found")
     tensors += [W(pconv[0]), bias(pconv[0]), W(p2)]
-    M, Ca, H = next(iter(widths)) if widths else (0, 0, 0)
-    arch = dict(name=f"alphavile_{len(kernels)}b", in_channels=int(W(stem).shape[1]), policy_channels=int(W(p2).shape[0]),
-                channels=C, kernels=kernels, se_types=[None] * len(kernels), c_ops=c_ops, ntb=ntb, mhsa=M, mhca=Ca, mlp=H,
-                wdl=wdl, value_channels=int(W(vconv[0]).shape[0]), value_fc=C if wdl else int(gw(fc[0]).shape[0]))
-    write_blob(blob_path, arch, tensors, _input_version(arch, input_version))
+    arch = dict(name=f"rise_{len(kernels)}b", in_channels=int(W(stem).shape[1]), policy_channels=int(W(p2).shape[0]),
+                channels=C, kernels=kernels, se_types=se_types, c_ops=c_ops, wdl=wdl, value_channels=int(W(vconv[0]).shape[0]),
+                value_fc=256)
+    if widths:
+        (M, Ca, H), = widths
+        arch.update(name=f"alphavile_{len(kernels)}b", ntb=ntb, mhsa=M, mhca=Ca, mlp=H,
+                    value_fc=C if wdl else int(W(fc[0]).shape[0]))
+    write_blob(blob_path, arch, tensors, input_version_of(arch, input_version))
     return arch
-
-
-def _downstream(cons, t, ops):
-    """the first node of one of ops reached from tensor t along single-consumer element-wise edges"""
-    seen = set()
-    frontier = [t]
-    while frontier:
-        nxt = []
-        for u in frontier:
-            for nd in cons[u]:
-                if nd[0] in ops:
-                    return nd
-                if id(nd) not in seen:
-                    seen.add(id(nd))
-                    nxt += nd[2]
-        frontier = nxt
-    return None
 
 
 if __name__ == "__main__":

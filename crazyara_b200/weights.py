@@ -36,22 +36,32 @@ def _np(t):
     return np.asarray(t, dtype=np.float64)
 
 
+def _bn_affine(gamma, beta, mean, var, eps):  # an eval-mode BatchNorm as (scale, shift): bn(x) = scale x + shift
+    s = gamma / np.sqrt(var + eps)
+    return s, beta - mean * s
+
+
+def _pre_bn(sd, prefix):  # the state_dict's BatchNorm `prefix` as (scale, shift)
+    return _bn_affine(*(_np(sd[prefix + k]) for k in (".weight", ".bias", ".running_mean", ".running_var")), BN_EPS)
+
+
 def _fold(sd, conv_key, bn_prefix):
-    w = _np(sd[conv_key])
-    g, b = _np(sd[bn_prefix + ".weight"]), _np(sd[bn_prefix + ".bias"])
-    m, v = _np(sd[bn_prefix + ".running_mean"]), _np(sd[bn_prefix + ".running_var"])
-    s = g / np.sqrt(v + BN_EPS)
-    return w * s.reshape(-1, *([1] * (w.ndim - 1))), b - m * s
+    w, (s, b) = _np(sd[conv_key]), _pre_bn(sd, bn_prefix)
+    return w * s.reshape(-1, *([1] * (w.ndim - 1))), b
+
+
+def input_version_of(arch, input_version=None):
+    """input_version, or by default the one the input channel count implies (34/39/63 -> 1.0, 51 -> 2.0, 52/64/80 -> 3.0)"""
+    if input_version is not None:
+        return input_version
+    return {34: 10, 63: 10, 39: 10, 51: 20, 52: 30, 64: 30, 80: 30}.get(arch["in_channels"], 10)
 
 
 def export_blob(sd, arch, path, input_version=10):
     """arch: dict(in_channels, policy_channels, kernels[], se_types[], c_ops[], wdl) as in oracle-free product use;
     see crazyara_b200.nn.ARCH_RISEV2 / ARCH_RISEV33 helpers."""
     tensors = []
-
-    def put(a):
-        tensors.append(np.ascontiguousarray(a, dtype=np.float32).reshape(-1))
-
+    put = tensors.append  # (write_blob writes each as float32)
     w, b = _fold(sd, "body_spatial.0.body.0.weight", "body_spatial.0.body.1")
     put(w), put(b)
     ntb = arch.get("ntb") or [False] * len(arch["kernels"])
@@ -87,13 +97,6 @@ def export_blob(sd, arch, path, input_version=10):
     put(w), put(b)
     put(_np(sd["policy_head.body.3.weight"]))
     return write_blob(path, arch, tensors, input_version)
-
-
-def _pre_bn(sd, prefix):
-    """a BatchNorm in front of a layer as (scale, shift): bn(x) = scale x + shift"""
-    g, b = _np(sd[prefix + ".weight"]), _np(sd[prefix + ".bias"])
-    s = g / np.sqrt(_np(sd[prefix + ".running_var"]) + BN_EPS)
-    return s, b - _np(sd[prefix + ".running_mean"]) * s
 
 
 def ntb_tensors(sd, p):
@@ -154,6 +157,53 @@ def write_blob(path, arch, tensors, input_version):
     return path
 
 
+def read_blob(path):
+    """The inverse of write_blob: an ARAB2001 / 2002 / 2003 blob -> (arch, tensors [flat float32], input_version).  arch
+    holds what the header and block table say, under write_blob's keys; write_blob(path2, *read_blob(path)) rewrites the
+    file byte for byte.  A blob write_blob cannot have written (ARAB2002 block flags other than the ones it sets, an unknown
+    block type, a tensor past the end of the file) is refused."""
+    buf = open(path, "rb").read()
+    magic = buf[:8]
+    if magic not in (b"ARAB2001", b"ARAB2002", b"ARAB2003"):
+        raise ValueError(f"{path}: not an ARAB2001 / 2002 / 2003 blob")
+    mx, v3 = magic == b"ARAB2002", magic == b"ARAB2003"
+    cin, pch, n, C, vc, fc, wdl, version = struct.unpack_from("<8i", buf, 8)
+    arch = dict(in_channels=cin, policy_channels=pch, channels=C, value_channels=vc, value_fc=fc, wdl=bool(wdl),
+                kernels=[], se_types=[], c_ops=[])
+    off = 40
+    if mx or v3:
+        stem_act, policy_bias = struct.unpack_from("<2i", buf, off)
+        arch.update(stem_act=bool(stem_act), policy_bias=bool(policy_bias))
+        off += 8
+    if mx:
+        arch.update(semantics="mxnet", se_gates=[])
+    if v3:
+        arch.update(ntb=[], mhsa=0, mhca=0, mlp=0)
+    width = 4 if v3 else 5 if mx else 3
+    for i in range(n):
+        rec = struct.unpack_from(f"<{width}i", buf, off)
+        off += 4 * width
+        if v3:
+            if rec[0] not in (0, 1):
+                raise ValueError(f"{path}: block {i} has type {rec[0]}")
+            arch["ntb"].append(rec[0] == 1)
+            if rec[0] == 1:
+                arch.update(mhsa=rec[1], mhca=rec[2], mlp=rec[3])
+            rec = (0, 3, 0) if rec[0] == 1 else rec[1:]
+        cop, k, se = rec[:3]
+        if mx:
+            if rec[3] != SHORTCUT_PRE_SE | (SE_BIAS if se == 1 else 0):
+                raise ValueError(f"{path}: block {i} has flags {rec[3]}")
+            arch["se_gates"].append({0: None, 1: "hard_sigmoid", 2: "sigmoid"}[rec[4]])
+        arch["c_ops"].append(cop), arch["kernels"].append(k), arch["se_types"].append({0: None, 1: "ca_se", 2: "eca_se"}[se])
+    tensors = []
+    while off < len(buf):
+        size, = struct.unpack_from("<q", buf, off)
+        tensors.append(np.frombuffer(buf, "<f4", size, off + 8).copy())
+        off += 8 + 4 * size
+    return arch, tensors, version
+
+
 # ---------------------------------------------------------------------------------------------- MXNet symbols
 def mx_bn_prefix(params, prefix):
     """the BatchNorm behind layer `prefix`: `<prefix>` (rise_mobile_v2.py, get_stem, the heads) or `<prefix>_bn1`
@@ -173,8 +223,7 @@ def _mx_fold(params, conv, bn, eps, fix_gamma):
     w = _np(params[conv + "_weight"])
     e = eps.get(bn, MX_BN_EPS) if isinstance(eps, dict) else eps
     g = np.ones(w.shape[0]) if fix_gamma else _np(params[bn + "_gamma"])
-    s = g / np.sqrt(_np(params[bn + "_moving_var"]) + e)
-    b = _np(params[bn + "_beta"]) - _np(params[bn + "_moving_mean"]) * s
+    s, b = _bn_affine(g, _np(params[bn + "_beta"]), _np(params[bn + "_moving_mean"]), _np(params[bn + "_moving_var"]), e)
     if conv + "_bias" in params:  # (the symbols' convolutions in front of a BatchNorm have none)
         b = b + _np(params[conv + "_bias"]) * s
     return w * s.reshape(-1, *([1] * (w.ndim - 1))), b
@@ -293,9 +342,7 @@ def import_checkpoint(checkpoint_path, blob_path, input_version=None):
     sd = ck.get("model_state_dict", ck) if isinstance(ck, dict) else ck
     sd = {k[7:] if k.startswith("module.") else k: v for k, v in sd.items()}  # DataParallel prefix
     arch = arch_from_state_dict(sd)
-    if input_version is None:
-        input_version = {34: 10, 63: 10, 39: 10, 51: 20, 52: 30, 64: 30, 80: 30}.get(arch["in_channels"], 10)
-    export_blob(sd, arch, blob_path, input_version=input_version)
+    export_blob(sd, arch, blob_path, input_version=input_version_of(arch, input_version))
     return arch
 
 

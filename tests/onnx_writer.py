@@ -40,7 +40,11 @@ def _node(op, ins, outs, attrs=()):
     return msg
 
 
-def write_rise_onnx(sd, arch, path):
+def write_rise_onnx(sd, arch, path, shuffle=None, torch_se=False):
+    """shuffle: a seed to write the nodes in a random order, as tests/onnx_mx_writer.py does; torch_se: the
+    squeeze-excitation as torch.onnx.export writes the reference's modules (builder_util.py:86-116), the pooled vector
+    reshaped rather than flattened and the gate broadcast by view() and expand_as(x): GlobalAveragePool -> Reshape, gate ->
+    Reshape -> Expand -> Mul"""
     nodes, inits, n = [], [], [0]
 
     def const(a):
@@ -76,15 +80,18 @@ def write_rise_onnx(sd, arch, path):
         p = f"body_spatial.{i + 1}"
         xin = x
         if se in ("ca_se", "se"):
-            g = unary("Flatten", unary("GlobalAveragePool", x))
+            g = unary("Reshape" if torch_se else "Flatten", unary("GlobalAveragePool", x))
             g = unary("Relu", gemm(g, f32(_np(sd[p + ".se.fc.0.weight"])), None))
             g = unary("HardSigmoid", gemm(g, f32(_np(sd[p + ".se.fc.2.weight"])), None))
-            n[0] += 1
-            nodes.append(_node("Mul", [x, g], [f"t_{n[0]}"]))
-            xin = f"t_{n[0]}"
         elif se == "eca_se":
             g = unary("GlobalAveragePool", x)
             g = unary("HardSigmoid", conv(unary("Reshape", g), f32(_np(sd[p + ".se.body.0.weight"])), f32(_np(sd[p + ".se.body.0.bias"]))))
+        if se:
+            if torch_se:
+                ins = [unary("Reshape", g), unary("Shape", x)]
+                n[0] += 1
+                nodes.append(_node("Expand", ins, [f"t_{n[0]}"]))
+                g = f"t_{n[0]}"
             n[0] += 1
             nodes.append(_node("Mul", [x, g], [f"t_{n[0]}"]))
             xin = f"t_{n[0]}"
@@ -108,8 +115,30 @@ def write_rise_onnx(sd, arch, path):
     w, b = _fold(sd, "policy_head.body.0.weight", "policy_head.body.1")
     y = unary("Relu", conv(x, f32(w), f32(b)))
     unary("Flatten", conv(y, f32(_np(sd["policy_head.body.3.weight"])), None))
+    if shuffle is not None:
+        nodes = [nodes[j] for j in np.random.default_rng(shuffle).permutation(len(nodes))]
     graph = b"".join(_ld(1, nd) for nd in nodes) + _ld(2, b"torch_jit") + b"".join(_ld(5, t) for t in inits)
     model = _vi(1, 8) + _ld(2, b"pytorch") + _ld(7, graph)
     with open(path, "wb") as f:
         f.write(model)
+    return path
+
+
+def add_shape_concat(path):
+    """rewrites the file with the shape arithmetic of a dynamic-batch export in front of a view(): Shape -> Gather ->
+    Unsqueeze -> Concat (with a constant) -> Reshape of the stem's output, the Concat taking no activation"""
+    from crazyara_b200.onnx_import import _fields
+    model = memoryview(open(path, "rb").read())
+    out = b""
+    for f, w, v in _fields(model):
+        if f == 7:
+            first = next(bytes(nv) for nf, nw, nv in _fields(v) if nf == 1)
+            x = next(bytes(gv).decode() for g, gw, gv in _fields(memoryview(first)) if g == 2)  # the stem's output
+            extra = [_node("Shape", [x], ["s_shape"]), _node("Gather", ["s_shape", "s_idx"], ["s_b"]),
+                     _node("Unsqueeze", ["s_b"], ["s_bu"]), _node("Concat", ["s_bu", "s_tail"], ["s_new"], [("axis", 0)]),
+                     _node("Reshape", [x, "s_new"], ["s_view"])]
+            consts = [_tensor("s_idx", np.zeros(1, np.float32)), _tensor("s_tail", np.array([256, 1], np.float32))]
+            v = bytes(v) + b"".join(_ld(1, nd) for nd in extra) + b"".join(_ld(5, t) for t in consts)
+        out += _vi(f, v) if w == 0 else _ld(f, bytes(v))
+    open(path, "wb").write(out)
     return path

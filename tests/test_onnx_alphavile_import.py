@@ -27,38 +27,16 @@ def test_onnx_import_rejects_a_wrong_attention_scale(tmp_path):
         import_onnx(path, str(tmp_path / "x.arab"))
 
 
-def _with_shape_concat(path):
-    """the file with the shape arithmetic of a dynamic-batch export in front of a view(): Shape -> Gather -> Unsqueeze ->
-    Concat (with a constant) -> Reshape, the Concat taking no activation"""
-    import numpy as np
-    from crazyara_b200.onnx_import import _fields
-    from tests.onnx_writer import _ld, _node, _tensor, _vi
-    model = memoryview(open(path, "rb").read())
-    out = b""
-    for f, w, v in _fields(model):
-        if f == 7:
-            first = next(bytes(nv) for nf, nw, nv in _fields(v) if nf == 1)
-            x = next(bytes(gv).decode() for g, gw, gv in _fields(memoryview(first)) if g == 2)  # the stem's output
-            extra = [_node("Shape", [x], ["s_shape"]), _node("Gather", ["s_shape", "s_idx"], ["s_b"]),
-                     _node("Unsqueeze", ["s_b"], ["s_bu"]), _node("Concat", ["s_bu", "s_tail"], ["s_new"], [("axis", 0)]),
-                     _node("Reshape", [x, "s_new"], ["s_view"])]
-            consts = [_tensor("s_idx", np.zeros(1, np.float32)), _tensor("s_tail", np.array([256, 1], np.float32))]
-            v = bytes(v) + b"".join(_ld(1, nd) for nd in extra) + b"".join(_ld(5, t) for t in consts)
-        out += _vi(f, v) if w == 0 else _ld(f, bytes(v))
-    open(path, "wb").write(out)
-    return path
-
-
 @pytest.mark.parametrize("name", ["risev2", "risev33"])
 def test_rise_graph_with_a_shape_concat_still_imports_as_rise(tmp_path, name):
-    """Only a Concat of activations marks an AlphaVile graph: the shape-only Concat a dynamic-batch RISE export carries
-    leaves the RISE import byte-identical to the state-dict import."""
+    """The shape-only Concat a dynamic-batch RISE export carries in front of a view() is not an NTB: the import stays
+    byte-identical to the state-dict import."""
     from crazyara_b200 import synthetic
-    from tests.onnx_writer import write_rise_onnx
+    from tests.onnx_writer import add_shape_concat, write_rise_onnx
     arch = synthetic.risev2(34, 81) if name == "risev2" else synthetic.risev33(52, 76)
     sd = synthetic.random_state_dict(arch, 3)
     ref = export_blob(sd, arch, str(tmp_path / "ref.arab"), input_version=10 if name == "risev2" else 30)
-    path = _with_shape_concat(write_rise_onnx(sd, arch, str(tmp_path / "m.onnx")))
+    path = add_shape_concat(write_rise_onnx(sd, arch, str(tmp_path / "m.onnx")))
     got = import_onnx(path, str(tmp_path / "onnx.arab"))
     assert got["kernels"] == list(arch["kernels"]) and "ntb" not in got
     assert open(ref, "rb").read() == open(tmp_path / "onnx.arab", "rb").read()

@@ -1,6 +1,6 @@
 """AlphaVile on the CPU: the oracle (oracle/net_alphavile.py) against the real reference module's outputs
 (tests/golden/net_alphavile_*.json, written by tests/golden/gen_alphavile_golden.py), architecture recognition, and the
-ARAB2003 blob read back by a NumPy reader that pads the trunk to 256 channels the way Net::read_blob does."""
+ARAB2003 blob read back by weights.read_blob and run with the trunk padded to 256 channels the way Net::read_blob does."""
 import json
 import os
 import struct
@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from crazyara_b200 import synthetic
-from crazyara_b200.weights import arch_from_state_dict, export_blob, import_checkpoint
+from crazyara_b200.weights import arch_from_state_dict, export_blob, import_checkpoint, read_blob
 from oracle import net_alphavile as oav
 from tests.golden.gen_net_golden import golden_input
 
@@ -80,26 +80,7 @@ def test_checkpoint_import_equals_direct_export(tmp_path):
     assert (tmp_path / "a.arab").read_bytes()[:8] == b"ARAB2003"
 
 
-# ------------------------------------------------------------------------------------------- NumPy ARAB2003 reader
-def read_blob3(path):
-    """-> (header dict, blocks [(type, fields)], tensors list) of an ARAB2003 blob"""
-    buf = open(path, "rb").read()
-    assert buf[:8] == b"ARAB2003"
-    h = struct.unpack_from("<10i", buf, 8)
-    off = 48
-    hdr = dict(zip(("cin", "pch", "n", "C", "vc", "fc", "wdl", "ver", "stem_act", "pol_bias"), h))
-    blocks = []
-    for _ in range(hdr["n"]):
-        blocks.append(struct.unpack_from("<4i", buf, off))
-        off += 16
-    tensors = []
-    while off < len(buf):
-        (n,) = struct.unpack_from("<q", buf, off)
-        tensors.append(np.frombuffer(buf, np.float32, n, off + 8).astype(np.float64))
-        off += 8 + 4 * n
-    return hdr, blocks, tensors
-
-
+# ------------------------------------------------------------------------------------------- ARAB2003 read back
 def pad(a, shape):
     o = np.zeros(shape)
     o[tuple(slice(0, s) for s in a.shape)] = a
@@ -109,22 +90,21 @@ def pad(a, shape):
 def blob_forward(path, x):
     """the network an ARAB2003 blob describes, padded to 256 channels, in float64 NumPy / torch"""
     import torch.nn.functional as F
-    hdr, blocks, ts = read_blob3(path)
-    C, cin, P, fc = hdr["C"], hdr["cin"], hdr["pch"], hdr["fc"]
+    arch, ts, _ = read_blob(path)
+    C, cin, P, fc = arch["channels"], arch["in_channels"], arch["policy_channels"], arch["value_fc"]
     it = iter(ts)
-    nxt = lambda *shape: next(it).reshape(shape)
+    nxt = lambda *shape: next(it).astype(np.float64).reshape(shape)
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a))
     conv = lambda x, w, b=None, pd=0, groups=1: F.conv2d(x, T(w), None if b is None else T(b), padding=pd, groups=groups)
     x = torch.as_tensor(x, dtype=torch.float64)
     out = F.relu(conv(x, pad(nxt(C, cin, 3, 3), (256, cin, 3, 3)), pad(nxt(C), (256,)), 1))
-    for ty, a, b, c in blocks:
-        if ty == 0:
-            cop, k = a, b
+    for is_ntb, cop, k in zip(arch["ntb"], arch["c_ops"], arch["kernels"]):
+        if not is_ntb:
             h = F.relu(conv(out, pad(nxt(cop, C, 1, 1), (cop, 256, 1, 1)), nxt(cop)))
             h = F.relu(conv(h, nxt(cop, 1, k, k), nxt(cop), k // 2, cop))
             out = out + conv(h, pad(nxt(C, cop, 1, 1), (256, cop, 1, 1)), pad(nxt(C), (256,)))
             continue
-        M, Ca, H = a, b, c
+        M, Ca, H = arch["mhsa"], arch["mhca"], arch["mlp"]
         y = conv(out, pad(nxt(M, C, 1, 1), (M, 256, 1, 1)), nxt(M))
         qkv = F.conv2d(y, T(nxt(3 * M, M, 1, 1)), T(nxt(3 * M))).flatten(2).transpose(1, 2)  # [B, 64, 3M]
         q, k, v = (qkv[..., i * M:(i + 1) * M].reshape(-1, 64, M // 32, 32).transpose(1, 2) for i in range(3))
@@ -139,7 +119,7 @@ def blob_forward(path, x):
         out = x2 + conv(u, pad(nxt(C, H, 1, 1), (256, H, 1, 1)), pad(nxt(C), (256,)))
     assert torch.count_nonzero(out[:, C:]) == 0
     vh = F.relu(conv(out, pad(nxt(8, C, 1, 1), (8, 256, 1, 1)), nxt(8))).reshape(x.shape[0], -1)
-    if hdr["wdl"]:
+    if arch["wdl"]:
         wdl = vh @ T(nxt(3, 512)).T + T(nxt(3))
         nxt(1, 512), nxt(1)
         sm = torch.softmax(wdl, 1)

@@ -2,18 +2,17 @@
  - always: against tests/golden/mx_net_*.json (outputs of the reference's symbol code evaluated by
    tests/golden/mx_standin.py, written by gen_mx_net_golden.py), parameter names included;
  - where the reference tree is present: live against the symbol code;
- - crazyara_b200.weights.export_mx_blob: a NumPy reading of the blob it writes, with the flags it carries, computes the
-   oracle's network."""
+ - crazyara_b200.weights.export_mx_blob: the blob it writes, read back by weights.read_blob, computes the oracle's
+   network."""
 import json
 import os
-import struct
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from crazyara_b200.weights import eca_band, export_mx_blob
+from crazyara_b200.weights import eca_band, export_mx_blob, read_blob
 from oracle import net_mx
 from tests.golden.gen_mx_net_golden import ARCHS, REFERENCE, reference_symbol_forward
 from tests.golden.gen_net_golden import golden_input
@@ -58,46 +57,35 @@ def test_eca_band_is_the_channel_convolution():
 
 
 def _blob_forward(path, x):
-    """the network an ARAB2002 blob describes (net.cu's reading of it), in torch fp32"""
-    b = open(path, "rb").read()
-    assert b[:8] == b"ARAB2002"
-    h = struct.unpack_from("<10i", b, 8)
-    cin, P, nb, stem_act, policy_bias = h[0], h[1], h[2], h[8], h[9]
-    o = 48
-    blocks = [struct.unpack_from("<5i", b, o + 20 * i) for i in range(nb)]
-    o += 20 * nb
-
-    def t(*shape):
-        nonlocal o
-        n, = struct.unpack_from("<q", b, o)
-        a = np.frombuffer(b, "<f4", n, o + 8).copy()
-        o += 8 + 4 * n
-        return torch.tensor(a).reshape(shape) if shape else torch.tensor(a)
-
-    gates = {0: F.hardsigmoid, 1: lambda y: torch.clamp(0.2 * y + 0.5, 0, 1), 2: torch.sigmoid}
+    """the network an ARAB2002 blob describes (net.cu's reading of it: every block's shortcut from its input before the
+    SE, ca_se with biases), in torch fp32"""
+    arch, tensors, _ = read_blob(path)
+    assert arch["semantics"] == "mxnet"
+    it = iter(tensors)
+    t = lambda *shape: torch.tensor(next(it)).reshape(shape or (-1,))
+    gates = {None: F.hardsigmoid, "hard_sigmoid": lambda y: torch.clamp(0.2 * y + 0.5, 0, 1), "sigmoid": torch.sigmoid}
     x = torch.tensor(x)
-    out = F.conv2d(x, t(256, cin, 3, 3), t(), padding=1)
-    out = F.relu(out) if stem_act else out
-    for cop, k, se, flags, gate in blocks:
+    out = F.conv2d(x, t(256, arch["in_channels"], 3, 3), t(), padding=1)
+    out = F.relu(out) if arch["stem_act"] else out
+    for cop, k, se, gate in zip(arch["c_ops"], arch["kernels"], arch["se_types"], arch["se_gates"]):
         d = out
-        if se == 1:
-            w1, b1 = t(128, 256), t() if flags & 2 else torch.zeros(128)
-            w2, b2 = t(256, 128), t() if flags & 2 else torch.zeros(256)
+        if se == "ca_se":
+            w1, b1, w2, b2 = t(128, 256), t(), t(256, 128), t()
             d = d * gates[gate](F.linear(F.relu(F.linear(d.mean((2, 3)), w1, b1)), w2, b2))[:, :, None, None]
-        elif se == 2:
+        elif se == "eca_se":
             w, bb = t(256, 256), t()
             d = d * gates[gate](F.linear(d.mean((2, 3)), w, bb))[:, :, None, None]
         hh = F.relu(F.conv2d(d, t(cop, 256, 1, 1), t()))
         hh = F.relu(F.conv2d(hh, t(cop, 1, k, k), t(), padding=k // 2, groups=cop))
         hh = F.conv2d(hh, t(256, cop, 1, 1), t())
-        out = hh + (out if flags & 1 else d)
+        out = hh + out
     v = F.relu(F.conv2d(out, t(8, 256, 1, 1), t())).reshape(x.shape[0], -1)
     w1, b1, w2, b2 = t(256, 512), t(), t(1, 256), t()
     v = torch.tanh(F.linear(F.relu(F.linear(v, w1, b1)), w2, b2))[:, 0]
     ph = F.relu(F.conv2d(out, t(256, 256, 3, 3), t(), padding=1))
-    w = t(P, 256, 3, 3)
-    logits = F.conv2d(ph, w, t() if policy_bias else None, padding=1).reshape(x.shape[0], -1)
-    assert o == len(b)
+    w = t(arch["policy_channels"], 256, 3, 3)
+    logits = F.conv2d(ph, w, t() if arch["policy_bias"] else None, padding=1).reshape(x.shape[0], -1)
+    assert next(it, None) is None
     return v.numpy(), logits.numpy()
 
 
