@@ -57,16 +57,27 @@ struct NullWriterFactory {  // fake backend: no planes needed
     ARA_HD Target make(int) const { return Target{}; }
 };
 
-// limits: per tree {simulations, nodes} of this go (ara_search_set_limits), or the settings' for every tree
-__global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const uint2* limits) {
+// What the next go asks of one tree: its limits (ara_search_set_limits, else the settings') and whether it takes part
+// (ara_search_set_active).  Uploaded before every root phase.
+struct TreeLimits {
+    unsigned simulations, nodes;
+    int active;
+};
+
+__global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const TreeLimits* limits) {
     __shared__ WarpScratch ws;
     const TreeDev t = trees[blockIdx.x];
+    const TreeLimits lim = limits[blockIdx.x];
+    if (!lim.active) {  // (the second thread's counters were cleared by begin())
+        if (threadIdx.x == 0) idle_root(t);
+        return;
+    }
     // the subtree kept by ara_search_apply_move is searched on if it is this position, else a new tree starts
     if (!reuse_root(t, sp, &roots[blockIdx.x])) create_root(t, sp, ws, &roots[blockIdx.x]);
     __syncwarp();
     if (threadIdx.x == 0) {
-        t.st->limit_simulations = limits[blockIdx.x].x;
-        t.st->limit_nodes = limits[blockIdx.x].y;
+        t.st->limit_simulations = lim.simulations;
+        t.st->limit_nodes = lim.nodes;
     }
 }
 
@@ -86,10 +97,12 @@ struct CompactInfo {
     int cand;    // its root
     int n_nodes, n_edges;
 };
-__global__ void __launch_bounds__(32) compact_decide_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, CompactInfo* info) {
+// (an idle tree is not searched in this go, and its roots[] entry may be stale: it is left alone)
+__global__ void __launch_bounds__(32) compact_decide_kernel(const TreeDev* trees, SearchParams sp, const Board* roots,
+                                                            const TreeLimits* limits, CompactInfo* info) {
     if (threadIdx.x != 0) return;
     const TreeDev t = trees[blockIdx.x];
-    const int cand = kept_subtree_root(t, &roots[blockIdx.x]);
+    const int cand = limits[blockIdx.x].active ? kept_subtree_root(t, &roots[blockIdx.x]) : -1;
     CompactInfo c;
     c.cand = cand;
     c.n_nodes = t.st->n_nodes;
@@ -333,6 +346,7 @@ class Search {
     int init(Net* net, const SearchParams& sp, int device, int n_trees, int max_nodes);
     int set_position(int tree, const Board& root, const uint64_t* hist_keys, const int16_t* hist_reps, int hist_len);
     int set_limits(int tree, unsigned simulations, unsigned nodes);
+    int set_active(int tree, int active);
     int go();
     int begin();
     int step(int n_batches);
@@ -475,8 +489,9 @@ class Search {
     int* d_keep_n_ = nullptr;
     int* d_keep_e_ = nullptr;
     int* d_ctotal_ = nullptr;
-    std::vector<uint2> h_limits_;  // per tree {simulations, nodes} of the next go
-    uint2* d_limits_ = nullptr;
+    std::vector<TreeLimits> h_limits_;  // per tree, the next go
+    TreeLimits* d_limits_ = nullptr;
+    int n_active_ = 0;  // trees that take part in the current go (begin())
     Board* d_roots_ = nullptr;
     std::vector<Board> h_roots_;
     std::vector<TreeState*> d_states_;
@@ -649,7 +664,7 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     if (mem_.dalloc(&s0.d_trees, n_trees) || mem_.dalloc(&d_roots_, n_trees) || mem_.dalloc(&d_results_, n_trees) || mem_.dalloc(&d_limits_, n_trees) ||
         mem_.dalloc(&d_tstats_, 1) || mem_.dalloc(&s0.d_count, 1) || mem_.dalloc(&d_node_view_, 1))
         return -1;
-    h_limits_.assign(n_trees, make_uint2(sp.simulations, sp.nodes));
+    h_limits_.assign(n_trees, TreeLimits{sp.simulations, sp.nodes, 1});
     for (int i = 0; i < n_trees; ++i) {  // the trees' Dirichlet generators (TreeState::rng)
         const uint32_t x = minstd_seed(sp.seed, i);
         ARA_CUDA_OK(cudaMemcpy(&d_states_[i]->rng, &x, sizeof(x), cudaMemcpyHostToDevice));
@@ -842,9 +857,9 @@ int Search::iterate(int count) {
 // uploads them.
 int Search::compact_pools() {
     bool any = false;
-    for (char a : advanced_) any = any || a != 0;
+    for (size_t i = 0; i < advanced_.size(); ++i)
+        if (advanced_[i] && h_limits_[i].active) any = true, advanced_[i] = 0;  // (an idle tree's move waits for its next go)
     if (!any) return 0;
-    advanced_.assign(n_trees, 0);
     if (d_cinfo_ == nullptr) {
         if (mem_.dalloc(&d_cinfo_, n_trees) || mem_.dalloc(&d_keep_n_, static_cast<size_t>(max_nodes_) + 1) ||
             mem_.dalloc(&d_keep_e_, static_cast<size_t>(max_nodes_) + 1) || mem_.dalloc(&d_ctotal_, 2))
@@ -853,7 +868,7 @@ int Search::compact_pools() {
         for (auto& t : shadow_) t.hdr = nullptr;
     }
     Slot& s0 = slots_[0];
-    if (launch(compact_decide_kernel, n_trees, 32, 0, stream_, s0.d_trees, sp, d_roots_, d_cinfo_)) return -1;
+    if (launch(compact_decide_kernel, n_trees, 32, 0, stream_, s0.d_trees, sp, d_roots_, d_limits_, d_cinfo_)) return -1;
     std::vector<CompactInfo> info(n_trees);
     ARA_CUDA_OK(cudaMemcpyAsync(info.data(), d_cinfo_, sizeof(CompactInfo) * n_trees, cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
@@ -897,6 +912,9 @@ int Search::begin() {
     ARA_CUDA_OK(cudaEventRecord(ev0_, stream_));
     ARA_CUDA_OK(cudaMemcpyAsync(s.d_trees, s.h_trees.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
     ARA_CUDA_OK(cudaMemcpyAsync(d_roots_, h_roots_.data(), sizeof(Board) * n_trees, cudaMemcpyHostToDevice, stream_));
+    ARA_CUDA_OK(cudaMemcpyAsync(d_limits_, h_limits_.data(), sizeof(TreeLimits) * n_trees, cudaMemcpyHostToDevice, stream_));
+    n_active_ = 0;
+    for (const TreeLimits& l : h_limits_) n_active_ += l.active ? 1 : 0;
     if (compact_pools()) return -1;
     if (threads_ == 2) {  // the second thread's views of the trees: same pools, its own batch arrays
         Slot& s1 = slots_[1];
@@ -911,8 +929,12 @@ int Search::begin() {
     }
     const int B = sp.batch_size;
     // root: create, expand, evaluate (set_root_node_predictions), scatter, prepare_node_for_visits (+ Dirichlet)
-    ARA_CUDA_OK(cudaMemcpyAsync(d_limits_, h_limits_.data(), sizeof(uint2) * n_trees, cudaMemcpyHostToDevice, stream_));
-    if (launch(root_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, d_roots_, d_limits_) || pack_expand(s)) return -1;
+    if (launch(root_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, d_roots_, d_limits_)) return -1;
+    if (n_active_ == 0) {  // every tree idle: root_kernel has marked them done, nothing goes to the network
+        ARA_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+    if (pack_expand(s)) return -1;
     // a single-tree search only needs row 0; the new roots of a multi-tree search are packed into the first rows
     if (evaluate(s, n_trees == 1 ? 1 : n_trees * B, stream_, n_trees > 1 ? s.d_count : nullptr, false)) return -1;
     if (launch(scatter_kernel, n_trees * B, 32, 0, stream_, s.d_trees, sp, B, s.values, s.probs, n_labels_) ||
@@ -946,7 +968,7 @@ int Search::step(int n_batches) {
     ARA_CUDA_OK(cudaSetDevice(device_));
     if (!searched_) return set_error("ara_search_step: ara_search_begin has not been called");
     if (n_batches < 1) return set_error("ara_search_step: n_batches %d < 1", n_batches);
-    if (iterate(threads_ == 2 ? 2 * n_batches : n_batches)) return -1;
+    if (n_active_ > 0 && iterate(threads_ == 2 ? 2 * n_batches : n_batches)) return -1;
     const int running = poll_running();
     if (running < 0 || fetch_results()) return -1;  // ara_search_result between steps shows the tree as it is now
     return running;
@@ -1048,7 +1070,14 @@ int Search::set_limits(int tree, unsigned simulations, unsigned nodes) {
     if (tree < -1 || tree >= n_trees) return set_error("ara_search_set_limits: tree %d out of range", tree);
     if (simulations == 0 && nodes == 0) return set_error("ara_search_set_limits: neither Simulations nor Nodes given");
     for (int i = 0; i < n_trees; ++i)
-        if (tree < 0 || tree == i) h_limits_[i] = make_uint2(simulations, nodes);
+        if (tree < 0 || tree == i) h_limits_[i].simulations = simulations, h_limits_[i].nodes = nodes;
+    return 0;
+}
+
+int Search::set_active(int tree, int active) {
+    if (tree < -1 || tree >= n_trees) return set_error("ara_search_set_active: tree %d out of range", tree);
+    for (int i = 0; i < n_trees; ++i)
+        if (tree < 0 || tree == i) h_limits_[i].active = active ? 1 : 0;
     return 0;
 }
 
@@ -1165,6 +1194,10 @@ extern "C" int ara_search_apply_move(ara_search_t h, int tree, unsigned short mo
 extern "C" int ara_search_set_limits(ara_search_t h, int tree, unsigned simulations, unsigned nodes) {
     if (h == nullptr) return ara::set_error("ara_search_set_limits: null handle");
     return reinterpret_cast<Search*>(h)->set_limits(tree, simulations, nodes);
+}
+extern "C" int ara_search_set_active(ara_search_t h, int tree, int active) {
+    if (h == nullptr) return ara::set_error("ara_search_set_active: null handle");
+    return reinterpret_cast<Search*>(h)->set_active(tree, active);
 }
 
 extern "C" int ara_search_stop(ara_search_t h) {

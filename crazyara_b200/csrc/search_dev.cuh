@@ -1537,6 +1537,15 @@ ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* roo
     return ok;
 }
 
+// The root phase of a tree left out of a go (ara_search_set_active), in place of reuse_root / create_root: the tree, its
+// Dirichlet generator and a candidate root kept by advance_root stay as they are.  `done` makes every later kernel of
+// the go pass the tree by; the mini-batch counters are cleared because the root phase's scatter / backup / prepare steps
+// and pack_kernel read them, and left over from the tree's last mini-batch they would apply that batch again.  Lane 0.
+ARA_HD void idle_root(const TreeDev& t) {
+    t.st->done = 1;
+    t.bs->n_new = t.bs->n_coll = t.bs->n_exp = 0;
+}
+
 // second half: after expand_pending + network + scatter_pending + backup_results (root trajectory is empty)
 ARA_HD void finalize_root(const TreeDev& t, const SearchParams& sp, WarpScratch& ws) {
     if (ARA_LANE == 0 && !t.st->done && !t.st->error) {

@@ -126,6 +126,7 @@ def _L():
         L.ara_time_continue_search.argtypes = [vp, ctypes.c_double, ctypes.c_float, vp, vp]
         L.ara_search_set_movetime.argtypes = [vp, ctypes.c_double]
         L.ara_search_set_limits.argtypes = [vp, ci, ctypes.c_uint, ctypes.c_uint]
+        L.ara_search_set_active.argtypes = [vp, ci, ci]
         L.ara_search_profile.argtypes = [vp] + [vp] * 4
         L.ara_search_last_go_ms.restype = ctypes.c_double
         L.ara_search_last_go_ms.argtypes = [vp]
@@ -384,6 +385,12 @@ class MCTSAgent:
     def set_search_limits(self, simulations, nodes, tree=-1):
         """SearchLimits::simulations / nodes of the following searches of `tree` (-1 = all trees) instead of the settings'."""
         check(_L().ara_search_set_limits(self._h, int(tree), int(simulations), int(nodes)))
+
+    def set_active(self, tree, active=True):
+        """Leave `tree` (-1 = all trees) out of the following searches, or take it back in (ara_search_set_active).  An
+        idle tree keeps its statistics, its root noise generator, its last result and a subtree kept by
+        apply_move_to_tree, and costs the network batch nothing."""
+        check(_L().ara_search_set_active(self._h, int(tree), int(bool(active))))
 
     def set_profile(self, on=True):
         check(_L().ara_search_set_profile(self._h, int(on)))

@@ -15,8 +15,9 @@ Per game, SelfPlay::generate_game (selfplay.cpp:192-261) with the RL defaults of
     exported q is EvalInfo::bestMoveQ[0] (traindataexporter.cpp:50-53);
   * a game may be resigned (Centi_Resign_Probability of the games, Centi_Resign_Threshold, :163-190).
 Every game may have its own variant (a MODE_LICHESS build plays whatever UCI_Variant is set, selfplay.cpp:367-385):
-`variant` may be a list, one entry per game (cycled).  Not reproduced: quick searches (off in rl_config), opening plies
-sampled from the raw policy (MeanInitPly 0 in rl_config), EPD start positions.
+`variant` may be a list, one entry per game (cycled).  Games may start from random lines of an EPD file (`epd_path`,
+load_random_fen, selfplay.cpp:58-79).  Not reproduced: quick searches (off in rl_config), opening plies sampled from the
+raw policy (MeanInitPly 0 in rl_config).
 Optional outputs: training samples (`exporter=`, crazyara_b200.export) and the games as PGN (`pgn_path=`).
 """
 import os
@@ -84,11 +85,74 @@ def quantile_clip(p, quantile):
     return q / q.sum()
 
 
+def set_best_move(res, ply, rng, temperature, temperature_moves, temperature_decay=0.92, quantile_clipping=0.0):
+    """Agent::set_best_move (agents/agent.cpp:38-53): index of the move to play from a search result at game ply `ply`"""
+    pol = res["policy"]
+    if ply < temperature_moves and temperature > 0.01 and pol.sum() > 0:
+        temp = temperature * temperature_decay ** ply        # get_current_temperature (playsettings.cpp:31-34)
+        p = np.power(pol, 1.0 / temp)                         # apply_temperature (blazeutil.h:78-88)
+        p = p / p.sum()
+        if quantile_clipping != 0:                            # apply_quantile_clipping (agent.cpp:118-127)
+            p = quantile_clip(p, quantile_clipping)
+        return int(rng.choice(len(p), p=p))
+    return int(res["best_idx"])
+
+
+def load_random_fen(path, rng):
+    """load_random_fen (rl/selfplay.cpp:58-79): a line of the EPD file `path` drawn uniformly, without a trailing ';'.
+    No path (None, "" or the reference's "<empty>") gives "", the variant's start position."""
+    if not path or path == "<empty>":
+        return ""
+    with open(path) as f:
+        lines = f.read().splitlines()
+    if not lines:
+        raise ValueError(f"{path}: no positions")
+    line = lines[int(rng.integers(len(lines)))]
+    return line[:-1] if line.endswith(";") else line
+
+
+def start_fen(rng, variant, is960, epd_path=None):
+    """FEN of a new game: a random EPD line, else a random chess960 set-up (chess only), else "" (the start position)."""
+    fen = load_random_fen(epd_path, rng)
+    if not fen and is960 and variant == 0:
+        fen = chess960_fen(rng)
+    return fen
+
+
+def game_result(term, stm_at_end):
+    """WHITE_WIN / BLACK_WIN / DRAWN of a game that ended with TerminalType `term`, `stm_at_end` (0 white) to move: that
+    side lost (mate, variant loss) or won (variant win); everything else is a draw"""
+    if term == TERMINAL_LOSS:
+        return BLACK_WIN if stm_at_end == 0 else WHITE_WIN
+    if term == TERMINAL_WIN:
+        return WHITE_WIN if stm_at_end == 0 else BLACK_WIN
+    return DRAWN
+
+
+def search_concurrently(agents):
+    """evaluate_board_state of every agent, each from its own host thread: the C call releases the GIL, so one agent's
+    tree kernels run while another agent's network forward does"""
+    errors = []
+
+    def go(a):
+        try:
+            a.evaluate_board_state()
+        except Exception as e:  # noqa: BLE001 -- re-raised below on the calling thread
+            errors.append(e)
+    threads = [threading.Thread(target=go, args=(a,)) for a in agents]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    if errors:
+        raise errors[0]
+
+
 class Arena:
     def __init__(self, net, settings, variant, n_games, device=0, is960=False, temperature=0.8, temperature_moves=15,
                  max_plies=512, seed=0, max_nodes=0, exporter=None, reuse_tree=False, pgn_path=None,
                  temperature_decay=0.92, quantile_clipping=0.0, policy_clip_thresh=0.01, node_random_factor=0.1,
-                 resign_probability=0.9, resign_threshold=-0.9):
+                 resign_probability=0.9, resign_threshold=-0.9, epd_path=None):
         # one variant for all games, or one per game (cycled): KOTH + Three-check mixed = variant=[2, 3]
         self.variants = [int(v) for v in variant] if isinstance(variant, (list, tuple)) else [int(variant)]
         self.variant, self.is960 = self.variants[0], is960
@@ -98,6 +162,7 @@ class Arena:
         self.policy_clip_thresh, self.node_random_factor = policy_clip_thresh, node_random_factor
         self.resign_probability, self.resign_threshold = resign_probability, resign_threshold
         self.rng = np.random.default_rng(seed)
+        self.epd_path = epd_path
         # every process / group of games draws its own root noise: the trees' Dirichlet generators start from
         # settings.seed ^ tree index (TreeState::rng), so the groups get distinct seeds derived from the arena's
         import copy
@@ -145,35 +210,19 @@ class Arena:
     def _new_state(self, t):
         # BoardState::init (boardstate.cpp:260-270): chess960 games start from a random chess960 position
         v = self.game_variant[t]
-        if self.is960 and v == 0:
-            return BoardState().set(chess960_fen(self.rng), True, 0)
-        return BoardState().set("", self.is960, v)
+        return BoardState().set(start_fen(self.rng, v, self.is960, self.epd_path), self.is960, v)
 
     def _draw_resign(self):
         # SelfPlay::is_resignation_allowed (selfplay.cpp:163-168): decided once per game
         return self.resign_probability >= 0.01 and self.rng.random() < self.resign_probability
 
     def _pick(self, res, ply):
-        """Agent::set_best_move (agents/agent.cpp:38-53)"""
-        pol = res["policy"]
-        if ply < self.temperature_moves and self.temperature > 0.01 and pol.sum() > 0:
-            temp = self.temperature * self.temperature_decay ** ply   # get_current_temperature (playsettings.cpp:31-34)
-            p = np.power(pol, 1.0 / temp)                             # apply_temperature (blazeutil.h:78-88)
-            p = p / p.sum()
-            if self.quantile_clipping != 0:                           # apply_quantile_clipping (agent.cpp:118-127)
-                p = quantile_clip(p, self.quantile_clipping)
-            return int(self.rng.choice(len(p), p=p))
-        return int(res["best_idx"])
+        return set_best_move(res, ply, self.rng, self.temperature, self.temperature_moves, self.temperature_decay,
+                             self.quantile_clipping)
 
     def _game_over(self, t, term, stm_at_end):
         self.finished.append((self.plies[t], term, stm_at_end))
-        # the side to move at the end lost (mate, variant loss) or won (variant win); everything else is a draw
-        if term == TERMINAL_LOSS:
-            result = BLACK_WIN if stm_at_end == 0 else WHITE_WIN
-        elif term == TERMINAL_WIN:
-            result = WHITE_WIN if stm_at_end == 0 else BLACK_WIN
-        else:
-            result = DRAWN
+        result = game_result(term, stm_at_end)
         if self.exporter is not None:
             self.exporter.export_game_samples(self.records[t], result)
             self.records[t] = self.exporter.new_game()
@@ -200,21 +249,8 @@ class Arena:
         if len(self.agents) == 1:
             self.agent.evaluate_board_state()
             self.search_ms += self.agent.last_go_ms()
-        else:  # the C call releases the GIL: the groups' searches overlap on the device
-            errors = []
-
-            def go(a):
-                try:
-                    a.evaluate_board_state()
-                except Exception as e:  # noqa: BLE001 -- re-raised below on the calling thread
-                    errors.append(e)
-            threads = [threading.Thread(target=go, args=(a,)) for a in self.agents]
-            for th in threads:
-                th.start()
-            for th in threads:
-                th.join()
-            if errors:
-                raise errors[0]
+        else:
+            search_concurrently(self.agents)
             self.search_ms += (time.perf_counter() - t_search) * 1e3
         planes = None
         if self.exporter is not None:  # un-normalised planes of every searched position, one GPU call

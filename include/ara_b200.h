@@ -190,6 +190,14 @@ int ara_search_set_position(ara_search_t s, int tree, const ara_board_t* root, c
  * handle was created for (ara_search_create max_nodes).  Self-play jitters the node budget of every search
  * (SelfPlay::adjust_node_count, rl/selfplay.cpp:146-152). */
 int ara_search_set_limits(ara_search_t s, int tree, unsigned simulations, unsigned nodes);
+/* tree -1 = every tree.  An inactive tree is left out of the following ara_search_begin / step / go calls until it is
+ * made active again; new handles start with every tree active.  The set is read when a search begins.  An idle tree is
+ * not touched: its statistics, its Dirichlet generator and a subtree kept by ara_search_apply_move stay as they are
+ * (a second apply_move still descends from that subtree), it adds no row to the network batch, and ara_search_result
+ * gives its last search's result (n_moves 0 if it has never searched).  With every tree idle no network forward runs
+ * and step / go report 0 trees running.  A match between two networks uses this: each player's handle searches only
+ * the games in which that player is to move (crazyara_b200/match.py). */
+int ara_search_set_active(ara_search_t s, int tree, int active);
 /* runs all trees to their limits (synchronous) and fetches the results */
 int ara_search_go(ara_search_t s);
 int ara_search_result(ara_search_t s, int tree, ara_search_result_t* out);
