@@ -311,9 +311,14 @@ struct SelectStep {
 };
 
 struct SelectPick {
-    int ci;        // winning child index (same in every lane)
-    bool owner;    // this lane holds the winning edge in `x`
+    int ci;         // winning child index (same in every lane)
+    bool owner;     // this lane holds the winning edge in `x`
     EdgeRegs x;
+    // set by pick_child: what the pick adds to sum_select_k, and the node's header refresh after the visit
+    int counted_k;
+    uint32_t vs_new;  // visit_sum + 1, its cput and sqrt
+    float cput_new;
+    double sqrt_new;
 };
 
 // Exact arithmetic of the reference (get_current_u_values, node.cpp:1056-1063): the blaze expression
@@ -391,32 +396,60 @@ ARA_HD SelectPick pick_fast(const TreeDev& t, const NodeHdr& h, const EdgeRegs& 
     return r;
 }
 
-// forced >= 0: the child index was chosen by the exploration prologue (eps_prologue) -- no selection, the visit only
-ARA_HD SelectStep select_and_visit(const TreeDev& t, const SearchParams& sp, int nid, const NodeHdr& h,
-                                   const EdgeRegs& pre, int forced = -1) {
-    NodeHdr* hp = &t.hdr[nid];
+// The child select_child_node picks at a node with header `h` (`pre`: this lane's edge).  forced >= 0: the child index
+// was chosen by the exploration prologue (eps_prologue) -- no selection, the visit only.
+ARA_HD SelectPick pick_child(const TreeDev& t, const SearchParams& sp, const NodeHdr& h, const EdgeRegs& pre, int forced) {
     const int k = h.no_visit_idx;
-    const uint32_t e = h.edge_base;
     const bool single = forced >= 0 || k == 1 || h.checkmate_idx != kNoCheckmate;
-    ARA_FINE_T0(tf);
-    // (prefetching every open child's header and edge lines here was measured: 2 % slower, the issue slots cost more
-    // than the earlier start of the round trip saves)
     // header refresh values, off the dependent chain
     const uint32_t vs_new = h.visit_sum + 1;
     const float cput_new = current_cput(t, sp, vs_new);
     const double sqrt_new = sqrt_visits(t, vs_new);
-    ARA_FINE(t.st, 4, tf, pre.c ^ static_cast<int>(pre.n) ^ __double2hiint(sqrt_new));
     SelectPick pk;
     if (single) {  // only one open child, or a forced win
         pk.ci = forced >= 0 ? forced : (k == 1 ? 0 : h.checkmate_idx);
         pk.owner = ARA_LANE == (pk.ci & (ARA_WARP_N - 1));
         pk.x = pre;
-        if (pk.owner && pk.ci != ARA_LANE) pk.x = load_edge(t, e + pk.ci);
+        if (pk.owner && pk.ci != ARA_LANE) pk.x = load_edge(t, h.edge_base + pk.ci);
     } else {
         bool sure = false;
         pk = pick_fast(t, h, pre, &sure);
         if (!sure) pk = pick_exact(t, h, pre);
     }
+    // (sum_select_k counts what select_child_node reads: nothing for a forced child, nor for its two shortcuts)
+    pk.counted_k = single ? 0 : k;
+    pk.vs_new = vs_new;
+    pk.cput_new = cput_new;
+    pk.sqrt_new = sqrt_new;
+    return pk;
+}
+
+// The virtual visit of the picked child of node `nid`: apply_virtual_loss_to_child on the owner lane (registers in,
+// stores out), and the header refresh on lane 0.
+ARA_HD void apply_visit(const TreeDev& t, const SearchParams& sp, int nid, const NodeHdr& h, const SelectPick& pk) {
+    if (pk.owner) {
+        const uint32_t ee = h.edge_base + static_cast<uint32_t>(pk.ci);
+        if (virtual_style_of(sp, pk.x.n) == VS_VIRTUAL_LOSS)
+            t.Q[ee] = static_cast<float>((static_cast<double>(pk.x.q) * pk.x.n - 1) / static_cast<double>(pk.x.n + 1));
+        t.N[ee] = pk.x.n + 1;
+        t.vl[ee] = static_cast<uint8_t>(pk.x.vl + 1);
+    }
+    if (ARA_LANE == 0) {
+        NodeHdr* hp = &t.hdr[nid];
+        hp->visit_sum = pk.vs_new;
+        hp->cput = pk.cput_new;
+        hp->sqrt_vs = pk.sqrt_new;
+        if (!(h.flags & NF_HAS_D)) hp->flags = h.flags | NF_HAS_D | NF_SORTED;  // prepare_node_for_visits (lazy flag)
+    }
+}
+
+ARA_HD SelectStep select_and_visit(const TreeDev& t, const SearchParams& sp, int nid, const NodeHdr& h,
+                                   const EdgeRegs& pre, int forced = -1) {
+    ARA_FINE_T0(tf);
+    // (prefetching every open child's header and edge lines here was measured: 2 % slower, the issue slots cost more
+    // than the earlier start of the round trip saves)
+    ARA_FINE(t.st, 4, tf, pre.c ^ static_cast<int>(pre.n));
+    const SelectPick pk = pick_child(t, sp, h, pre, forced);
     SelectStep r;
     r.ci = pk.ci;
     const int owner_lane = pk.ci & (ARA_WARP_N - 1);
@@ -431,22 +464,9 @@ ARA_HD SelectStep select_and_visit(const TreeDev& t, const SearchParams& sp, int
 #if defined(ARA_PROF_FINE)
     ARA_FINE(t.st, 5, tf, r.child >= 0 ? (r.ch.flags ^ r.pre.c) : 0);
 #endif
-    if (pk.owner) {
-        // apply_virtual_loss_to_child on the owner lane: registers in, stores out
-        const uint32_t ee = e + static_cast<uint32_t>(pk.ci);
-        if (virtual_style_of(sp, pk.x.n) == VS_VIRTUAL_LOSS)
-            t.Q[ee] = static_cast<float>((static_cast<double>(pk.x.q) * pk.x.n - 1) / static_cast<double>(pk.x.n + 1));
-        t.N[ee] = pk.x.n + 1;
-        t.vl[ee] = static_cast<uint8_t>(pk.x.vl + 1);
-    }
-    if (ARA_LANE == 0) {
-        // (sum_select_k counts what select_child_node reads: nothing for a forced child, nor for its two shortcuts)
-        if (!single) t.st->sum_select_k += static_cast<unsigned long long>(k);
-        hp->visit_sum = vs_new;
-        hp->cput = cput_new;
-        hp->sqrt_vs = sqrt_new;
-        if (!(h.flags & NF_HAS_D)) hp->flags = h.flags | NF_HAS_D | NF_SORTED;  // prepare_node_for_visits (lazy flag)
-    }
+    apply_visit(t, sp, nid, h, pk);
+    // (last: placed ahead of the look-ahead loads, its shared-memory round trip delayed them -- measured 1.6 % slower)
+    if (ARA_LANE == 0) t.st->sum_select_k += static_cast<unsigned long long>(pk.counted_k);
     return r;
 }
 
@@ -1099,42 +1119,156 @@ ARA_HD void eps_prologue(const TreeDev& t, const SearchParams& sp, WarpScratch& 
     ARA_WARP_SYNC();
 }
 
+// ------------------------------------------------------------------ the steps of create_mini_batch shared by both select
+// kernels: create_mini_batch_impl below (one warp per tree) and wave_mini_batch (search_wave.cuh, a wavefront of warps)
+ARA_HD void clear_batch(BatchState& bs) { bs.n_new = bs.n_coll = bs.n_exp = 0; }
+
+// A search begins on the tree's root: the settings' SearchLimits (root_kernel applies the tree's own), every logical
+// thread live, the counters at zero.  pre_nodes: EvalInfo::nodesPreSearch.  Lane 0.
+ARA_HD void begin_search(TreeState& st, BatchState& bs, const SearchParams& sp, unsigned pre_nodes) {
+    clear_batch(bs);
+    bs.done = 0;
+    st.live_threads = sp.threads == 2 ? 2 : 1;
+    st.limit_simulations = sp.simulations;
+    st.limit_nodes = sp.nodes;
+    st.done = 0;
+    st.iterations = 0;
+    st.evals = 0;
+    st.pre_nodes = pre_nodes;
+    st.sum_select_k = 0;
+    st.sum_depth = 0;
+    for (int i = 0; i < 8; ++i) st.prof[i] = 0;
+}
+
+// run_search_thread loop condition (searchthread.cpp:326-340, :418-426), checked before every mini-batch.  True: this
+// thread makes no mini-batch now and its counters are cleared.  A thread whose condition fails leaves its loop for good,
+// like a returning run_search_thread; the search is over when the last thread has left.  Stores on lane 0.
+ARA_HD bool thread_loop_ends(const TreeDev& t, const SearchParams& sp) {
+    TreeState& st = *t.st;
+    BatchState& bs = *t.bs;
+    if (st.done || st.error || bs.done) {
+        if (ARA_LANE == 0) clear_batch(bs);
+        return true;
+    }
+    const NodeHdr& r = t.hdr[st.root];
+    const uint32_t node_count = r.visit_sum - r.free_visits;
+    const bool limits_ok = (st.limit_nodes == 0 || node_count < st.limit_nodes) &&
+                           (st.limit_simulations == 0 || r.visit_sum < st.limit_simulations);
+    // (a pool sized for a visit budget can never trip the last test before the budget does; it only ends
+    // time-limited searches whose pool is exhausted before their time)
+    const bool pool_ok = st.n_nodes + 3 * sp.batch_size + 8 <= t.max_nodes;
+    if (!(limits_ok && r.node_type == NT_UNSOLVED) || r.n_moves <= 1 || !pool_ok) {
+        if (ARA_LANE == 0) {
+            bs.done = 1;
+            clear_batch(bs);
+            if (--st.live_threads <= 0) st.done = 1;
+        }
+        return true;
+    }
+    return false;
+}
+
+// A step of the descent from node `cur` (header `h`) to its child `ci`, at ply `depth` below the root: the trajectory
+// entry, and the node's key for the repetition scan.  Indexed by the ply below the root even when the trajectory starts
+// deeper (EPS): the backup kernel gives every ply its own lane, which is what keeps two trajectories' updates of one node
+// in order.  Lane 0.
+ARA_HD void record_step(WarpScratch& ws, int depth, int cur, int ci, const NodeHdr& h) {
+    ws.traj_node[depth] = cur;
+    ws.traj_ci[depth] = static_cast<uint16_t>(ci);
+    ws.traj_edge[depth] = h.edge_base + static_cast<uint32_t>(ci);
+    ws.path_key[depth] = h.key;
+    ws.path_rep[depth] = h.repetition;
+}
+
+// The position of a new leaf, child `ci` of node `cur` (header `h`), into ws.child.  It was usually prepared by a
+// parallel warp after the previous mini-batch (prepare_child), and then its verdict is returned as well; otherwise
+// (second expansion of a node within one mini-batch) the move is made here and -1 returned: leaf_verdict is still to
+// run.  *slot_out / *prepared_out: the prepared-child slot, for commit_parent.  Warp-collective.
+ARA_HD int leaf_board(const TreeDev& t, WarpScratch& ws, int cur, int ci, const NodeHdr& h, int* slot_out,
+                      bool* prepared_out) {
+    // (slot index, verdict and board are fetched together, speculatively: one round trip)
+    const int slot = cur * kPrepSlots + (ci % kPrepSlots);
+    const int slot_ci = t.prep_ci[slot];
+    const int slot_tt = t.prep_term[slot];
+#if defined(__CUDA_ARCH__)
+    uint4 slot_b = make_uint4(0u, 0u, 0u, 0u);
+    if (ARA_LANE < 8) slot_b = reinterpret_cast<const uint4*>(&t.prep_board[slot])[ARA_LANE];
+#endif
+    const bool prepared = slot_ci == ci;
+    *slot_out = slot;
+    *prepared_out = prepared;
+    if (prepared) {
+#if defined(__CUDA_ARCH__)
+        if (ARA_LANE < 8) reinterpret_cast<uint4*>(&ws.child)[ARA_LANE] = slot_b;
+        ARA_WARP_SYNC();
+#else
+        ws.child = t.prep_board[slot];
+#endif
+        return slot_tt;
+    }
+    copy_board(&ws.child, &t.board[cur]);
+    if (ARA_LANE == 0) do_move(ws.child, t.move[h.edge_base + ci]);
+    ARA_WARP_SYNC();
+    return -1;
+}
+
+// The parent's share of the expansion of one of its children: increment_no_visit_idx opens the next-best sibling (its
+// edge slots are pre-initialised), the prepared slot the child came from is used up, and the parent is listed in
+// exp_parent for prepare_item.  Lane 0; n_exp counts the mini-batch's exp_parent entries.
+ARA_HD void commit_parent(const TreeDev& t, int cur, const NodeHdr& h, int slot, bool prepared, int& n_exp, int B) {
+    if (h.no_visit_idx < h.n_moves) t.hdr[cur].no_visit_idx = static_cast<uint16_t>(h.no_visit_idx + 1);
+    if (prepared) t.prep_ci[slot] = -1;
+    if (n_exp < 3 * B) t.exp_parent[n_exp++] = cur;
+}
+
+// The end of a playout of `type` (0 new leaf, 1 collision, 2 terminal) that reached `leaf`, `depth` plies below the
+// root, with its trajectory in ws.traj_* from ply `start` on.  A terminal is backed up at once, for free, sequentially
+// leaf -> root because the MCTS solver propagates bottom-up; the others become trajectory `row` of the mini-batch, which
+// backup_results backs up or reverts.  Warp-collective.
+ARA_HD void store_trajectory(const TreeDev& t, const SearchParams& sp, WarpScratch& ws, int type, int row, int start,
+                             int depth, int leaf) {
+    if (type == 2) {
+        if (ARA_LANE == 0) {
+            t.st->sum_depth += static_cast<unsigned long long>(depth);
+            backup_value(t, sp, node_value(t.hdr[leaf]), ws.traj_node + start, ws.traj_ci + start, depth - start, true,
+                         sp.mcts_solver != 0);
+        }
+        return;
+    }
+    for (int i = start + ARA_LANE; i < depth; i += ARA_WARP_N) {
+        t.traj_node[row * kMaxDepth + i] = ws.traj_node[i];
+        t.traj_ci[row * kMaxDepth + i] = ws.traj_ci[i];
+        t.traj_edge[row * kMaxDepth + i] = ws.traj_edge[i];
+    }
+    if (ARA_LANE == 0) {
+        t.st->sum_depth += static_cast<unsigned long long>(depth);
+        t.traj_len[row] = depth;
+        if (type == 0) t.new_node[row] = leaf;
+    }
+}
+
+// What the mini-batch hands to the steps after the select, and the search's counters.  Lane 0.
+ARA_HD void end_mini_batch(TreeState& st, BatchState& bs, int n_new, int n_coll, int n_exp) {
+    bs.n_new = n_new;
+    bs.n_coll = n_coll;
+    bs.n_exp = n_exp;
+    st.iterations++;
+    st.evals += static_cast<unsigned>(n_new);
+}
+
 // ------------------------------------------------------------------ one mini-batch: SearchThread::create_mini_batch
 // Sequential per tree (one warp).  New leaves are only created here (expand_node_seq); their move lists, edges and
 // input planes are produced afterwards by expand_pending, one warp per leaf.
 // EPS: epsilon-greedy / epsilon-check exploration compiled in (its own instantiation: the ordinary descent stays as lean
 // as it is).  With it a playout may start below the root: `depth` counts plies below the root (path keys, repetition),
-// `tlen` the trajectory entries (what is stored and backed up).
+// `skipped` the plies above the trajectory (which is what is stored and backed up).
 template <bool EPS>
 ARA_HD void create_mini_batch_impl(const TreeDev& t, const SearchParams& sp, WarpScratch& ws) {
+    if (thread_loop_ends(t, sp)) return;
     TreeState& st = *t.st;
-    BatchState& bs = *t.bs;  // (global memory: touched at the start and the end only)
-    int n_exp = 0;           // lane 0's count of exp_parent entries
-    if (st.done || st.error || bs.done) {
-        if (ARA_LANE == 0) bs.n_new = 0, bs.n_coll = 0, bs.n_exp = 0;
-        return;
-    }
-    // run_search_thread loop condition (searchthread.cpp:326-340, :418-426), checked before every iteration
-    {
-        const NodeHdr& r = t.hdr[st.root];
-        const uint32_t node_count = r.visit_sum - r.free_visits;
-        const bool limits_ok = (st.limit_nodes == 0 || node_count < st.limit_nodes) &&
-                               (st.limit_simulations == 0 || r.visit_sum < st.limit_simulations);
-        // (a pool sized for a visit budget can never trip the last test before the budget does; it only ends
-        // time-limited searches whose pool is exhausted before their time)
-        const bool pool_ok = st.n_nodes + 3 * sp.batch_size + 8 <= t.max_nodes;
-        if (!(limits_ok && r.node_type == NT_UNSOLVED) || r.n_moves <= 1 || !pool_ok) {
-            // this thread leaves its loop (for good, like a returning run_search_thread); the search is over when the
-            // last thread has left
-            if (ARA_LANE == 0) {
-                bs.done = 1, bs.n_new = 0, bs.n_coll = 0, bs.n_exp = 0;
-                if (--st.live_threads <= 0) st.done = 1;
-            }
-            return;
-        }
-    }
     const int B = sp.batch_size;
     int n_new = 0, n_coll = 0, n_term = 0;
+    int n_exp = 0;  // lane 0's count of exp_parent entries
     while (n_new < B && n_coll != B && n_term < 2 * B) {
         int cur = st.root, depth = 0, type = -1, leaf = -1;  // type: 0 new, 1 collision, 2 terminal
         int forced = -1, skipped = 0;  // EPS: first child forced by the prologue; plies skipped above the trajectory
@@ -1156,50 +1290,15 @@ ARA_HD void create_mini_batch_impl(const TreeDev& t, const SearchParams& sp, War
             forced = -1;
             const int ci = step.ci;
             const int next = step.child;
-            if (ARA_LANE == 0) {
-                // (indexed by the ply below the root even when the trajectory starts deeper -- EPS --: the backup kernel
-                // gives every ply its own lane, which is what keeps two trajectories' updates of one node in order)
-                ws.traj_node[depth] = cur;
-                ws.traj_ci[depth] = static_cast<uint16_t>(ci);
-                ws.traj_edge[depth] = h.edge_base + static_cast<uint32_t>(ci);
-                ws.path_key[depth] = h.key;
-                ws.path_rep[depth] = h.repetition;
-            }
+            if (ARA_LANE == 0) record_step(ws, depth, cur, ci, h);
             ARA_WARP_SYNC();
             depth++;
             if (next < 0) {
                 ARA_PROF(st, 0, tq);
-                // the child's position, repetition state and verdict were usually prepared by a parallel warp after
-                // the previous mini-batch (prepare_child); otherwise (second expansion of a node within one
-                // mini-batch) they are computed here
-                // (slot index, verdict and board are fetched together, speculatively: one round trip)
-                const int slot = cur * kPrepSlots + (ci % kPrepSlots);
-                const int slot_ci = t.prep_ci[slot];
-                const int slot_tt = t.prep_term[slot];
-#if defined(__CUDA_ARCH__)
-                uint4 slot_b = make_uint4(0u, 0u, 0u, 0u);
-                if (ARA_LANE < 8) slot_b = reinterpret_cast<const uint4*>(&t.prep_board[slot])[ARA_LANE];
-#endif
-                const bool prepared = slot_ci == ci;
-                int tt_known = -1;
-                if (prepared) {
-#if defined(__CUDA_ARCH__)
-                    if (ARA_LANE < 8) reinterpret_cast<uint4*>(&ws.child)[ARA_LANE] = slot_b;
-                    ARA_WARP_SYNC();
-#else
-                    ws.child = t.prep_board[slot];
-#endif
-                    tt_known = slot_tt;
-                } else {
-                    copy_board(&ws.child, &t.board[cur]);
-                    if (ARA_LANE == 0) do_move(ws.child, t.move[h.edge_base + ci]);
-                }
-                if (ARA_LANE == 0) {
-                    // increment_no_visit_idx: open the next-best sibling (its edge slots are pre-initialised)
-                    if (h.no_visit_idx < h.n_moves) t.hdr[cur].no_visit_idx = static_cast<uint16_t>(h.no_visit_idx + 1);
-                    if (prepared) t.prep_ci[slot] = -1;
-                    if (n_exp < 3 * B) t.exp_parent[n_exp++] = cur;
-                }
+                int slot = 0;
+                bool prepared = false;
+                const int tt_known = leaf_board(t, ws, cur, ci, h, &slot, &prepared);
+                if (ARA_LANE == 0) commit_parent(t, cur, h, slot, prepared, n_exp, B);
                 ARA_WARP_SYNC();
                 ARA_PROF(st, 1, tq);
                 int is_term = 0;
@@ -1228,40 +1327,16 @@ ARA_HD void create_mini_batch_impl(const TreeDev& t, const SearchParams& sp, War
         }
         if (type == -2) break;
         if (type != 0) ARA_PROF(st, 0, tq);
-        if (type == 2) {
-            if (ARA_LANE == 0) {
-                st.sum_depth += static_cast<unsigned long long>(depth);
-                // terminal: free backup, sequential leaf -> root because the MCTS solver propagates bottom-up
-                backup_value(t, sp, node_value(t.hdr[leaf]), ws.traj_node + skipped, ws.traj_ci + skipped, depth - skipped, true,
-                             sp.mcts_solver != 0);
-            }
-        } else {
-            const int row = type == 1 ? B + n_coll : n_new;
-            for (int i = skipped + ARA_LANE; i < depth; i += ARA_WARP_N) {
-                t.traj_node[row * kMaxDepth + i] = ws.traj_node[i];
-                t.traj_ci[row * kMaxDepth + i] = ws.traj_ci[i];
-                t.traj_edge[row * kMaxDepth + i] = ws.traj_edge[i];
-            }
-            if (ARA_LANE == 0) {
-                st.sum_depth += static_cast<unsigned long long>(depth);
-                t.traj_len[row] = depth;
-                if (EPS) t.traj_start[row] = skipped;  // (stays 0 without the exploration)
-                if (type == 0) t.new_node[n_new] = leaf;
-            }
-        }
+        const int row = type == 1 ? B + n_coll : n_new;
+        store_trajectory(t, sp, ws, type, row, skipped, depth, leaf);
+        if (EPS && type != 2 && ARA_LANE == 0) t.traj_start[row] = skipped;  // (stays 0 without the exploration)
         ARA_WARP_SYNC();
         ARA_PROF(st, type == 2 ? 5 : 6, tq);
         if (type == 2) ++n_term;
         else if (type == 1) ++n_coll;
         else ++n_new;
     }
-    if (ARA_LANE == 0) {
-        bs.n_new = n_new;
-        bs.n_coll = n_coll;
-        bs.n_exp = n_exp;
-        st.iterations++;
-        st.evals += static_cast<unsigned>(n_new);
-    }
+    if (ARA_LANE == 0) end_mini_batch(st, *t.bs, n_new, n_coll, n_exp);
     ARA_WARP_SYNC();
 }
 
@@ -1437,21 +1512,8 @@ ARA_HD void create_root(const TreeDev& t, const SearchParams& sp, WarpScratch& w
         st.next_valid = 0;
         st.n_nodes = 0;
         st.n_edges = 0;
-        t.bs->n_new = 0;
-        t.bs->n_coll = 0;
-        t.bs->n_exp = 0;
-        t.bs->done = 0;
-        st.live_threads = sp.threads == 2 ? 2 : 1;
-        st.limit_simulations = sp.simulations;
-        st.limit_nodes = sp.nodes;
-        st.done = 0;
         st.error = 0;
-        st.iterations = 0;
-        st.evals = 0;
-        st.pre_nodes = 0;
-        st.sum_select_k = 0;
-        st.sum_depth = 0;
-        for (int i = 0; i < 8; ++i) st.prof[i] = 0;
+        begin_search(st, *t.bs, sp, 0);
     }
     ARA_WARP_SYNC();
     int is_term = 0;
@@ -1520,17 +1582,8 @@ ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* roo
             NodeHdr& h = t.hdr[cand];
             st.root = cand;
             h.parent = -1;  // make_to_root: the path walks of prepare_child stop here
-            t.bs->n_new = t.bs->n_coll = t.bs->n_exp = t.bs->done = 0;
-            st.live_threads = sp.threads == 2 ? 2 : 1;
-            st.limit_simulations = sp.simulations;
-            st.limit_nodes = sp.nodes;
-            st.done = ((h.flags & NF_TERMINAL) || h.n_moves == 0) ? 1 : 0;
-            st.iterations = 0;
-            st.evals = 0;
-            st.pre_nodes = h.visit_sum - h.free_visits;
-            st.sum_select_k = 0;
-            st.sum_depth = 0;
-            for (int i = 0; i < 8; ++i) st.prof[i] = 0;
+            begin_search(st, *t.bs, sp, h.visit_sum - h.free_visits);
+            if ((h.flags & NF_TERMINAL) || h.n_moves == 0) st.done = 1;
         }
     }
     ARA_WARP_SYNC();
@@ -1543,7 +1596,7 @@ ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* roo
 // and pack_kernel read them, and left over from the tree's last mini-batch they would apply that batch again.  Lane 0.
 ARA_HD void idle_root(const TreeDev& t) {
     t.st->done = 1;
-    t.bs->n_new = t.bs->n_coll = t.bs->n_exp = 0;
+    clear_batch(*t.bs);
 }
 
 // second half: after expand_pending + network + scatter_pending + backup_results (root trajectory is empty)

@@ -167,87 +167,19 @@ __device__ void wave_answer_abort(WaveShared& S, const TreeDev& t, const SearchP
     __threadfence_block();
 }
 
-// One step of a playout at node `nid` (header `h`, this lane's edge `pre`, both read after wave_acquire):
-// select_child_node + apply_virtual_loss_to_child, as select_and_visit without the look-ahead loads.
-struct WaveStep {
-    int ci, child;
-    uint32_t cb;
-    float old_q;
-    int counted_k;  // what the step adds to sum_select_k
-};
-__device__ __forceinline__ WaveStep wave_step(const TreeDev& t, const SearchParams& sp, int nid, const NodeHdr& h,
-                                              const EdgeRegs& pre) {
-    NodeHdr* hp = &t.hdr[nid];
-    const int k = h.no_visit_idx;
-    const uint32_t e = h.edge_base;
-    const bool single = k == 1 || h.checkmate_idx != kNoCheckmate;
-    const uint32_t vs_new = h.visit_sum + 1;
-    const float cput_new = current_cput(t, sp, vs_new);
-    const double sqrt_new = sqrt_visits(t, vs_new);
-    SelectPick pk;
-    if (single) {
-        pk.ci = k == 1 ? 0 : h.checkmate_idx;
-        pk.owner = ARA_LANE == (pk.ci & (ARA_WARP_N - 1));
-        pk.x = pre;
-        if (pk.owner && pk.ci != ARA_LANE) pk.x = load_edge(t, e + pk.ci);
-    } else {
-        bool sure = false;
-        pk = pick_fast(t, h, pre, &sure);
-        if (!sure) pk = pick_exact(t, h, pre);
-    }
-    WaveStep r;
-    r.ci = pk.ci;
-    r.counted_k = single ? 0 : k;
-    const int owner_lane = pk.ci & (ARA_WARP_N - 1);
-    r.child = __shfl_sync(0xffffffffu, pk.x.c, owner_lane);
-    r.cb = __shfl_sync(0xffffffffu, pk.x.cb, owner_lane);
-    r.old_q = __shfl_sync(0xffffffffu, pk.x.q, owner_lane);
-    if (pk.owner) {
-        const uint32_t ee = e + static_cast<uint32_t>(pk.ci);
-        if (virtual_style_of(sp, pk.x.n) == VS_VIRTUAL_LOSS)
-            t.Q[ee] = static_cast<float>((static_cast<double>(pk.x.q) * pk.x.n - 1) / static_cast<double>(pk.x.n + 1));
-        t.N[ee] = pk.x.n + 1;
-        t.vl[ee] = static_cast<uint8_t>(pk.x.vl + 1);
-    }
-    if (ARA_LANE == 0) {
-        hp->visit_sum = vs_new;
-        hp->cput = cput_new;
-        hp->sqrt_vs = sqrt_new;
-        if (!(h.flags & NF_HAS_D)) hp->flags = h.flags | NF_HAS_D | NF_SORTED;
-    }
-    return r;
-}
-
 // One mini-batch of tree `t_in` by the kWaveWarps warps of this CTA (blockDim.x == 32 * kWaveWarps).
 __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, WaveShared& S, WaveWarp& W) {
     const int w = static_cast<int>(threadIdx.x) >> 5;
     WarpScratch& ws = W.ws;
     TreeDev t = t_in;
     t.st = &S.st;
-    BatchState& bs = *t_in.bs;
     if (w == 0) {
         if (ARA_LANE == 0) {
             S.st = *t_in.st;
             for (int i = 0; i < kWaveWarps; ++i) S.state[i] = -1, S.blk[i] = -1, S.ack[i] = -1;
             S.started = -1, S.committed = -1, S.abort_at = kWaveNone, S.over = 0;
             S.n_new = 0, S.n_coll = 0, S.n_term = 0, S.n_exp = 0;
-            TreeState& st = S.st;
-            if (st.done || st.error || bs.done) {
-                bs.n_new = 0, bs.n_coll = 0, bs.n_exp = 0;
-                S.over = 2;
-            } else {
-                // run_search_thread loop condition (searchthread.cpp:326-340, :418-426), as create_mini_batch_impl
-                const NodeHdr& r = t.hdr[st.root];
-                const uint32_t node_count = r.visit_sum - r.free_visits;
-                const bool limits_ok = (st.limit_nodes == 0 || node_count < st.limit_nodes) &&
-                                       (st.limit_simulations == 0 || r.visit_sum < st.limit_simulations);
-                const bool pool_ok = st.n_nodes + 3 * sp.batch_size + 8 <= t.max_nodes;
-                if (!(limits_ok && r.node_type == NT_UNSOLVED) || r.n_moves <= 1 || !pool_ok) {
-                    bs.done = 1, bs.n_new = 0, bs.n_coll = 0, bs.n_exp = 0;
-                    if (--st.live_threads <= 0) st.done = 1;
-                    S.over = 2;
-                }
-            }
+            if (thread_loop_ends(t, sp)) S.over = 2;
         }
     }
     __syncthreads();
@@ -308,17 +240,19 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
                     rc = 2;
                     break;
                 }
-                const WaveStep step = wave_step(t, sp, cur, h, pre);
-                ci = step.ci;
-                const int next = step.child;
-                sel_k += static_cast<unsigned long long>(step.counted_k);
+                // select_and_visit without the look-ahead loads (h and pre were read after wave_acquire); the edge's old
+                // Q goes to the undo record
+                const SelectPick pk = pick_child(t, sp, h, pre, -1);
+                ci = pk.ci;
+                const int owner_lane = ci & (ARA_WARP_N - 1);
+                const int next = __shfl_sync(0xffffffffu, pk.x.c, owner_lane);
+                const uint32_t cb = __shfl_sync(0xffffffffu, pk.x.cb, owner_lane);
+                const float old_q = __shfl_sync(0xffffffffu, pk.x.q, owner_lane);
+                apply_visit(t, sp, cur, h, pk);
+                sel_k += static_cast<unsigned long long>(pk.counted_k);
                 if (ARA_LANE == 0) {
-                    ws.traj_node[depth] = cur;
-                    ws.traj_ci[depth] = static_cast<uint16_t>(ci);
-                    ws.traj_edge[depth] = h.edge_base + static_cast<uint32_t>(ci);
-                    ws.path_key[depth] = h.key;
-                    ws.path_rep[depth] = h.repetition;
-                    W.undo.q[depth] = step.old_q;
+                    record_step(ws, depth, cur, ci, h);
+                    W.undo.q[depth] = old_q;
                     W.undo.flags[depth] = h.flags;
                     if (next < 0) S.blk[w] = cur;
                 }
@@ -335,7 +269,7 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
                 __threadfence_block();
                 NodeHdr ch;
                 load_hdr(&ch, &t.hdr[next]);
-                EdgeRegs cpre = load_edge(t, step.cb + ARA_LANE);
+                EdgeRegs cpre = load_edge(t, cb + ARA_LANE);
                 if (ch.flags & NF_TERMINAL) {  // (these two flags of an existing node do not change inside this kernel)
                     type = 2, leaf = next;
                     break;
@@ -350,7 +284,7 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
                     WAVE_PROF(S, 1, tw);
                     if (rc) break;
                     load_hdr(&ch, &t.hdr[next]);
-                    cpre = load_edge(t, step.cb + ARA_LANE);
+                    cpre = load_edge(t, cb + ARA_LANE);
                 }
                 cur = next;
                 h = ch;
@@ -365,22 +299,8 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
                 if (type == 0) {
                     // the unordered half of the expansion: position, repetition state and verdict of the new leaf
                     // (the parent is blocked for younger playouts, its prepared slots are stable)
-                    slot = cur * kPrepSlots + (ci % kPrepSlots);
-                    const int slot_ci = t.prep_ci[slot];
-                    const int slot_tt = t.prep_term[slot];
-                    uint4 slot_b = make_uint4(0u, 0u, 0u, 0u);
-                    if (ARA_LANE < 8) slot_b = reinterpret_cast<const uint4*>(&t.prep_board[slot])[ARA_LANE];
-                    prepared = slot_ci == ci;
-                    if (prepared) {
-                        if (ARA_LANE < 8) reinterpret_cast<uint4*>(&ws.child)[ARA_LANE] = slot_b;
-                        __syncwarp();
-                        tt = slot_tt;
-                    } else {
-                        copy_board(&ws.child, &t.board[cur]);
-                        if (ARA_LANE == 0) do_move(ws.child, t.move[h.edge_base + ci]);
-                        __syncwarp();
-                        tt = leaf_verdict(t, ws, depth);
-                    }
+                    tt = leaf_board(t, ws, cur, ci, h, &slot, &prepared);
+                    if (tt < 0) tt = leaf_verdict(t, ws, depth);
                 }
                 WAVE_PROF(S, 3, tw);
                 // ---------------------------------------------------------- wait for the commit turn
@@ -414,11 +334,7 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
             __threadfence_block();
             // -------------------------------------------------------------- commit (playout order)
             if (type == 0) {
-                if (ARA_LANE == 0) {
-                    if (h.no_visit_idx < h.n_moves) t.hdr[cur].no_visit_idx = static_cast<uint16_t>(h.no_visit_idx + 1);
-                    if (prepared) t.prep_ci[slot] = -1;
-                    if (S.n_exp < 3 * B) t.exp_parent[S.n_exp++] = cur;
-                }
+                if (ARA_LANE == 0) commit_parent(t, cur, h, slot, prepared, S.n_exp, B);
                 __syncwarp();
                 leaf = expand_node_alloc(t, sp, ws, cur, ci, tt, h.edge_base);
                 if (leaf < 0) {
@@ -445,24 +361,9 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
                     wave_backoff();
                 }
                 __threadfence_block();
-                if (ARA_LANE == 0) {
-                    S.started = k;
-                    S.st.sum_depth += static_cast<unsigned long long>(depth);
-                    backup_value(t, sp, node_value(t.hdr[leaf]), ws.traj_node, ws.traj_ci, depth, true, sp.mcts_solver != 0);
-                }
-            } else {
-                const int row = type == 1 ? B + S.n_coll : S.n_new;
-                for (int i = ARA_LANE; i < depth; i += ARA_WARP_N) {
-                    t.traj_node[row * kMaxDepth + i] = ws.traj_node[i];
-                    t.traj_ci[row * kMaxDepth + i] = ws.traj_ci[i];
-                    t.traj_edge[row * kMaxDepth + i] = ws.traj_edge[i];
-                }
-                if (ARA_LANE == 0) {
-                    S.st.sum_depth += static_cast<unsigned long long>(depth);
-                    t.traj_len[row] = depth;
-                    if (type == 0) t.new_node[S.n_new] = leaf;
-                }
+                if (ARA_LANE == 0) S.started = k;
             }
+            store_trajectory(t, sp, ws, type, type == 1 ? B + S.n_coll : S.n_new, 0, depth, leaf);
             __syncwarp();
             if (ARA_LANE == 0) {
                 S.st.sum_select_k += sel_k;
@@ -485,13 +386,7 @@ __device__ void wave_mini_batch(const TreeDev& t_in, const SearchParams& sp, Wav
 out:
     __syncthreads();
     if (threadIdx.x == 0) {
-        if (S.over != 2) {
-            bs.n_new = S.n_new;
-            bs.n_coll = S.n_coll;
-            bs.n_exp = S.n_exp;
-            S.st.iterations++;
-            S.st.evals += static_cast<unsigned>(S.n_new);
-        }
+        if (S.over != 2) end_mini_batch(S.st, *t.bs, S.n_new, S.n_coll, S.n_exp);
         *t_in.st = S.st;
     }
 }
