@@ -28,6 +28,9 @@ ARA_HD int planes_channels(int mode, int version) {
     return version == 3 ? 80 : 63;
 }
 
+// length of the policy-map vector: 64 squares x the mode's move planes
+ARA_HD int policy_labels(int mode) { return (mode == MODE_CRAZYHOUSE ? 81 : (mode == MODE_CHESS ? 76 : 84)) * 64; }
+
 ARA_HD uint64_t bswap64_portable(uint64_t x) {  // flip_vertical (sfutil.cpp:178)
     x = ((x & 0x00FF00FF00FF00FFULL) << 8) | ((x >> 8) & 0x00FF00FF00FF00FFULL);
     x = ((x & 0x0000FFFF0000FFFFULL) << 16) | ((x >> 16) & 0x0000FFFF0000FFFFULL);

@@ -451,7 +451,7 @@ class Search {
     int iterate(int count);
     int compact_pools();
     int poll_running();
-    int read_time_stats(RootStatsHost* out);
+    int read_time_stats(RootTimeStats* out);
     cudaEvent_t prof_event();
     int prof_collect();
 
@@ -596,7 +596,7 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     if (const char* e = getenv("ARA_WAVE")) wave_ = !eps_ && atoi(e) != 0;
     if (wave_)
         ARA_CUDA_OK(cudaFuncSetAttribute(select_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kWaveSmemBytes)));
-    n_labels_ = (sp.mode == MODE_CRAZYHOUSE ? 81 : (sp.mode == MODE_CHESS ? 76 : 84)) * 64;
+    n_labels_ = policy_labels(sp.mode);
     Slot& s0 = slots_[0];
     if (net_ != nullptr) {
         if (net_->batch < n_trees * sp.batch_size)
@@ -1016,7 +1016,7 @@ int Search::go() {
         if (timed && polled_root) {
             const double now = elapsed_ms();
             if (managed && now >= next_check && now < period_end) {
-                RootStatsHost rs;
+                RootTimeStats rs;
                 if (read_time_stats(&rs)) return -1;
                 const double remaining = period_end - next_check;  // remainingMoveTimeMS after this interval
                 next_check += tc.update_interval_ms;
@@ -1036,7 +1036,7 @@ int Search::go() {
                 // the search here -- evaluated all the same, with the same arguments
                 bool more = false;
                 if (managed) {
-                    RootStatsHost rs;
+                    RootTimeStats rs;
                     if (read_time_stats(&rs)) return -1;
                     tr.value_eval = rs.value_eval;
                     const double left = move_ms - std::floor(move_ms / tc.update_interval_ms) * tc.update_interval_ms;
@@ -1081,12 +1081,11 @@ int Search::set_active(int tree, int active) {
     return 0;
 }
 
-int Search::read_time_stats(RootStatsHost* out) {
+int Search::read_time_stats(RootTimeStats* out) {
     if (launch(time_stats_kernel, 1, 32, 0, stream_, slots_[0].d_trees, d_tstats_)) return -1;
     ARA_CUDA_OK(cudaMemcpyAsync(h_tstats_, d_tstats_, sizeof(RootTimeStats), cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
-    static_assert(sizeof(RootStatsHost) == sizeof(RootTimeStats), "root statistics layout");
-    memcpy(out, h_tstats_, sizeof(*out));
+    *out = *h_tstats_;
     return 0;
 }
 
@@ -1115,8 +1114,6 @@ int Search::fetch_results() {
 
 // --------------------------------------------------------------------------------------------------------- C-ABI
 using ara::Search;
-static_assert(sizeof(ara_search_settings_t) == sizeof(ara::SearchParams), "settings layout");
-static_assert(sizeof(ara_search_result_t) == sizeof(ara::SearchResult), "result layout");
 static_assert(sizeof(ara_board_t) == sizeof(ara::Board), "board layout");
 
 extern "C" void ara_search_default_settings(ara_search_settings_t* s, int mode) {
@@ -1145,10 +1142,8 @@ extern "C" ara_search_t ara_search_create(ara_net_t net, const ara_search_settin
         ara::set_error("ara_search_create: null settings");
         return nullptr;
     }
-    ara::SearchParams sp;
-    memcpy(&sp, settings, sizeof(sp));
     std::unique_ptr<Search> s(new Search());
-    if (s->init(reinterpret_cast<ara::Net*>(net), sp, device, n_trees, max_nodes) != 0) return nullptr;
+    if (s->init(reinterpret_cast<ara::Net*>(net), *settings, device, n_trees, max_nodes) != 0) return nullptr;
     return reinterpret_cast<ara_search_t>(s.release());
 }
 extern "C" void ara_search_destroy(ara_search_t h) { delete reinterpret_cast<Search*>(h); }
@@ -1166,7 +1161,6 @@ extern "C" int ara_search_go(ara_search_t h) {
     if (s->go()) return -1;
     return s->fetch_results();
 }
-static_assert(sizeof(ara_node_view_t) == sizeof(ara::NodeView), "node view layout");
 extern "C" int ara_search_begin(ara_search_t h) {
     if (h == nullptr) return ara::set_error("ara_search_begin: null handle");
     return reinterpret_cast<Search*>(h)->begin();
@@ -1177,14 +1171,14 @@ extern "C" int ara_search_step(ara_search_t h, int n_batches) {
 }
 extern "C" int ara_search_node(ara_search_t h, int tree, int node_id, ara_node_view_t* out) {
     if (h == nullptr || out == nullptr) return ara::set_error("ara_search_node: null argument");
-    return reinterpret_cast<Search*>(h)->node_view(tree, node_id, reinterpret_cast<ara::NodeView*>(out));
+    return reinterpret_cast<Search*>(h)->node_view(tree, node_id, out);
 }
 
 extern "C" int ara_search_result(ara_search_t h, int tree, ara_search_result_t* out) {
     if (h == nullptr || out == nullptr) return ara::set_error("ara_search_result: null argument");
     Search* s = reinterpret_cast<Search*>(h);
     if (tree < 0 || tree >= s->n_trees) return ara::set_error("ara_search_result: tree %d out of range", tree);
-    memcpy(out, &s->results[tree], sizeof(*out));
+    *out = s->results[tree];
     return 0;
 }
 extern "C" int ara_search_apply_move(ara_search_t h, int tree, unsigned short move) {
@@ -1238,14 +1232,14 @@ extern "C" int ara_time_early_stopping(const ara_time_control_t* tc, double rema
                                        int max_q_is_max_visits, unsigned first_visits, unsigned second_visits, float q_first,
                                        float q_second) {
     if (tc == nullptr) return ara::set_error("ara_time_early_stopping: null argument");
-    const ara::RootStatsHost r{node_count, first_visits, second_visits, q_first, q_second, max_q_is_max_visits, 0.0f, 1};
+    const ara::RootTimeStats r{node_count, first_visits, second_visits, q_first, q_second, max_q_is_max_visits, 0.0f, 1};
     return ara::tm_early_stopping(*tc, remaining_ms, r);
 }
 extern "C" int ara_time_continue_search(const ara_time_control_t* tc, double remaining_ms, float value_eval, int* checked,
                                         float* last_value_eval) {
     if (tc == nullptr || checked == nullptr || last_value_eval == nullptr)
         return ara::set_error("ara_time_continue_search: null argument");
-    ara::RootStatsHost r{};
+    ara::RootTimeStats r{};
     r.value_eval = value_eval;
     r.valid = 1;
     return ara::tm_continue_search(*tc, remaining_ms, r, checked, last_value_eval) ? 1 : 0;

@@ -19,9 +19,11 @@
 #pragma once
 #include <math.h>
 
+#include "ara_b200.h"
 #include "chess_dev.cuh"
 #include "glibc_flt32.cuh"
 #include "planes_dev.cuh"
+#include "time_manager.h"
 
 namespace ara {
 
@@ -33,29 +35,14 @@ enum : int { VS_VIRTUAL_LOSS = 0, VS_VIRTUAL_VISIT = 1, VS_VIRTUAL_OFFSET = 2, V
 enum : int { NT_WIN = 0, NT_DRAW = 1, NT_LOSS = 2, NT_UNSOLVED = 3 };
 enum : int { NF_TERMINAL = 1, NF_HAS_NN = 2, NF_HAS_D = 4, NF_SORTED = 8, NF_INSPECTED = 16 };
 
-// Same layout as OSettings (oracle/mcts.h) and ara_search_settings_t (include/ara_b200.h).
-struct SearchParams {
-    int batch_size;
-    float dirichlet_epsilon;
-    float dirichlet_alpha;
-    float node_policy_temperature;
-    float q_value_weight;
-    float q_veto_delta;
-    float cpuct_init;
-    float cpuct_base;
-    int mcts_solver;
-    int virtual_style;
-    unsigned virtual_mix_threshold;
-    unsigned simulations;
-    unsigned nodes;
-    unsigned long long seed;
-    int mode;
-    int input_version;
-    int threads;                 // 1 or 2 logical search threads per tree (search.cu)
-    int epsilon_greedy_counter;  // 0 = off
-    int epsilon_checks_counter;  // 0 = off
-    int reserved;
-};
+// The structs that cross the C-ABI are the public header's: the kernels read and fill them as the caller sees them.
+// OSettings (oracle/mcts.h) restates the settings with the same field names for the oracle.
+using SearchParams = ara_search_settings_t;
+using SearchResult = ara_search_result_t;
+using NodeView = ara_node_view_t;
+static_assert(sizeof(SearchResult::moves) / sizeof(Move) == kMaxMoves && sizeof(NodeView::moves) / sizeof(Move) == kMaxMoves,
+              "the header's move arrays hold kMaxMoves entries");
+static_assert(sizeof(SearchResult::pv) / sizeof(Move) == kMaxDepth, "the header's principal variation holds kMaxDepth moves");
 
 struct alignas(16) NodeHdr {  // 64 B: one line per visited node on the select path
     double value_sum;
@@ -1610,17 +1597,7 @@ ARA_HD void finalize_root(const TreeDev& t, const SearchParams& sp, WarpScratch&
 }
 
 // ------------------------------------------------------------------ root statistics for the ThreadManager heuristics
-// What ThreadManager::early_stopping / continue_search (manager/threadmanager.cpp:114-178) read off the root while the
-// search runs.  Lane 0.
-struct RootTimeStats {
-    unsigned node_count;      // Node::get_node_count(): visits - free visits of the root
-    unsigned first_visits;    // first_and_second_max over the open children, each less its child's free visits
-    unsigned second_visits;
-    float q_first, q_second;  // Node::get_q_value of those two
-    int max_q_is_max_visits;  // max_q_child() == max_visits_child()
-    float value_eval;         // Node::updated_value_eval (node.cpp:784-810)
-    int valid;                // the root has at least one open child
-};
+// RootTimeStats (time_manager.h) of the tree's root.  Lane 0.
 ARA_HD void collect_time_stats(const TreeDev& t, RootTimeStats* r) {
     const TreeState& st = *t.st;
     const NodeHdr& h = t.hdr[st.root];
@@ -1663,61 +1640,7 @@ ARA_HD void collect_time_stats(const TreeDev& t, RootTimeStats* r) {
     }
 }
 
-// ------------------------------------------------------------------ results (lane 0): update_eval_info
-struct SearchResult {
-    int n_moves;
-    int no_visit_idx;
-    int best_idx;
-    int node_type;
-    int pv_len;
-    float root_value;
-    float best_move_q;
-    unsigned visit_sum;
-    unsigned free_visits;
-    unsigned iterations;
-    unsigned evals;
-    int tree_nodes;
-    int error;
-    unsigned nodes_pre_search;
-    unsigned long long sum_select_k;
-    unsigned long long sum_depth;
-    Move moves[kMaxMoves];
-    uint32_t visits[kMaxMoves];
-    float q[kMaxMoves];
-    float prior[kMaxMoves];
-    double policy[kMaxMoves];
-    Move pv[kMaxDepth];
-};
-
-// What Node's getters expose (node.h:97-124, :345-460) and Node::print_node_statistics prints (node.cpp:1248-1301) for
-// one node of the device-resident tree.  Same layout as ara_node_view_t (include/ara_b200.h).
-struct NodeView {
-    int node_id;
-    int parent;         // -1 for the root of the tree
-    int parent_child_idx;
-    int n_moves;        // Node::get_number_child_nodes
-    int no_visit_idx;   // children opened so far (Node::get_no_visit_idx); 0 until the node is a playout node
-    int node_type;      // 0 win, 1 draw, 2 loss, 3 unsolved
-    int flags;          // 1 terminal, 2 has network results, 4 playout node (NodeData exists), 8 sorted
-    int checkmate_idx;  // 65535 none
-    int end_in_ply;
-    int n_unsolved;
-    int repetition;
-    int pad_;
-    unsigned visit_sum;    // Node::get_visits
-    unsigned real_visits;  // Node::get_real_visits
-    unsigned free_visits;
-    float value;           // Node::get_value = valueSum / realVisits
-    double value_sum;
-    unsigned long long key;  // Node::hash_key
-    Move moves[kMaxMoves];       // Node::get_action(i)
-    int32_t child[kMaxMoves];    // node id of child i, -1 = not expanded (Node::get_child_node)
-    uint32_t visits[kMaxMoves];  // childNumberVisits
-    float q[kMaxMoves];          // qValues
-    float prior[kMaxMoves];      // policyProbSmall
-    uint8_t vl[kMaxMoves];       // virtualLossCounter
-    uint8_t child_type[kMaxMoves];
-};
+// ------------------------------------------------------------------ results: the view of one node, update_eval_info
 ARA_HD void collect_node_view(const TreeDev& t, int nid, NodeView* v) {  // lane-strided; nid < 0 = the current root
     const TreeState& st = *t.st;
     const int id = nid < 0 ? st.root : nid;

@@ -8,12 +8,16 @@
 
 namespace ara {
 
-struct RootStatsHost {  // mirror of RootTimeStats (search_dev.cuh)
-    unsigned node_count, first_visits, second_visits;
-    float q_first, q_second;
-    int max_q_is_max_visits;
-    float value_eval;
-    int valid;
+// What ThreadManager::early_stopping / continue_search (manager/threadmanager.cpp:114-178) read off the root while the
+// search runs; collect_time_stats (search_dev.cuh) fills it on the device.
+struct RootTimeStats {
+    unsigned node_count;      // Node::get_node_count(): visits - free visits of the root
+    unsigned first_visits;    // first_and_second_max over the open children, each less its child's free visits
+    unsigned second_visits;
+    float q_first, q_second;  // Node::get_q_value of those two
+    int max_q_is_max_visits;  // max_q_child() == max_visits_child()
+    float value_eval;         // Node::updated_value_eval (node.cpp:784-810)
+    int valid;                // the root has at least one open child
 };
 
 // TimeManager::get_time_for_move (manager/timemanager.cpp:51-98) for a search without node / depth limits, with the
@@ -38,7 +42,7 @@ inline int tm_time_for_move(long movetime, int time_me, int inc_me, int movestog
 }
 
 // ThreadManager::early_stopping: 1 "max nodes" rule, 2 "second move cannot catch up" rule, 0 keep searching
-inline int tm_early_stopping(const ara_time_control_t& tc, double remaining_ms, const RootStatsHost& r) {
+inline int tm_early_stopping(const ara_time_control_t& tc, double remaining_ms, const RootTimeStats& r) {
     if (!tc.in_game || tc.overall_nps == 0.0 || !r.valid) return 0;
     if (r.node_count > tc.overall_nps * (tc.movetime_ms / 1000.0f) * 2 && r.max_q_is_max_visits) return 1;
     // (the reference divides the NPS by 1000 in float before multiplying by the remaining milliseconds)
@@ -50,7 +54,7 @@ inline int tm_early_stopping(const ara_time_control_t& tc, double remaining_ms, 
 
 // ThreadManager::continue_search: prolong by another move time if the evaluation dropped since the last move.
 // `checked` is checkedContinueSearch, `last_eval` tData->lastValueEval; both are updated like the reference does.
-inline bool tm_continue_search(const ara_time_control_t& tc, double remaining_ms, const RootStatsHost& r, int* checked,
+inline bool tm_continue_search(const ara_time_control_t& tc, double remaining_ms, const RootTimeStats& r, int* checked,
                                float* last_eval) {
     if (!tc.in_game || !tc.can_prolong || tc.overall_nps == 0.0 || *checked > 1) return false;
     if (tc.movetime_ms * 2 > tc.safe_remaining_ms) return false;  // make sure not to flag when continuing

@@ -250,12 +250,19 @@ class BoardState:
         return encode_planes([self.board()], mode, version, normalize)[0]
 
 
+def planes_channels(mode, version):
+    """Input channels of the network for a (mode, input version) pair, as planes_channels of csrc/planes_dev.cuh."""
+    c = {(0, 1): 34, (0, 2): 51, (0, 3): 64, (1, 1): 39, (1, 3): 52, (2, 1): 63, (2, 2): 63, (2, 3): 80}.get((mode, version))
+    if c is None:
+        raise AraError(f"no input representation for mode {mode}, version {version}")
+    return c
+
+
 def encode_planes(boards, mode, version, normalize=True):
     m = MODES[mode] if isinstance(mode, str) else mode
     n = len(boards)
     arr = (AraBoard * n)(*boards)
-    c = {(0, 1): 34, (0, 2): 51, (0, 3): 64, (1, 1): 39, (1, 3): 52, (2, 1): 63, (2, 2): 63, (2, 3): 80}[(m, version)]
-    out = np.full((n, c, 8, 8), np.nan, np.float32)
+    out = np.full((n, planes_channels(m, version), 8, 8), np.nan, np.float32)
     check(_L().ara_encode_planes(arr, n, m, version, int(bool(normalize)), out.ctypes.data))
     return out
 
@@ -273,15 +280,16 @@ def legal_moves_gpu(boards):
             [pidx[i, :counts[i]].tolist() for i in range(n)])
 
 
-def _result_to_dict(r, is960):
+def result_to_dict(r, uci_fn):
+    """EvalInfo dict of a SearchResult; uci_fn spells a 16-bit move code."""
     k = r.n_moves
-    d = dict(moves=[move_to_uci(m, is960) for m in r.moves[:k]], visits=np.array(r.visits[:k], np.uint32),
+    d = dict(moves=[uci_fn(m) for m in r.moves[:k]], visits=np.array(r.visits[:k], np.uint32),
              q=np.array(r.q[:k], np.float32), prior=np.array(r.prior[:k], np.float32),
              policy=np.array(r.policy[:k], np.float64), root_value=r.root_value, visit_sum=r.visit_sum,
              free_visits=r.free_visits, nodes=r.visit_sum - r.free_visits, best_idx=r.best_idx,
              best_move_q=r.best_move_q, node_type=r.node_type, pv_len=r.pv_len, iterations=r.iterations, evals=r.evals,
              tree_nodes=r.tree_nodes, sum_select_k=r.sum_select_k, sum_depth=r.sum_depth, nodes_pre_search=r.nodes_pre_search, error=r.error,
-             pv=[move_to_uci(m, is960) for m in r.pv[:r.pv_len]])
+             pv=[uci_fn(m) for m in r.pv[:r.pv_len]])
     if k > 0 and r.best_idx >= 0:
         d["best_move"] = d["moves"][r.best_idx]
     return d
@@ -347,7 +355,8 @@ class MCTSAgent:
         r = SearchResult()
         check(_L().ara_search_result(self._h, tree, ctypes.byref(r)))
         st = self._states[tree]
-        d = _result_to_dict(r, st.is960 if st is not None else False)
+        is960 = st.is960 if st is not None else False
+        d = result_to_dict(r, lambda m: move_to_uci(m, is960))
         ms = _L().ara_search_last_go_ms(self._h)
         d["elapsed_ms"] = ms
         # EvalInfo::calculate_nps (evalinfo.cpp:73-85): (nodes - nodesPreSearch) / elapsed

@@ -216,9 +216,9 @@ typedef struct ara_node_view_s {
     int parent;           /* node id of the parent, -1 for the root of the tree */
     int parent_child_idx;
     int n_moves;          /* Node::get_number_child_nodes */
-    int no_visit_idx;     /* Node::get_no_visit_idx: children opened so far */
+    int no_visit_idx;     /* Node::get_no_visit_idx: children opened so far; 0 until the node is a playout node */
     int node_type;        /* 0 win, 1 draw, 2 loss, 3 unsolved (nodedata.h NodeType) */
-    int flags;            /* 1 terminal, 2 has NN results, 4 playout node, 8 sorted */
+    int flags;            /* 1 terminal, 2 has NN results, 4 playout node (NodeData exists), 8 sorted */
     int checkmate_idx;    /* 65535 = none */
     int end_in_ply;
     int n_unsolved;
@@ -227,7 +227,7 @@ typedef struct ara_node_view_s {
     unsigned visit_sum;   /* Node::get_visits */
     unsigned real_visits; /* Node::get_real_visits */
     unsigned free_visits;
-    float value;          /* Node::get_value */
+    float value;          /* Node::get_value = valueSum / realVisits */
     double value_sum;
     unsigned long long key;      /* Node::hash_key */
     unsigned short moves[512];   /* Node::get_action(i), 16-bit move codes, sorted by prior once the node is visited */

@@ -3,6 +3,8 @@ import ctypes
 import os
 import subprocess
 
+from crazyara_b200.engine import SearchResult, result_to_dict
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(os.path.dirname(_HERE))
 _LIB = None
@@ -107,31 +109,6 @@ class HeState:
         return ctypes.string_at(self.L.he_board(self.h), 128)
 
 
-class SearchResult(ctypes.Structure):
-    _fields_ = [("n_moves", ctypes.c_int), ("no_visit_idx", ctypes.c_int), ("best_idx", ctypes.c_int),
-                ("node_type", ctypes.c_int), ("pv_len", ctypes.c_int), ("root_value", ctypes.c_float),
-                ("best_move_q", ctypes.c_float), ("visit_sum", ctypes.c_uint), ("free_visits", ctypes.c_uint),
-                ("iterations", ctypes.c_uint), ("evals", ctypes.c_uint), ("tree_nodes", ctypes.c_int),
-                ("error", ctypes.c_int), ("nodes_pre_search", ctypes.c_uint), ("sum_select_k", ctypes.c_ulonglong), ("sum_depth", ctypes.c_ulonglong),
-                ("moves", ctypes.c_uint16 * 512), ("visits", ctypes.c_uint32 * 512), ("q", ctypes.c_float * 512),
-                ("prior", ctypes.c_float * 512), ("policy", ctypes.c_double * 512), ("pv", ctypes.c_uint16 * 256)]
-
-
-def result_to_dict(r, uci_fn):
-    import numpy as np
-    k = r.n_moves
-    d = dict(moves=[uci_fn(m) for m in r.moves[:k]], visits=np.array(r.visits[:k], np.uint32),
-             q=np.array(r.q[:k], np.float32), prior=np.array(r.prior[:k], np.float32),
-             policy=np.array(r.policy[:k], np.float64), root_value=r.root_value, visit_sum=r.visit_sum,
-             free_visits=r.free_visits, nodes=r.visit_sum - r.free_visits, best_idx=r.best_idx,
-             best_move_q=r.best_move_q, node_type=r.node_type, pv_len=r.pv_len, iterations=r.iterations,
-             evals=r.evals, tree_nodes=r.tree_nodes, sum_select_k=r.sum_select_k, sum_depth=r.sum_depth, nodes_pre_search=r.nodes_pre_search,
-             error=r.error, pv=[uci_fn(m) for m in r.pv[:r.pv_len]])
-    if k > 0 and r.best_idx >= 0:
-        d["best_move"] = d["moves"][r.best_idx]
-    return d
-
-
 class HeSearch:
     """Host emulation of the GPU search, driven like oracle.search.Search."""
 
@@ -159,6 +136,8 @@ class HeSearch:
         L.he_search_result.restype = ctypes.POINTER(SearchResult)
         L.he_search_result.argtypes = [ctypes.c_void_p]
         L.he_fake_eval.argtypes = [ctypes.c_ulonglong, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        L.he_search_apply_move.argtypes = [ctypes.c_void_p, ctypes.c_uint16]
+        L.he_search_time_stats.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
         assert L.he_sizeof_result() == ctypes.sizeof(SearchResult)
         self.settings = settings
         self.h = L.he_search_new(ctypes.byref(settings), max_nodes, max_edges)
@@ -184,13 +163,11 @@ class HeSearch:
 
     def apply_move(self, move):
         """MCTSAgent::apply_move_to_tree (16-bit move code of the device rules)."""
-        self.L.he_search_apply_move.argtypes = [ctypes.c_void_p, ctypes.c_uint16]
         self.L.he_search_apply_move(self.h, int(move))
 
     def time_stats(self):
         """collect_time_stats of the current tree (what the ThreadManager rules read)."""
         i, f = (ctypes.c_uint * 5)(), (ctypes.c_float * 3)()
-        self.L.he_search_time_stats.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
         self.L.he_search_time_stats(self.h, i, f)
         return dict(node_count=i[0], first_visits=i[1], second_visits=i[2], max_q_is_max_visits=int(i[3]), valid=int(i[4]),
                     q_first=f[0], q_second=f[1], value_eval=f[2])

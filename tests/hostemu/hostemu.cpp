@@ -132,7 +132,7 @@ HeSearch* he_search_new(const SearchParams* sp, int max_nodes, int max_edges) {
     s->vl.resize(max_edges);
     s->etype.resize(max_edges);
     s->channels = planes_channels(sp->mode, sp->input_version);
-    s->n_labels = (sp->mode == MODE_CRAZYHOUSE ? 81 : (sp->mode == MODE_CHESS ? 76 : 84)) * 64;
+    s->n_labels = policy_labels(sp->mode);
     const int lut_len = 1 << 16;
     s->lut.resize(lut_len);
     for (int i = 0; i < lut_len; ++i) s->lut[i] = logf((static_cast<float>(i) + sp->cpuct_base + 1) / sp->cpuct_base) + sp->cpuct_init;

@@ -79,3 +79,41 @@ def test_header_is_plain_c(tmp_path):
     src.write_text('#include "ara_b200.h"\nint main(void) { ara_time_control_t t; ara_search_result_t r; (void)t; (void)r; return 0; }\n')
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-pedantic", "-I", os.path.join(root, "include"), "-c",
                     str(src), "-o", str(tmp_path / "h.o")], check=True)
+
+
+def _header_struct_fields(typedef):
+    """Field names of `typedef struct ... { ... } <typedef>;` in include/ara_b200.h, in declaration order."""
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "ara_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef\s+struct\s*\w*\s*\{([^{}]*)\}\s*" + typedef + r"\s*;", src).group(1)
+    return [re.search(r"(\w+)\s*(\[\d+\])?$", decl.strip()).group(1) for decl in body.split(";") if decl.strip()]
+
+
+def test_ctypes_structs_have_the_header_layout(tmp_path):
+    """engine.py restates the header's structs for ctypes; the device code uses the header's own.  Every field of the
+    mirror must sit at the offset and have the size the C compiler gives the field of the same name."""
+    import subprocess
+    from crazyara_b200 import engine
+    mirrors = {"ara_search_settings_t": engine.SearchSettings, "ara_search_result_t": engine.SearchResult,
+               "ara_node_view_t": engine.NodeView, "ara_time_control_t": engine.TimeControl,
+               "ara_time_report_t": engine.TimeReport}
+    fields = {t: _header_struct_fields(t) for t in mirrors}
+    lines = ['#include <stddef.h>', '#include <stdio.h>', '#include "ara_b200.h"', 'int main(void) {']
+    for t, names in fields.items():
+        lines.append(f'    printf("{t} . 0 %zu\\n", sizeof({t}));')
+        lines += [f'    printf("{t} {n} %zu %zu\\n", offsetof({t}, {n}), sizeof((({t}*)0)->{n}));' for n in names]
+    lines += ['    return 0;', '}', '']
+    (tmp_path / "layout.c").write_text("\n".join(lines))
+    exe = str(tmp_path / "layout")
+    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(tmp_path / "layout.c"),
+                    "-o", exe], check=True)
+    in_c = {}
+    for line in subprocess.run([exe], check=True, capture_output=True, text=True).stdout.splitlines():
+        t, n, offset, size = line.split()
+        in_c[t, n] = (int(offset), int(size))
+    for t, cls in mirrors.items():
+        assert [n for n, _ in cls._fields_] == fields[t], t
+        assert len(fields[t]) >= 5
+        assert ctypes.sizeof(cls) == in_c[t, "."][1], t
+        for n in fields[t]:
+            f = getattr(cls, n)
+            assert (f.offset, f.size) == in_c[t, n], f"{t}.{n}"

@@ -11,7 +11,8 @@ import pytest
 
 from oracle import search as osr
 from oracle.chess import Position
-from tests.hostemu import HeSearch, HeState, result_to_dict
+from crazyara_b200.engine import result_to_dict
+from tests.hostemu import HeSearch, HeState
 from tests.test_search_hostemu import assert_same_search
 from tests.test_tree_reuse_hostemu import CASES
 

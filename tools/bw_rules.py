@@ -39,9 +39,9 @@ def positions(variant, n, seed=42):
 def main():
     import torch
     from crazyara_b200 import lib
-    from crazyara_b200.engine import AraBoard, legal_moves_gpu
+    from crazyara_b200.engine import AraBoard, legal_moves_gpu, planes_channels
     variant, mode, version = (int(x) for x in (sys.argv[1:4] if len(sys.argv) >= 4 else (1, 0, 1)))
-    channels = {(0, 1): 34, (0, 2): 51, (0, 3): 64, (1, 1): 39, (1, 3): 52, (2, 1): 63, (2, 3): 80}[(mode, version)]
+    channels = planes_channels(mode, version)
     t0 = time.time()
     boards = positions(variant, N)
     arr = (AraBoard * N)(*boards)
