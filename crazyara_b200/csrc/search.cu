@@ -57,11 +57,13 @@ struct NullWriterFactory {  // fake backend: no planes needed
     ARA_HD Target make(int) const { return Target{}; }
 };
 
-// What the next go asks of one tree: its limits (ara_search_set_limits, else the settings') and whether it takes part
+// What the next go asks of one tree: its limits (ara_search_set_limits, else the settings'), its Q-value weight and
+// Dirichlet epsilon (ara_search_set_tree_settings, negative = the settings') and whether it takes part
 // (ara_search_set_active).  Uploaded before every root phase.
 struct TreeLimits {
     unsigned simulations, nodes;
     int active;
+    float q_value_weight, dirichlet_epsilon;
 };
 
 __global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const TreeLimits* limits) {
@@ -78,6 +80,7 @@ __global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchPa
     if (threadIdx.x == 0) {
         t.st->limit_simulations = lim.simulations;
         t.st->limit_nodes = lim.nodes;
+        apply_tree_settings(*t.st, lim.q_value_weight, lim.dirichlet_epsilon);
     }
 }
 
@@ -346,6 +349,7 @@ class Search {
     int init(Net* net, const SearchParams& sp, int device, int n_trees, int max_nodes);
     int set_position(int tree, const Board& root, const uint64_t* hist_keys, const int16_t* hist_reps, int hist_len);
     int set_limits(int tree, unsigned simulations, unsigned nodes);
+    int set_tree_settings(int tree, float q_value_weight, float dirichlet_epsilon);
     int set_active(int tree, int active);
     int go();
     int begin();
@@ -664,7 +668,7 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     if (mem_.dalloc(&s0.d_trees, n_trees) || mem_.dalloc(&d_roots_, n_trees) || mem_.dalloc(&d_results_, n_trees) || mem_.dalloc(&d_limits_, n_trees) ||
         mem_.dalloc(&d_tstats_, 1) || mem_.dalloc(&s0.d_count, 1) || mem_.dalloc(&d_node_view_, 1))
         return -1;
-    h_limits_.assign(n_trees, TreeLimits{sp.simulations, sp.nodes, 1});
+    h_limits_.assign(n_trees, TreeLimits{sp.simulations, sp.nodes, 1, -1.0f, -1.0f});
     for (int i = 0; i < n_trees; ++i) {  // the trees' Dirichlet generators (TreeState::rng)
         const uint32_t x = minstd_seed(sp.seed, i);
         ARA_CUDA_OK(cudaMemcpy(&d_states_[i]->rng, &x, sizeof(x), cudaMemcpyHostToDevice));
@@ -1074,6 +1078,18 @@ int Search::set_limits(int tree, unsigned simulations, unsigned nodes) {
     return 0;
 }
 
+int Search::set_tree_settings(int tree, float q_value_weight, float dirichlet_epsilon) {
+    if (tree < -1 || tree >= n_trees) return set_error("ara_search_set_tree_settings: tree %d out of range", tree);
+    // the reference's option ranges: Centi_Q_Value_Weight 0..99999; an epsilon above 1 would make priors negative
+    if (!std::isfinite(q_value_weight) || q_value_weight > 999.99f)
+        return set_error("ara_search_set_tree_settings: Q-value weight %g out of range", q_value_weight);
+    if (!std::isfinite(dirichlet_epsilon) || dirichlet_epsilon > 1.0f)
+        return set_error("ara_search_set_tree_settings: Dirichlet epsilon %g out of range", dirichlet_epsilon);
+    for (int i = 0; i < n_trees; ++i)
+        if (tree < 0 || tree == i) h_limits_[i].q_value_weight = q_value_weight, h_limits_[i].dirichlet_epsilon = dirichlet_epsilon;
+    return 0;
+}
+
 int Search::set_active(int tree, int active) {
     if (tree < -1 || tree >= n_trees) return set_error("ara_search_set_active: tree %d out of range", tree);
     for (int i = 0; i < n_trees; ++i)
@@ -1188,6 +1204,10 @@ extern "C" int ara_search_apply_move(ara_search_t h, int tree, unsigned short mo
 extern "C" int ara_search_set_limits(ara_search_t h, int tree, unsigned simulations, unsigned nodes) {
     if (h == nullptr) return ara::set_error("ara_search_set_limits: null handle");
     return reinterpret_cast<Search*>(h)->set_limits(tree, simulations, nodes);
+}
+extern "C" int ara_search_set_tree_settings(ara_search_t h, int tree, float q_value_weight, float dirichlet_epsilon) {
+    if (h == nullptr) return ara::set_error("ara_search_set_tree_settings: null handle");
+    return reinterpret_cast<Search*>(h)->set_tree_settings(tree, q_value_weight, dirichlet_epsilon);
 }
 extern "C" int ara_search_set_active(ara_search_t h, int tree, int active) {
     if (h == nullptr) return ara::set_error("ara_search_set_active: null handle");

@@ -88,7 +88,10 @@ struct TreeState {
     // them per tree (self-play jitters the node budget of every search, rl/selfplay.cpp:146-152)
     uint32_t limit_simulations;
     uint32_t limit_nodes;
-    int pad1_;
+    // the settings' Q-value weight (posterior) and Dirichlet epsilon (root noise) of the current go, unless
+    // ara_search_set_tree_settings overrides them per tree (self-play's quick searches, rl/selfplay.cpp:214-241)
+    float q_value_weight;
+    float dirichlet_epsilon;
     int root;        // node id of the current root (0 for a new tree, the re-rooted child when the tree is reused)
     int next_root;   // candidate root after ara_search_apply_move (MCTSAgent::ownNextRoot / opponentsNextRoot), -1 none
     int next_valid;  // apply_move has been called since the last search: only next_root may be reused
@@ -98,7 +101,6 @@ struct TreeState {
     unsigned iterations;
     unsigned evals;
     unsigned pre_nodes;  // EvalInfo::nodesPreSearch: node count of the root when the search began (0 for a new tree)
-    unsigned pad_;
     unsigned long long sum_select_k;
     unsigned long long sum_depth;
     // SM-clock cycles spent per phase of create_mini_batch (lane 0): 0 descent, 1 board copy + do_move, 2 repetition +
@@ -974,9 +976,10 @@ ARA_HD void apply_dirichlet_to_root(const TreeDev& t, const SearchParams& sp, Wa
         ws.sort_p[i] = gamma_f(g, sp.dirichlet_alpha);
         sum += ws.sort_p[i];
     }
+    const float eps = t.st->dirichlet_epsilon;
     for (int i = 0; i < n; ++i) {
         const float noise = ws.sort_p[i] / sum;
-        t.P[h.edge_base + i] = (1 - sp.dirichlet_epsilon) * t.P[h.edge_base + i] + sp.dirichlet_epsilon * noise;
+        t.P[h.edge_base + i] = (1 - eps) * t.P[h.edge_base + i] + eps * noise;
     }
     t.st->rng = g.x;
     h.no_visit_idx = static_cast<uint16_t>(n);  // fully_expand_node (edges are pre-initialised)
@@ -1110,14 +1113,16 @@ ARA_HD void eps_prologue(const TreeDev& t, const SearchParams& sp, WarpScratch& 
 // kernels: create_mini_batch_impl below (one warp per tree) and wave_mini_batch (search_wave.cuh, a wavefront of warps)
 ARA_HD void clear_batch(BatchState& bs) { bs.n_new = bs.n_coll = bs.n_exp = 0; }
 
-// A search begins on the tree's root: the settings' SearchLimits (root_kernel applies the tree's own), every logical
-// thread live, the counters at zero.  pre_nodes: EvalInfo::nodesPreSearch.  Lane 0.
+// A search begins on the tree's root: the settings' SearchLimits, Q-value weight and Dirichlet epsilon (root_kernel
+// applies the tree's own), every logical thread live, the counters at zero.  pre_nodes: EvalInfo::nodesPreSearch.  Lane 0.
 ARA_HD void begin_search(TreeState& st, BatchState& bs, const SearchParams& sp, unsigned pre_nodes) {
     clear_batch(bs);
     bs.done = 0;
     st.live_threads = sp.threads == 2 ? 2 : 1;
     st.limit_simulations = sp.simulations;
     st.limit_nodes = sp.nodes;
+    st.q_value_weight = sp.q_value_weight;
+    st.dirichlet_epsilon = sp.dirichlet_epsilon;
     st.done = 0;
     st.iterations = 0;
     st.evals = 0;
@@ -1125,6 +1130,13 @@ ARA_HD void begin_search(TreeState& st, BatchState& bs, const SearchParams& sp, 
     st.sum_select_k = 0;
     st.sum_depth = 0;
     for (int i = 0; i < 8; ++i) st.prof[i] = 0;
+}
+
+// The tree's own Q-value weight and Dirichlet epsilon (ara_search_set_tree_settings) over the settings' values that
+// begin_search put in place; a negative value keeps the settings' value.  After reuse_root / create_root.  Lane 0.
+ARA_HD void apply_tree_settings(TreeState& st, float q_value_weight, float dirichlet_epsilon) {
+    if (q_value_weight >= 0) st.q_value_weight = q_value_weight;
+    if (dirichlet_epsilon >= 0) st.dirichlet_epsilon = dirichlet_epsilon;
 }
 
 // run_search_thread loop condition (searchthread.cpp:326-340, :418-426), checked before every mini-batch.  True: this
@@ -1591,7 +1603,7 @@ ARA_HD void finalize_root(const TreeDev& t, const SearchParams& sp, WarpScratch&
     if (ARA_LANE == 0 && !t.st->done && !t.st->error) {
         NodeHdr& h = t.hdr[t.st->root];
         h.flags |= NF_HAS_D | NF_SORTED;  // prepare_node_for_visits
-        if (sp.dirichlet_epsilon > 0.009f && h.n_moves > 1) apply_dirichlet_to_root(t, sp, ws);
+        if (t.st->dirichlet_epsilon > 0.009f && h.n_moves > 1) apply_dirichlet_to_root(t, sp, ws);
     }
     ARA_WARP_SYNC();
 }
@@ -1707,7 +1719,8 @@ ARA_HD int mcts_policy(const TreeDev& t, const SearchParams& sp, const NodeHdr& 
                 const int c = t.child[e + i];
                 if (c >= 0 && (t.hdr[c].flags & NF_HAS_D) && t.hdr[c].node_type == NT_WIN) out[i] = 0;
             }
-        if (sp.q_value_weight > 0) {
+        const float q_value_weight = t.st->q_value_weight;
+        if (q_value_weight > 0) {
             int best_q = 0;
             for (int i = 1; i < k; ++i)
                 if (t.Q[e + i] > t.Q[e + best_q]) best_q = i;
@@ -1733,7 +1746,7 @@ ARA_HD int mcts_policy(const TreeDev& t, const SearchParams& sp, const NodeHdr& 
                 }
             } else if (best != second_arg && t.Q[e + second_arg] > t.Q[e + best]) {
                 const float q_diff = t.Q[e + second_arg] - t.Q[e + best];
-                out[second_arg] += q_diff * sp.q_value_weight * out[best];
+                out[second_arg] += q_diff * q_value_weight * out[best];
             }
         }
     }

@@ -3,6 +3,7 @@
   BoardState  <-> engine/src/environments/chess_related/boardstate.h  (State interface, engine/src/state.h:287-509)
   SearchSettings / default_settings <-> agents/config/searchsettings.h + uci/optionsuci.cpp defaults
   MCTSAgent   <-> agents/mctsagent.{h,cpp}: evaluate_board_state() runs the device-resident search
+  RawNetAgent <-> agents/rawnetagent.{h,cpp}: the network's policy alone, no search
   EvalInfo (dict) <-> evalinfo.{h,cpp}
 
 Same names and argument meaning as the reference so that tests read like the reference's own.  No CPU fallback.
@@ -126,6 +127,7 @@ def _L():
         L.ara_time_continue_search.argtypes = [vp, ctypes.c_double, ctypes.c_float, vp, vp]
         L.ara_search_set_movetime.argtypes = [vp, ctypes.c_double]
         L.ara_search_set_limits.argtypes = [vp, ci, ctypes.c_uint, ctypes.c_uint]
+        L.ara_search_set_tree_settings.argtypes = [vp, ci, ctypes.c_float, ctypes.c_float]
         L.ara_search_set_active.argtypes = [vp, ci, ci]
         L.ara_search_profile.argtypes = [vp] + [vp] * 4
         L.ara_search_last_go_ms.restype = ctypes.c_double
@@ -280,6 +282,62 @@ def legal_moves_gpu(boards):
             [pidx[i, :counts[i]].tolist() for i in range(n)])
 
 
+def value_to_centipawn(value, mode):
+    """value_to_centipawn (evalinfo.cpp:102-110) with VALUE_TO_CENTI_PARAM 1.4 (MODE_CHESS) or 1.2 (constants.h:90-92)"""
+    value = np.float32(value)
+    if abs(value) >= 1:
+        return int(np.sign(value)) * 9999
+    param = np.float32(1.4 if (MODES[mode] if isinstance(mode, str) else mode) == 1 else 1.2)
+    return int(-(np.sign(value) * np.log(np.float32(1) - abs(value)) / np.log(param)) * np.float32(100))
+
+
+class RawNetAgent:
+    """RawNetAgent of the reference (agents/rawnetagent.cpp:45-83): the move the network's policy prefers, without a
+    search.  `net` is a crazyara_b200.nn.NeuralNetAPI; `mode` / `input_version` are the input representation the
+    searches of the same network use (SearchSettings.mode / input_version)."""
+
+    def __init__(self, net, mode, input_version):
+        if net is None:
+            raise AraError("RawNetAgent needs a network")
+        self.net, self.mode, self.input_version = net, mode, input_version
+
+    def predict(self, states):
+        """For every state: its legal moves (16-bit codes), their priors (entries of the soft-maxed policy) and the value.
+        One forward per network batch over all the states (ara_net_predict_priors)."""
+        boards = [s.board() for s in states]
+        moves, _, pidx = legal_moves_gpu(boards)
+        planes = encode_planes(boards, self.mode, self.input_version)
+        out = []
+        B = self.net.get_batch_size()
+        for lo in range(0, len(states), B):
+            hi = min(lo + B, len(states))
+            counts = np.array([len(m) for m in moves[lo:hi]], np.int32)
+            idx = np.zeros((hi - lo, max(1, int(counts.max()))), np.int32)
+            for i, p in enumerate(pidx[lo:hi]):
+                idx[i, :len(p)] = p
+            value = np.zeros(hi - lo, np.float32)
+            priors = np.zeros(idx.shape, np.float32)
+            self.net.predict_priors(np.ascontiguousarray(planes[lo:hi]), idx, counts, value, priors, n=hi - lo)
+            out += [(moves[i], priors[i - lo, :counts[i - lo]].copy(), float(value[i - lo])) for i in range(lo, hi)]
+        return out
+
+    def evaluate_board_state(self, state):
+        """EvalInfo dict of RawNetAgent::evaluate_board_state: a single legal move is returned without a forward, else the
+        argmax of the legal moves' priors with the score of the network's value (depth, seldepth and nodes 1)."""
+        legal = state.legal_actions()
+        if not legal:
+            raise AraError(f"no legal move in {state.fen()}")
+        if len(legal) == 1:
+            m = state.action_to_uci(legal[0])
+            return dict(moves=[m], policy=np.ones(1), best_idx=0, best_move=m, pv=[m], centipawns=value_to_centipawn(0.0, self.mode),
+                        depth=0, seldepth=0, nodes=0)
+        (codes, priors, value), = self.predict([state])
+        best = int(np.argmax(priors))
+        moves = [state.action_to_uci(a) for a in codes]
+        return dict(moves=moves, policy=priors, best_idx=best, best_move=moves[best], pv=[moves[best]], value=value,
+                    centipawns=value_to_centipawn(value, self.mode), depth=1, seldepth=1, nodes=1)
+
+
 def result_to_dict(r, uci_fn):
     """EvalInfo dict of a SearchResult; uci_fn spells a 16-bit move code."""
     k = r.n_moves
@@ -394,6 +452,11 @@ class MCTSAgent:
     def set_search_limits(self, simulations, nodes, tree=-1):
         """SearchLimits::simulations / nodes of the following searches of `tree` (-1 = all trees) instead of the settings'."""
         check(_L().ara_search_set_limits(self._h, int(tree), int(simulations), int(nodes)))
+
+    def set_tree_settings(self, q_value_weight=-1.0, dirichlet_epsilon=-1.0, tree=-1):
+        """Q-value weight and Dirichlet epsilon of the following searches of `tree` (-1 = all trees) instead of the
+        settings'; a negative value restores the settings' value (ara_search_set_tree_settings)."""
+        check(_L().ara_search_set_tree_settings(self._h, int(tree), float(q_value_weight), float(dirichlet_epsilon)))
 
     def set_active(self, tree, active=True):
         """Leave `tree` (-1 = all trees) out of the following searches, or take it back in (ara_search_set_active).  An

@@ -4,6 +4,7 @@
 //   SearchSettings / SearchLimits   engine/src/agents/config/searchsettings.h, searchlimits.h
 //   EvalInfo       engine/src/evalinfo.h
 //   MCTSAgent      engine/src/agents/mctsagent.h: evaluate_board_state() -> device-resident search
+//   RawNetAgent    engine/src/agents/rawnetagent.h: evaluate_board_state() -> the network's policy alone
 //   SearchThread   engine/src/searchthread.h: thread_iteration() = one mini-batch of the device search (ara_search_step)
 //   Node           engine/src/node.h: read-only view of a node of the device-resident tree (ara_search_node)
 // Errors are rethrown as std::runtime_error / std::invalid_argument like the reference's backends do.
@@ -144,7 +145,7 @@ struct EvalInfo {  // engine/src/evalinfo.h
     float bestMoveQ = 0.0f;
     float rootValue = 0.0f;
     int centipawns = 0;
-    size_t nodes = 0, nodesPreSearch = 0, depth = 0;
+    size_t nodes = 0, nodesPreSearch = 0, depth = 0, selDepth = 0;
     double elapsedMs = 0.0;
     size_t calculate_nps() const {  // evalinfo.cpp:73-85
         const double ms = elapsedMs <= 0 ? 1.0 : elapsedMs;
@@ -321,13 +322,74 @@ class MCTSAgent {
     void set_movetime(double ms) {
         if (ara_search_set_movetime(search_, ms) != 0) throw std::runtime_error(ara_last_error());
     }
+    // MCTSAgent::update_q_value_weight / update_dirichlet_epsilon: the following searches use this value instead of the
+    // settings' (a negative value restores the settings' value)
+    void update_q_value_weight(float value) {
+        qValueWeight_ = value;
+        set_tree_settings();
+    }
+    void update_dirichlet_epsilon(float value) {
+        dirichletEpsilon_ = value;
+        set_tree_settings();
+    }
 
    private:
+    void set_tree_settings() {
+        if (ara_search_set_tree_settings(search_, -1, qValueWeight_, dirichletEpsilon_) != 0) throw std::invalid_argument(ara_last_error());
+    }
     SearchSettings settings_;
     ara_search_t search_ = nullptr;
     ara_search_result_t result_{};
     float lastValueEval_ = -1.0f, overallNPS_ = 0.0f;
+    float qValueWeight_ = -1.0f, dirichletEpsilon_ = -1.0f;
     size_t nbNPSentries_ = 0;
+};
+
+// RawNetAgent (agents/rawnetagent.cpp:45-83): the move the network's policy prefers, without a search.  mode / inputVersion
+// are the input representation the searches of the same network use (SearchSettings::mode / input_version).
+class RawNetAgent {
+   public:
+    RawNetAgent(NeuralNetAPI* net, int mode, int inputVersion) : net_(net), mode_(mode), inputVersion_(inputVersion) {
+        if (net == nullptr) throw std::invalid_argument("RawNetAgent needs a network");
+    }
+    void evaluate_board_state(const BoardState& state, EvalInfo& evalInfo) {
+        evalInfo = EvalInfo();
+        evalInfo.legalMoves = state.legal_actions();
+        if (evalInfo.legalMoves.empty()) throw std::runtime_error("no legal move in " + state.fen());
+        const float param = mode_ == 1 ? 1.4f : 1.2f;
+        if (evalInfo.legalMoves.size() == 1) {  // a single legal move is played without a forward (depth and nodes 0)
+            evalInfo.policyProbSmall.assign(1, 1.0);
+            evalInfo.bestMove = evalInfo.legalMoves[0];
+            evalInfo.pv = {evalInfo.bestMove};
+            evalInfo.centipawns = value_to_centipawn(0.0f, param);
+            return;
+        }
+        ara_board_t board;
+        ara_state_board(state.handle(), &board);
+        Action moves[512];
+        int policyIdx[512], count = 0;
+        if (ara_legal_moves(&board, 1, moves, &count, nullptr, policyIdx) != 0) throw std::runtime_error(ara_last_error());
+        std::vector<float> planes(net_->get_nb_input_values_total()), priors(count);
+        state.get_state_planes(true, planes.data(), mode_, inputVersion_);
+        float value = 0.0f;
+        if (ara_net_predict_priors(net_->handle(), planes.data(), 1, policyIdx, &count, count, &value, priors.data(), nullptr) != 0)
+            throw std::runtime_error(ara_last_error());
+        evalInfo.legalMoves.assign(moves, moves + count);
+        evalInfo.policyProbSmall.assign(priors.begin(), priors.end());
+        evalInfo.priors = priors;
+        size_t best = 0;  // argmax: the first of equal priors
+        for (size_t i = 1; i < priors.size(); ++i)
+            if (priors[i] > priors[best]) best = i;
+        evalInfo.bestMove = moves[best];
+        evalInfo.pv = {evalInfo.bestMove};
+        evalInfo.rootValue = value;
+        evalInfo.centipawns = value_to_centipawn(value, param);
+        evalInfo.depth = evalInfo.selDepth = evalInfo.nodes = 1;
+    }
+
+   private:
+    NeuralNetAPI* net_;
+    int mode_, inputVersion_;
 };
 
 }  // namespace crazyara

@@ -1,7 +1,8 @@
 // Minimal UCI front-end over the C++ host classes (engine/src/uci/crazyara.cpp:76-143 command loop, option names of
 // uci/optionsuci.cpp:66-220).  Supported: uci, isready, setoption, ucinewgame, position [startpos|fen] [moves ...],
 // go [nodes N | movetime T | wtime W btime B [winc I] [binc I] [movestogo M]] (or the Simulations / Nodes options),
-// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], root, quit.  The move time follows TimeManager::get_time_for_move (manager/timemanager.cpp:51-100) without its
+// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], root, quit.  With Use_Raw_Network a `go`
+// is answered by RawNetAgent (the network's policy alone) instead of a search.  The move time follows TimeManager::get_time_for_move (manager/timemanager.cpp:51-100) without its
 // random factor; the search then also stops after that much wall time (ara_search_set_movetime), and in clock games
 // the ThreadManager's early stopping / prolongation rules run on top (ara_search_set_time_control).
 #include <algorithm>
@@ -34,7 +35,7 @@ struct Options {
                                              {"UCI_Chess960", "false"},     {"Input_Version", "0"},    {"Dirichlet_Seed", "42"},
                                              {"Move_Overhead", "20"},       {"Timed_Search_Nodes", "1000000"},
                                              {"Reuse_Tree", "true"},           {"Use_NPS_Time_Manager", "true"},
-                                             {"Precision", "float16"},
+                                             {"Precision", "float16"},      {"Use_Raw_Network", "false"},
                                              // the reference's defaults (optionsuci.cpp:89-90, :182); Threads 1 and both epsilons 0
                                              // give the deterministic single-threaded search
                                              {"Threads", "2"},              {"Centi_Epsilon_Greedy", "5"},
@@ -69,6 +70,7 @@ int main() {
     Options opt;
     std::unique_ptr<NeuralNetAPI> net;
     std::unique_ptr<MCTSAgent> agent;
+    std::unique_ptr<RawNetAgent> rawAgent;  // Use_Raw_Network (crazyara.cpp:204-209): `go` answers with the policy alone
     BoardState state;
     EvalInfo info;
     bool ready = false;
@@ -104,10 +106,13 @@ int main() {
         s.epsilon_checks_counter = opt.i("Centi_Epsilon_Checks") > 0 ? static_cast<int>(std::lround(100.0 / opt.i("Centi_Epsilon_Checks"))) : 0;
         if (opt.i("Input_Version") > 0) s.input_version = opt.i("Input_Version");
         agent.reset();
+        rawAgent.reset();
         net.reset();
-        if (!opt.kv["Model_Path"].empty())
+        if (!opt.kv["Model_Path"].empty()) {
             net.reset(new NeuralNetAPI("gpu", opt.i("First_Device_ID"), static_cast<unsigned>(s.batch_size), opt.kv["Model_Path"],
                                        opt.kv["Precision"]));
+            rawAgent.reset(new RawNetAgent(net.get(), mode, s.input_version));
+        }
         // a time-limited search has no visit budget to size the node pool from
         // a kept subtree lives in the same pools as the next search: room for a few searches, then the library compacts
         // the subtree to the front of its second set of pools (ara_search_apply_move)
@@ -236,6 +241,25 @@ int main() {
                     ready = false;
                 }
                 if (!ready) prepare();
+                if (opt.b("Use_Raw_Network")) {
+                    if (!rawAgent) {
+                        std::cout << "info string Use_Raw_Network needs a network (setoption name Model_Path)" << std::endl;
+                        continue;
+                    }
+                    searched = false;  // no tree to walk: the position's moves are not announced to it (crazyara.cpp:281)
+                    infiniteSearch = false;
+                    searching.store(true);
+                    worker = std::thread([&]() {
+                        try {
+                            rawAgent->evaluate_board_state(state, info);
+                            print_result();
+                        } catch (const std::exception& e) {
+                            std::cout << "info string error: " << e.what() << std::endl;
+                        }
+                        searching.store(false);
+                    });
+                    continue;
+                }
                 const bool inGame = lim.time[0] != 0 || lim.time[1] != 0 || lim.movestogo != 0;  // is_game_sceneario
                 agent->clear_time_control();
                 const bool report = timed && inGame && !lim.infinite;

@@ -16,8 +16,15 @@ Per game, SelfPlay::generate_game (selfplay.cpp:192-261) with the RL defaults of
   * a game may be resigned (Centi_Resign_Probability of the games, Centi_Resign_Threshold, :163-190).
 Every game may have its own variant (a MODE_LICHESS build plays whatever UCI_Variant is set, selfplay.cpp:367-385):
 `variant` may be a list, one entry per game (cycled).  Games may start from random lines of an EPD file (`epd_path`,
-load_random_fen, selfplay.cpp:58-79).  Not reproduced: quick searches (off in rl_config), opening plies sampled from the
-raw policy (MeanInitPly 0 in rl_config).
+load_random_fen, selfplay.cpp:58-79).
+Two options buy more games per hour (both off by default, as in rl_config):
+  * quick searches (Centi_Quick_Probability, selfplay.cpp:154-159, :183-190, :214-241): each move, with probability
+    `quick_probability`, a game runs a cheap search instead -- `quick_nodes`, `quick_q_value_weight`,
+    `quick_dirichlet_epsilon` for that tree only (ara_search_set_tree_settings) -- and exports no sample for it;
+  * opening plies from the raw network (MeanInitPly, init_starting_state_from_raw_policy, selfplay.cpp:196-202,
+    :423-487): before its first search a game plays Exp(1 / `mean_init_ply`) plies (clipped by `max_init_ply`), each
+    sampled from the policy of RawNetAgent, sometimes flattened (`raw_prob_temperature`).  All games that start in the
+    same step share one network forward per ply.
 Optional outputs: training samples (`exporter=`, crazyara_b200.export) and the games as PGN (`pgn_path=`).
 """
 import os
@@ -26,8 +33,8 @@ import time
 
 import numpy as np
 
-from .engine import (BoardState, MCTSAgent, TERMINAL_DRAW, TERMINAL_LOSS, TERMINAL_NONE, TERMINAL_WIN, default_settings,
-                     encode_planes)
+from .engine import (BoardState, MCTSAgent, RawNetAgent, TERMINAL_DRAW, TERMINAL_LOSS, TERMINAL_NONE, TERMINAL_WIN,
+                     default_settings, encode_planes)
 from .export import BLACK_WIN, DRAWN, WHITE_WIN
 from .pgn import GamePGN, result_string
 
@@ -98,6 +105,36 @@ def set_best_move(res, ply, rng, temperature, temperature_moves, temperature_dec
     return int(res["best_idx"])
 
 
+def init_ply_count(rng, mean_init_ply, max_init_ply):
+    """Plies of a game's raw-network opening (generate_game, selfplay.cpp:196-197): size_t(Exp(1 / MeanInitPly) + 0.5),
+    and beyond MaxInitPly a draw modulo MaxInitPly instead (clip_ply, :466-472).  0 when MeanInitPly is 0 (no draws)."""
+    if mean_init_ply <= 0:
+        return 0
+    ply = int(rng.exponential(mean_init_ply) + 0.5)
+    if ply > max_init_ply:
+        ply = int(rng.integers(0, 1 << 31)) % max_init_ply
+    return ply
+
+
+def apply_raw_policy_temp(p, raw_prob_temperature, rng):
+    """apply_raw_policy_temp (selfplay.cpp:474-487): with probability `raw_prob_temperature` the raw policy is flattened by
+    apply_temperature (blazeutil.h:78-88) with T = 2, or T = 5 / 10 when a second draw falls below 0.25 / 0.05."""
+    p = np.asarray(p, np.float64)
+    if rng.random() < raw_prob_temperature:
+        u = rng.random()
+        temp = 10.0 if u < 0.05 else (5.0 if u < 0.25 else 2.0)
+        p = np.power(p, 1.0 / temp)
+        p = p / p.sum()
+    return p
+
+
+def leads_to_terminal(state, move):
+    """State::leads_to_terminal: the position after `move` (16-bit code) ends the game"""
+    after = state.clone()
+    after.do_action(move)
+    return after.is_terminal() != TERMINAL_NONE
+
+
 def load_random_fen(path, rng):
     """load_random_fen (rl/selfplay.cpp:58-79): a line of the EPD file `path` drawn uniformly, without a trailing ';'.
     No path (None, "" or the reference's "<empty>") gives "", the variant's start position."""
@@ -152,7 +189,13 @@ class Arena:
     def __init__(self, net, settings, variant, n_games, device=0, is960=False, temperature=0.8, temperature_moves=15,
                  max_plies=512, seed=0, max_nodes=0, exporter=None, reuse_tree=False, pgn_path=None,
                  temperature_decay=0.92, quantile_clipping=0.0, policy_clip_thresh=0.01, node_random_factor=0.1,
-                 resign_probability=0.9, resign_threshold=-0.9, epd_path=None):
+                 resign_probability=0.9, resign_threshold=-0.9, epd_path=None, quick_probability=0.0, quick_nodes=100,
+                 quick_q_value_weight=0.7, quick_dirichlet_epsilon=0.0, mean_init_ply=0, max_init_ply=0,
+                 raw_prob_temperature=0.0):
+        if mean_init_ply > 0 and max_init_ply <= 0:
+            raise ValueError("max_init_ply must be positive when mean_init_ply is")
+        if quick_probability >= 0.01 and quick_nodes <= 0:
+            raise ValueError("quick_nodes must be positive when quick_probability is")
         # one variant for all games, or one per game (cycled): KOTH + Three-check mixed = variant=[2, 3]
         self.variants = [int(v) for v in variant] if isinstance(variant, (list, tuple)) else [int(variant)]
         self.variant, self.is960 = self.variants[0], is960
@@ -163,6 +206,9 @@ class Arena:
         self.resign_probability, self.resign_threshold = resign_probability, resign_threshold
         self.rng = np.random.default_rng(seed)
         self.epd_path = epd_path
+        self.quick_probability, self.quick_nodes = quick_probability, quick_nodes
+        self.quick_q_value_weight, self.quick_dirichlet_epsilon = quick_q_value_weight, quick_dirichlet_epsilon
+        self.mean_init_ply, self.max_init_ply, self.raw_prob_temperature = mean_init_ply, max_init_ply, raw_prob_temperature
         # every process / group of games draws its own root noise: the trees' Dirichlet generators start from
         # settings.seed ^ tree index (TreeState::rng), so the groups get distinct seeds derived from the arena's
         import copy
@@ -184,6 +230,10 @@ class Arena:
             st_g.seed = base_seed + 7919 * g
             self.agents.append(MCTSAgent(n, st_g, device, self.per_group, max_nodes))
         self.agent = self.agents[0]
+        # the opening plies' priors come from the first group's network (every group runs the same weights)
+        self.raw_agent = RawNetAgent(nets[0], settings.mode, settings.input_version) if mean_init_ply > 0 else None
+        self.quick = [False] * n_games  # the tree's last search was a quick one: its limits and settings are overridden
+        self.init_plies = [0] * n_games  # raw-network plies still to play before the game's first search
         self.game_variant = [self.variants[t % len(self.variants)] for t in range(n_games)]
         self.states = [self._new_state(t) for t in range(n_games)]
         self.allow_resign = [self._draw_resign() for _ in range(n_games)]
@@ -206,15 +256,63 @@ class Arena:
             self.pgns = [GamePGN(self.game_variant[t], is960, "CrazyAra-B200", "CrazyAra-B200") for t in range(n_games)]
             for g, st in zip(self.pgns, self.states):
                 g.fen = st.fen()
+        self._play_openings(range(n_games))
 
     def _new_state(self, t):
-        # BoardState::init (boardstate.cpp:260-270): chess960 games start from a random chess960 position
+        # generate_game (selfplay.cpp:196-202): the opening's ply count, then the start position -- BoardState::init
+        # (boardstate.cpp:260-270): chess960 games start from a random chess960 position
+        self.init_plies[t] = init_ply_count(self.rng, self.mean_init_ply, self.max_init_ply)
         v = self.game_variant[t]
         return BoardState().set(start_fen(self.rng, v, self.is960, self.epd_path), self.is960, v)
+
+    def _play_openings(self, games):
+        """init_starting_state_from_raw_policy (selfplay.cpp:423-452) for the games that just started: ply by ply, one
+        network forward over all of them, each game samples its move from its legal moves' priors (apply_raw_policy_temp
+        first) and stops early before a move that would end the game.  The moves are game moves: they are in the PGN
+        after its start FEN and count as plies of the game."""
+        todo = [t for t in games if self.init_plies[t] > 0]
+        while todo:
+            evals = self.raw_agent.predict([self.states[t] for t in todo])
+            nxt = []
+            for t, (moves, priors, _) in zip(todo, evals):
+                st = self.states[t]
+                if len(moves) == 0:  # (a start position without a legal move: the first search ends the game)
+                    self.init_plies[t] = 0
+                    continue
+                p = apply_raw_policy_temp(priors, self.raw_prob_temperature, self.rng)
+                move = moves[int(self.rng.choice(len(p), p=p / p.sum()))]
+                if leads_to_terminal(st, move):
+                    self.init_plies[t] = 0
+                    continue
+                if self.pgns is not None:
+                    self.pgns[t].play_move(st, move)
+                else:
+                    st.do_action(move)
+                self.plies[t] += 1
+                self.init_plies[t] -= 1
+                if self.init_plies[t] > 0:
+                    nxt.append(t)
+            todo = nxt
 
     def _draw_resign(self):
         # SelfPlay::is_resignation_allowed (selfplay.cpp:163-168): decided once per game
         return self.resign_probability >= 0.01 and self.rng.random() < self.resign_probability
+
+    def _search_budget(self):
+        """The draws of generate_game before a search (selfplay.cpp:212-220): the random integer of adjust_node_count,
+        is_quick_search, then the node jitter on the budget of that search (adjust_node_count, :146-152: nodes +=
+        rand % maxRandomNodes - maxRandomNodes / 2).  Returns (node budget or None for the settings' own, quick?)."""
+        nodes = int(self.settings.nodes)
+        quick_on = self.quick_probability >= 0.01
+        span = int(nodes * self.node_random_factor) if self.node_random_factor > 0 else 0
+        rand_int = int(self.rng.integers(0, 1 << 31)) if span or quick_on else 0
+        quick = quick_on and self.rng.random() < self.quick_probability
+        if quick:
+            nodes = int(self.quick_nodes)
+            span = int(nodes * self.node_random_factor) if self.node_random_factor > 0 else 0
+        if span:
+            nodes += rand_int % span - span // 2
+        return (nodes if span or quick else None), quick
 
     def _pick(self, res, ply):
         return set_best_move(res, ply, self.rng, self.temperature, self.temperature_moves, self.temperature_decay,
@@ -238,13 +336,16 @@ class Arena:
         """One move in every running game."""
         G = self.per_group
         for t, st in enumerate(self.states):
-            self.agents[t // G].set_position(st, t % G)
-            if self.node_random_factor > 0 and self.settings.nodes:
-                # SelfPlay::adjust_node_count (selfplay.cpp:146-152): nodes += rand % maxRandomNodes - maxRandomNodes / 2
-                span = int(self.settings.nodes * self.node_random_factor)
-                if span:
-                    jitter = int(self.rng.integers(0, 1 << 31)) % span - span // 2
-                    self.agents[t // G].set_search_limits(self.settings.simulations, int(self.settings.nodes) + jitter, t % G)
+            agent, lt = self.agents[t // G], t % G
+            agent.set_position(st, lt)
+            nodes, quick = self._search_budget()
+            if nodes is not None or self.quick[t]:  # (after a quick search the settings' budget comes back)
+                agent.set_search_limits(self.settings.simulations, self.settings.nodes if nodes is None else nodes, lt)
+            if quick:
+                agent.set_tree_settings(self.quick_q_value_weight, self.quick_dirichlet_epsilon, lt)
+            elif self.quick[t]:  # reset_search_params (selfplay.cpp:183-190)
+                agent.set_tree_settings(-1.0, -1.0, lt)
+            self.quick[t] = quick
         t_search = time.perf_counter()
         if len(self.agents) == 1:
             self.agent.evaluate_board_state()
@@ -265,7 +366,7 @@ class Arena:
                 self._game_over(t, st.is_terminal(), st.side_to_move())
                 continue
             idx = self._pick(res, self.plies[t])
-            if self.exporter is not None:
+            if self.exporter is not None and not self.quick[t]:  # a quick search exports nothing (selfplay.cpp:228)
                 # sharpen_distribution (blazeutil.h:94-105) after the move has been chosen (selfplay.cpp:230-232); the
                 # stored q is EvalInfo::bestMoveQ[0], not the Q of the sampled move (traindataexporter.cpp:50-53)
                 self.exporter.save_sample(self.records[t], planes[t], res["moves"],
@@ -285,6 +386,7 @@ class Arena:
                 term = TERMINAL_WIN
             if term != TERMINAL_NONE or self.plies[t] >= self.max_plies:
                 self._game_over(t, term, st.side_to_move())
+        self._play_openings(range(self.n_games))  # (the games started in this step: the others have no plies left)
 
     def run(self, min_games=0, max_steps=1 << 30, max_seconds=1e30):
         t0 = time.perf_counter()
@@ -329,6 +431,12 @@ def plan_workers(total_games, devices, out_dir):
     return plan
 
 
+# Arena options of the launcher with the reference's defaults (optionsuci.cpp:200-217), except MeanInitPly / MaxInitPly /
+# Centi_Raw_Prob_Temperature, which default to 0 here: openings from the raw network are off unless asked for
+_OPTION_DEFAULTS = dict(quick_probability=0.0, quick_nodes=100, quick_q_value_weight=0.7, quick_dirichlet_epsilon=0.0,
+                        mean_init_ply=0, max_init_ply=0, raw_prob_temperature=0.0)
+
+
 def _worker(job, args):
     from .export import TrainDataExporter
     from .nn import NeuralNetAPI
@@ -339,9 +447,11 @@ def _worker(job, args):
     channels = nets[0].get_nb_input_values_total() // 64
     exporter = TrainDataExporter(job["zarr"], args.mode, channels, number_chunks=args.chunks) if args.export else None
     variants = [int(v) for v in str(args.variant).split(",")]
+    # quick searches and raw-network openings (off unless their flags are given)
+    options = {k: getattr(args, k) for k in _OPTION_DEFAULTS if getattr(args, k, None) is not None}
     arena = Arena(nets if groups > 1 else nets[0], st, variant=variants if len(variants) > 1 else variants[0], n_games=job["n_games"], device=job["device"],
                   is960=args.chess960, max_plies=args.max_plies, seed=args.seed + job["seed_offset"], exporter=exporter,
-                  pgn_path=job["pgn"] if args.pgn else None)
+                  pgn_path=job["pgn"] if args.pgn else None, **options)
     res = arena.run(min_games=args.games_per_worker, max_seconds=args.seconds)
     arena.close()
     for n in nets:
@@ -372,6 +482,18 @@ def main(argv=None):
     ap.add_argument("--out", default=".", help="directory of data_gpu_<id>.zarr / games_gpu_<id>.pgn")
     ap.add_argument("--no-export", dest="export", action="store_false")
     ap.add_argument("--no-pgn", dest="pgn", action="store_false")
+    ap.add_argument("--quick-probability", type=float, default=_OPTION_DEFAULTS["quick_probability"],
+                    help="Centi_Quick_Probability / 100: share of the moves searched with the quick settings (no sample exported)")
+    ap.add_argument("--quick-nodes", type=int, default=_OPTION_DEFAULTS["quick_nodes"], help="Quick_Nodes")
+    ap.add_argument("--quick-q-value-weight", type=float, default=_OPTION_DEFAULTS["quick_q_value_weight"],
+                    help="Centi_Quick_Q_Value_Weight / 100")
+    ap.add_argument("--quick-dirichlet-epsilon", type=float, default=_OPTION_DEFAULTS["quick_dirichlet_epsilon"],
+                    help="Centi_Quick_Dirichlet_Epsilon / 100")
+    ap.add_argument("--mean-init-ply", type=float, default=_OPTION_DEFAULTS["mean_init_ply"],
+                    help="MeanInitPly: mean number of opening plies sampled from the raw network (0 = off)")
+    ap.add_argument("--max-init-ply", type=int, default=_OPTION_DEFAULTS["max_init_ply"], help="MaxInitPly")
+    ap.add_argument("--raw-prob-temperature", type=float, default=_OPTION_DEFAULTS["raw_prob_temperature"],
+                    help="Centi_Raw_Prob_Temperature / 100: share of the opening plies sampled from a flattened policy")
     args = ap.parse_args(argv)
     os.makedirs(args.out, exist_ok=True)
     plan = plan_workers(args.games, [int(d) for d in args.devices.split(",")], args.out)

@@ -190,6 +190,13 @@ int ara_search_set_position(ara_search_t s, int tree, const ara_board_t* root, c
  * handle was created for (ara_search_create max_nodes).  Self-play jitters the node budget of every search
  * (SelfPlay::adjust_node_count, rl/selfplay.cpp:146-152). */
 int ara_search_set_limits(ara_search_t s, int tree, unsigned simulations, unsigned nodes);
+/* The Q-value weight of the posterior (Centi_Q_Value_Weight / 100, 0..999.99) and the Dirichlet epsilon of the root
+ * noise (Centi_Dirichlet_Epsilon / 100, 0..1) of the following go calls for tree `tree` (-1 = every tree) instead of
+ * the settings' values; a negative value means the settings' value again.  Like the limits, the values last until they
+ * are changed.  Self-play's quick searches use it: a game that draws a quick search gets a smaller node budget, its
+ * own Q-value weight and epsilon for that one search while the handle's other trees search as usual
+ * (SelfPlay::generate_game, rl/selfplay.cpp:214-241). */
+int ara_search_set_tree_settings(ara_search_t s, int tree, float q_value_weight, float dirichlet_epsilon);
 /* tree -1 = every tree.  An inactive tree is left out of the following ara_search_begin / step / go calls until it is
  * made active again; new handles start with every tree active.  The set is read when a search begins.  An idle tree is
  * not touched: its statistics, its Dirichlet generator and a subtree kept by ara_search_apply_move stay as they are
