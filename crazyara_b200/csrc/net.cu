@@ -151,9 +151,9 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
            : (hdr.channels != 256 || hdr.value_channels != 8 || hdr.value_fc != 256))
         return set_error("ara_net_create: unsupported trunk geometry (channels %d, value %d/%d)", hdr.channels,
                          hdr.value_channels, hdr.value_fc);
-    if (hdr.n_blocks < 1 || hdr.n_blocks > 64 || hdr.in_channels < 1 || hdr.in_channels > 256 ||
-        hdr.policy_channels < 1 || hdr.policy_channels > 256)
-        return set_error("ara_net_create: implausible header");
+    if (hdr.n_blocks < 1 || hdr.n_blocks > 64) return set_error("ara_net_create: %d blocks (1 .. 64)", hdr.n_blocks);
+    if (hdr.in_channels < 1 || hdr.in_channels > 256 || hdr.policy_channels < 1 || hdr.policy_channels > 256)
+        return set_error("ara_net_create: in_channels %d, policy_channels %d (1 .. 256 each)", hdr.in_channels, hdr.policy_channels);
     const int C = hdr.channels;
     blocks.resize(hdr.n_blocks);
     max_cop_ = 0;
@@ -361,6 +361,7 @@ int Net::build_half(const HostWeights& hw) {
     std::vector<TrunkBlockHost> tb;
     auto flush = [&]() {
         if (tb.empty()) return 0;
+        stages_.push_back({false, static_cast<int>(trunks_.size()), -1});
         trunks_.emplace_back(new RiseTrunk());
         if (rise_trunk_init(trunks_.back().get(), tb, trunks_.size() == 1 ? d_x[0] : d_x[1], d_x[1])) return -1;
         tb.clear();
@@ -370,10 +371,15 @@ int Net::build_half(const HostWeights& hw) {
         const BlockDesc& bd = blocks[i];
         const HostBlock& hb = hw.blocks[i];
         if (bd.ntb) {
+            if (flush()) return -1;
+            stages_.push_back({true, static_cast<int>(ntbs_.size()), i});
             ntbs_.emplace_back();
-            if (flush() || build_ntb_half(bd, hb, &ntbs_.back())) return -1;
+            if (build_ntb_half(bd, hb, &ntbs_.back())) return -1;
             continue;
         }
+        // a run of more blocks than one tower kernel's argument block holds continues in the next segment: the trunk
+        // passes between segments as fp16 in d_x[1], as the kernel keeps it between its own blocks
+        if (tb.size() == static_cast<size_t>(kTrunkMaxBlocks) && flush()) return -1;
         tb.emplace_back();
         TrunkBlockHost& t = tb.back();
         t.c_op = bd.c_op;
@@ -619,11 +625,9 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
         PdlSuspend no_pdl(io_in_h[1] != nullptr);
         if (launch_tower(0, n, s, cnt, (io == 1 && d_x0_alt != nullptr) ? d_x0_alt : nullptr)) return -1;
     }
-    // AlphaVile: NTB, tower segment, NTB, ... (the blob reader refuses an NTB at block 0)
-    for (size_t seg = 1, k = 0, i = 0; i < blocks.size(); ++i) {
-        if (!blocks[i].ntb) continue;
-        if (enqueue_ntb_half(blocks[i], ntbs_[k++], n, s, cnt)) return -1;
-        if (i + 1 < blocks.size() && !blocks[i + 1].ntb && launch_tower(seg++, n, s, cnt)) return -1;
+    for (size_t k = 1; k < stages_.size(); ++k) {
+        const Stage& st = stages_[k];
+        if (st.ntb ? enqueue_ntb_half(blocks[st.block], ntbs_[st.index], n, s, cnt) : launch_tower(st.index, n, s, cnt)) return -1;
     }
     __half* xfinal = d_x[1];
     ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};

@@ -175,9 +175,17 @@ class Net {
     ConvLayer stem_conv;
     ConvLayer stem_conv2;  // the stem reading the second input set
     std::vector<PreciseBlock> pb_;
-    // float16: the tower as segments, one tower kernel per run of bottleneck blocks between NTBs
+    // float16: the tower as segments, one tower kernel per run of at most kTrunkMaxBlocks bottleneck blocks
     std::vector<std::unique_ptr<RiseTrunk>> trunks_;
     std::vector<NtbLayers> ntbs_;  // one per NTB, in block order (both precisions)
+    // float16: what runs between the stem and the heads, in block order, as build_half laid it out: tower segment
+    // trunks_[index] or NTB ntbs_[index] (of block `block`).  Stage 0 is a tower segment (the blob reader refuses an NTB
+    // at block 0).
+    struct Stage {
+        bool ntb;
+        int index, block;
+    };
+    std::vector<Stage> stages_;
     int max_m_ = 0, max_ca_ = 0, max_h_ = 0;  // the widest NTB
     // NTB activations.  float16: d_nt [rows, 256] = y1 | z2 | 0, d_qkv [rows, 3M], d_att [rows, M], d_g [rows, Ca],
     // d_hid [rows, H].  float32: fp32 y / q|k|v / z / x2 and split y, attention, z, group conv, x2, hidden.

@@ -34,12 +34,16 @@ def av_net(tmp_path):
         n.close()
 
 
-def _predict(net, arch, x, batch):
+def _predict(net, arch, x, batch, aux=None):
+    """aux (optional): [n, 4] buffer for the WDL / plys outputs"""
     n, pch = x.shape[0], arch["policy_channels"]
     xin = np.zeros((batch, arch["in_channels"], 8, 8), np.float32)
     xin[:n] = x
     v, p = np.full(batch, np.nan, np.float32), np.full((batch, pch * 64), np.nan, np.float32)
-    net.predict(xin, v, p, None, n=n)
+    a = None if aux is None else np.full((batch, 4), np.nan, np.float32)
+    net.predict(xin, v, p, a, n=n)
+    if aux is not None:
+        aux[:] = a[:n]
     return v[:n].copy(), p[:n].copy()
 
 
@@ -65,10 +69,17 @@ def test_alphavile_float16_matches_oracle(av_net, name, n):
 def test_alphavile_float32_within_1e4_of_oracle(av_net, name, n):
     net, arch, sd = av_net(name, n, "float32")
     x = golden_input(arch, n=n, seed=22)
-    v, p = _predict(net, arch, x, n)
+    aux = np.full((n, 4), np.nan, np.float32)
+    v, p = _predict(net, arch, x, n, aux if arch["wdl"] else None)
     ref = oav.forward(sd, arch, x)
     np.testing.assert_allclose(v, ref["value"], atol=F32_ATOL, rtol=0)
     np.testing.assert_allclose(p, ref["prob"], atol=F32_ATOL, rtol=0)
+    np.testing.assert_allclose(p, ref["prob"], rtol=2e-3, atol=1e-8)  # and small probabilities relatively
+    lg = np.log(p) - np.log(p).mean(1, keepdims=True)
+    lr = ref["policy_logits"] - ref["policy_logits"].mean(1, keepdims=True)
+    assert np.abs(lg - lr).max() < 1e-3
+    if arch["wdl"]:
+        np.testing.assert_allclose(aux, ref["aux"], atol=F32_ATOL, rtol=0)
 
 
 @pytest.mark.gpu

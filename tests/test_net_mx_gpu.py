@@ -91,6 +91,10 @@ def test_mx_net_float32_within_1e4_of_oracle(mx_net, name, n):
     ref = net_mx.forward_mx(params, arch, x)
     np.testing.assert_allclose(v, ref["value"], atol=F32_ATOL, rtol=0)
     np.testing.assert_allclose(p, ref["prob"], atol=F32_ATOL, rtol=0)
+    np.testing.assert_allclose(p, ref["prob"], rtol=2e-3, atol=1e-8)  # and small probabilities relatively
+    lg = np.log(p) - np.log(p).mean(1, keepdims=True)
+    lr = ref["policy_logits"] - ref["policy_logits"].mean(1, keepdims=True)
+    assert np.abs(lg - lr).max() < 1e-3  # (the symbols' value heads have no WDL / plys outputs)
 
 
 @pytest.mark.gpu
