@@ -114,6 +114,11 @@ extern "C" int ara_encode_planes_device(const void* boards_dev, int n, int mode,
                                         void* planes_half_nhwc_dev, int cpad, void* stream) {
     const int c = planes_channels(mode, version);
     if (c < 0) return set_error("ara_encode_planes_device: unsupported mode %d / version %d", mode, version);
+    if (n < 0) return set_error("ara_encode_planes_device: negative board count %d", n);
+    if (planes_half_nhwc_dev != nullptr && normalize == 0)
+        return set_error("ara_encode_planes_device: the fp16 NHWC output is the stem's input and always normalised; "
+                         "normalize = 0 is only available for the fp32 output");
+    if (n == 0) return 0;
     const int grid = (n + kWarpsPerBlock - 1) / kWarpsPerBlock;
     if (planes_dev != nullptr)
         encode_planes_f32_kernel<<<grid, 32 * kWarpsPerBlock, 0, (cudaStream_t)stream>>>((const Board*)boards_dev, n, mode, version, normalize, planes_dev, c);

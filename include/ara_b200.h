@@ -86,7 +86,9 @@ int ara_move_to_uci(unsigned short move, int is960, char* buf8);
  * version: 1, 2, 3.  planes_out: [n, C, 8, 8] fp32, C = 34/51/64, 39/52, 63/80.  Host buffers. */
 int ara_encode_planes(const ara_board_t* boards, int n, int mode, int version, int normalize, float* planes_out);
 /* device-resident variant: boards_dev [n] in HBM -> planes_dev [n,C,8,8] fp32 and/or planes_half_nhwc_dev
- * [n, 64, cpad] fp16 (the stem convolution's input layout); asynchronous on `stream`. */
+ * [n, 64, cpad] fp16 (the stem convolution's input layout, cpad 64 or 128 >= C, channels >= C zero); asynchronous on
+ * `stream`.  The fp16 output is always normalised, as the network reads it: with planes_half_nhwc_dev set, normalize = 0
+ * is refused.  n = 0 launches nothing and returns 0; n < 0 is refused. */
 int ara_encode_planes_device(const void* boards_dev, int n, int mode, int version, int normalize, float* planes_dev,
                              void* planes_half_nhwc_dev, int cpad, void* stream);
 

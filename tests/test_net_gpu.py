@@ -136,24 +136,36 @@ def test_net_create_fails_loudly_on_bad_blob(tmp_path):
         NeuralNetAPI("gpu", 0, 8, str(tmp_path / "missing.arab"))
 
 
-@pytest.mark.gpu
-def test_net_output_of_a_position_does_not_depend_on_its_batch(tmp_path):
-    """The search relies on this: a leaf's value / policy are the same bits whichever mini-batch evaluates it."""
+def _assert_rows_independent(tmp_path, precision):
+    """A board's value / policy bits at a row of a batch of 3 equal its bits at its row of a batch of 64."""
     arch = onet.arch_risev2(34, 81)
     x = golden_input(arch, n=64, seed=9)
-    net64, _ = _make_net(tmp_path, arch, 64, 10)
+    net64, _ = _make_net(tmp_path, arch, 64, 10, precision)
     v64, p64 = np.zeros(64, np.float32), np.zeros((64, 81 * 64), np.float32)
     net64.predict(x, v64, p64, None, n=64)
     net64.close()
-    net3, _ = _make_net(tmp_path, arch, 3, 10)
+    net3, _ = _make_net(tmp_path, arch, 3, 10, precision)
     for src in (0, 37, 63):
         xin = np.zeros((3, 34, 8, 8), np.float32)
         xin[1] = x[src]
         xin[0] = x[(src + 5) % 64]
         v, p = np.zeros(3, np.float32), np.zeros((3, 81 * 64), np.float32)
         net3.predict(xin, v, p, None, n=2)
-        assert v[1] == v64[src] and np.array_equal(p[1], p64[src])
+        assert v[1] == v64[src] and np.array_equal(p[1], p64[src]), (precision, src)
     net3.close()
+
+
+@pytest.mark.gpu
+def test_net_output_of_a_position_does_not_depend_on_its_batch(tmp_path):
+    """The search relies on this: a leaf's value / policy are the same bits whichever mini-batch evaluates it."""
+    _assert_rows_independent(tmp_path, "float16")
+
+
+@pytest.mark.gpu
+def test_float32_net_output_of_a_position_does_not_depend_on_its_batch(tmp_path):
+    """The same in Precision float32, where the 1x1 convolutions of the tower are GEMM launches whose tile width follows
+    the batch (conv_layer_choose_bn): packed multi-tree float32 searches put a leaf at any row of a batch of any size."""
+    _assert_rows_independent(tmp_path, "float32")
 
 
 @pytest.mark.gpu

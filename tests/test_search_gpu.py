@@ -10,6 +10,7 @@ import pytest
 
 from oracle import search as osr
 from oracle.chess import Position
+from tests.test_device_rules_hostemu import FENS_960
 from tests.test_search_hostemu import CASES, assert_same_search, case_settings
 
 
@@ -131,41 +132,114 @@ def _net_fn(net):
     return fn
 
 
-REAL_CASES = [("crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, [], 8, 800),           # BASELINE cfg 2
-              ("crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, [], 64, 3200),         # the headline workload (bench.py)
-              ("crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, ["e2e4", "e7e5"], 64, 1600),
-              ("chess", 0, "chess", "risev33", 52, 76, 3, [], 64, 1600),                  # BASELINE cfg 3
-              ("kingofthehill", 2, "lichess", "risev2", 63, 84, 1, ["e2e4", "e7e5"], 128, 800),   # BASELINE cfg 5
-              ("3check", 3, "lichess", "risev2", 63, 84, 1, ["e2e4", "e7e5"], 128, 800)]
+def _arch(arch_name, cin, pch):
+    from oracle import net as onet
+    return onet.arch_risev2(cin, pch) if arch_name == "risev2" else onet.arch_risev33(cin, pch, True)
+
+
+# A middlegame with both pockets, promoted pieces of both colours ("~"), rule50 37 (/ 40) and move 253 (/ 500)
+CZ_MIDDLEGAME = "4R2b~/1N3rkb/1p2P1pp/p2P4/2P1P3/8/PP4Q~1/3R3K[QRBBNNNPPPPpp] w - - 37 253"
+
+# (id, variant, variant id, mode, network, input planes, policy planes, input version, FEN (None: start position),
+#  chess960, moves played first, Batch_Size, Simulations).  Every input layout of the device encoder: chess v3 is the
+#  layout of the chess960 self-play configuration (bench --config 4), lichess v1 that of KOTH + Three-check (--config 5),
+#  and lichess v3 (80 planes) the only one whose stem input is padded to 128 channels.
+REAL_CASES = [("cz1-b8", "crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, None, False, [], 8, 800),   # BASELINE cfg 2
+              ("cz1-b64-headline", "crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, None, False, [], 64, 3200),
+              ("cz1-b64-e4e5", "crazyhouse", 1, "crazyhouse", "risev2", 34, 81, 1, None, False, ["e2e4", "e7e5"], 64, 1600),
+              ("chess3-b64", "chess", 0, "chess", "risev33", 52, 76, 3, None, False, [], 64, 1600),   # BASELINE cfg 3
+              ("koth1-b128", "kingofthehill", 2, "lichess", "risev2", 63, 84, 1, None, False, ["e2e4", "e7e5"], 128, 800),
+              ("3check1-b128", "3check", 3, "lichess", "risev2", 63, 84, 1, None, False, ["e2e4", "e7e5"], 128, 800),
+              ("cz2-b16", "crazyhouse", 1, "crazyhouse", "risev2", 51, 81, 2, None, False, ["e2e4", "d7d5", "e4d5", "d8d5"],
+               16, 600),
+              ("cz3-b16-middlegame", "crazyhouse", 1, "crazyhouse", "risev33", 64, 81, 3, CZ_MIDDLEGAME, False, [], 16, 600),
+              ("cz2-b8-middlegame", "crazyhouse", 1, "crazyhouse", "risev2", 51, 81, 2, CZ_MIDDLEGAME, False, [], 8, 400),
+              ("chess1-b16", "chess", 0, "chess", "risev2", 39, 76, 1, None, False, ["e2e4", "c7c5"], 16, 600),
+              ("koth3-b16", "kingofthehill", 2, "lichess", "risev2", 80, 84, 3, None, False, ["e2e4", "e7e5", "e1e2"], 16, 600),
+              ("3check3-b32", "3check", 3, "lichess", "risev2", 80, 84, 3, None, False,
+               ["e2e4", "e7e5", "f1c4", "f8c5", "c4f7", "e8f7"], 32, 800),
+              ("chess960-3-b16", "chess", 0, "chess", "risev33", 52, 76, 3, FENS_960[2], True, [], 16, 600),
+              ("chess960-1-b16", "chess", 0, "chess", "risev2", 39, 76, 1, FENS_960[1], True, [], 16, 600)]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant,vid,mode,arch_name,cin,pch,version,premoves,batch,sims", REAL_CASES)
-def test_gpu_search_real_net_equals_oracle_driven_by_same_net(tmp_path, variant, vid, mode, arch_name, cin, pch, version,
-                                                              premoves, batch, sims):
-    from oracle import net as onet
-    arch = onet.arch_risev2(cin, pch) if arch_name == "risev2" else onet.arch_risev33(cin, pch, True)
-    net = _make_net(tmp_path, arch, batch, version * 10)
+@pytest.mark.parametrize("precision", ["float16", "float32"])
+@pytest.mark.parametrize("case", REAL_CASES, ids=[c[0] for c in REAL_CASES])
+def test_gpu_search_real_net_equals_oracle_driven_by_same_net(tmp_path, case, precision):
+    """The device search writes each leaf's planes straight into the network's input (the fp16 NHWC or, in Precision
+    float32, the split hi | hi | lo encoder of csrc/planes_dev.cuh); the oracle's planes reach the same network through
+    ara_net_predict and its NCHW conversion.  Both round alike, so one differing input bit shows up in a value and so in
+    Q: bit-exact in both precisions."""
+    _, variant, vid, mode, arch_name, cin, pch, version, fen, is960, premoves, batch, sims = case
+    net = _make_net(tmp_path, _arch(arch_name, cin, pch), batch, version * 10, precision=precision)
     st = osr.default_settings(mode, batch_size=batch, simulations=sims, node_policy_temperature=1.0, input_version=version)
-    pos = Position(variant=variant)
+    pos = Position(fen, variant, is960)
     pos.push_uci(*premoves)
     S = osr.Search(st)
     ro = S.run(pos, _net_fn(net))
-    rg = _gpu_search(vid, None, False, premoves, st, net=net)[0]
+    rg = _gpu_search(vid, fen, is960, premoves, st, net=net)[0]
     assert_same_search(ro, rg)
     # default node temperature 1.7: glibc powf restated on the device, sequential normalising sum -> still bit-exact
     st2 = osr.default_settings(mode, batch_size=batch, simulations=sims, input_version=version)
     st2.node_policy_temperature = 1.7
     ro2 = osr.Search(st2).run(pos, _net_fn(net))
-    rg2 = _gpu_search(vid, None, False, premoves, st2, net=net)[0]
+    rg2 = _gpu_search(vid, fen, is960, premoves, st2, net=net)[0]
     assert_same_search(ro2, rg2)
     # Threads = 2 with the real network (second input / output set of the net, forwards on the network stream)
     if 2 * batch < 256:
         st3 = osr.default_settings(mode, batch_size=batch, simulations=sims, input_version=version, threads=2)
         st3.node_policy_temperature = 1.7
         ro3 = osr.Search(st3).run(pos, _net_fn(net), threads=2)
-        rg3 = _gpu_search(vid, None, False, premoves, st3, net=net)[0]
+        rg3 = _gpu_search(vid, fen, is960, premoves, st3, net=net)[0]
         assert_same_search(ro3, rg3)
+    net.close()
+
+
+# Handles whose trees search different positions (and variants) and share every network batch, as self-play and
+# arena games do: (id, mode, network, input planes, policy planes, input version, [(variant, variant id, FEN, chess960,
+# moves played first)])
+PACKED_CASES = [
+    ("lichess1-koth-3check", "lichess", "risev2", 63, 84, 1,
+     [("kingofthehill", 2, None, False, []), ("3check", 3, None, False, ["e2e4", "e7e5"]),
+      ("kingofthehill", 2, None, False, ["e2e4", "e7e5", "e1e2"]), ("3check", 3, None, False, ["e2e4", "f7f6", "d1h5", "g7g6"])]),
+    ("lichess3-koth-3check", "lichess", "risev2", 80, 84, 3,
+     [("3check", 3, None, False, ["e2e4", "e7e5", "f1c4", "f8c5", "c4f7", "e8f7"]), ("kingofthehill", 2, None, False, ["d2d4"]),
+      ("3check", 3, None, False, []), ("kingofthehill", 2, None, False, ["e2e4", "e7e5", "e1e2", "e8e7"])]),
+    ("chess3-chess960", "chess", "risev33", 52, 76, 3,
+     [("chess", 0, FENS_960[0], True, []), ("chess", 0, FENS_960[1], True, []), ("chess", 0, FENS_960[2], True, ["b2b3"]),
+      ("chess", 0, None, False, ["e2e4"])]),
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("threads", [1, 2])
+@pytest.mark.parametrize("precision", ["float16", "float32"])
+@pytest.mark.parametrize("case", PACKED_CASES, ids=[c[0] for c in PACKED_CASES])
+def test_gpu_packed_trees_of_different_positions_equal_oracle_searches(tmp_path, case, precision, threads):
+    """One handle, one tree per position: the new leaves of all trees are packed into consecutive rows of each network
+    batch.  Every tree must equal the oracle's search of its own position driven by the same network (no Dirichlet
+    noise, so the per-tree seeds play no part)."""
+    from crazyara_b200.engine import BoardState, MCTSAgent, SearchSettings
+    _, mode, arch_name, cin, pch, version, trees = case
+    B, sims = 8, 400
+    net = _make_net(tmp_path, _arch(arch_name, cin, pch), len(trees) * B, version * 10, precision=precision)
+    st = osr.default_settings(mode, batch_size=B, simulations=sims, node_policy_temperature=1.7, input_version=version,
+                              threads=threads)
+    s = SearchSettings()
+    for f, _ in s._fields_:
+        setattr(s, f, getattr(st, f))
+    agent = MCTSAgent(net, s, 0, len(trees))
+    for t, (_, vid, fen, is960, moves) in enumerate(trees):
+        agent.set_position(BoardState().set(fen or "", is960, vid).do_uci(*moves), t)
+    agent.evaluate_board_state()
+    together = agent.results()
+    agent.close()
+    for t, (variant, _, fen, is960, moves) in enumerate(trees):
+        pos = Position(fen, variant, is960)
+        pos.push_uci(*moves)
+        ro = osr.Search(st).run(pos, _net_fn(net), threads=threads)
+        assert_same_search(ro, together[t])
+        assert together[t]["evals"] > 0
     net.close()
 
 
@@ -181,7 +255,7 @@ def test_gpu_search_float32_net_against_oracle_search_with_the_fp32_oracle_netwo
     contract is north_star's: root value, root priors, Q and the posterior within 1e-4, the same best move, and visit
     counts that differ by a handful at most."""
     from oracle import net as onet
-    arch = onet.arch_risev2(cin, pch) if arch_name == "risev2" else onet.arch_risev33(cin, pch, True)
+    arch = _arch(arch_name, cin, pch)
     sd = onet.make_state_dict(arch, 0)
     net = _make_net(tmp_path, arch, batch, version * 10, precision="float32")
     st = osr.default_settings(mode, batch_size=batch, simulations=sims, input_version=version)
