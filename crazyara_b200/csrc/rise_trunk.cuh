@@ -28,14 +28,15 @@ struct RtCfg {
 };
 
 // -DARA_TRUNK_PROF: per-role cycle counters of CTA 0 (args.prof[role * 16 + slot]; role 1: rise_trunk_kernel, role 0:
-// rise_trunk_pair_kernel); see tools/prof_trunk.py
+// rise_trunk_pair_kernel); see tools/prof_trunk.py.  32-bit sums (a tower takes well under 2^32 cycles): 64-bit ones
+// would take 16 more registers, and the pair kernel has none to spare at 3 warps per SM sub-partition (168 each)
 #if defined(ARA_TRUNK_PROF)
-#define RT_PROF_DECL() long long pt_ = clock64(); unsigned long long pacc_[16] = {}
-#define RT_PROF(idx)                                               \
-    do {                                                           \
-        const long long now_ = clock64();                          \
-        pacc_[idx] += static_cast<unsigned long long>(now_ - pt_); \
-        pt_ = now_;                                                \
+#define RT_PROF_DECL() long long pt_ = clock64(); unsigned pacc_[16] = {}
+#define RT_PROF(idx)                                      \
+    do {                                                  \
+        const long long now_ = clock64();                 \
+        pacc_[idx] += static_cast<unsigned>(now_ - pt_);  \
+        pt_ = now_;                                       \
     } while (0)
 #define RT_PROF_FLUSH(role)                                                          \
     do {                                                                             \
@@ -409,6 +410,20 @@ struct RtPairCfg {
 // both consumer warpgroups of a pair CTA (named barrier 3; 1 and 2 are the warpgroups' own)
 __device__ __forceinline__ void rt_pair_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
 
+// the X tile as MMA1's A operand in registers (wgmma_f16_rs): xa[4 p + k] = rows 16 w .. 16 w + 15 (w: the warp in its
+// warpgroup), channels 64 p + 16 k .. + 15.  ldmatrix.x4 lane l addresses row 16 w + 8 ((l >> 3) & 1) + (l & 7) of
+// tile l >> 3, whose channels start at 8 (l >> 4) of the k step.  Volatile: X changes between blocks at the same
+// addresses, so the loads must stay where they are.
+__device__ __forceinline__ void rt_load_x_frags(uint32_t aX, uint32_t (&xa)[16][4], int w, int lane) {
+    const int row = 16 * w + 8 * ((lane >> 3) & 1) + (lane & 7), c8 = 8 * (lane >> 4);
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(xa[i][0]), "=r"(xa[i][1]), "=r"(xa[i][2]), "=r"(xa[i][3])
+                     : "r"(aX + rt_x_off(row, 16 * i + c8))
+                     : "memory");
+}
+
 // squeeze-excitation of the pair on the block input, in place; tid: 0 .. 255 over both consumer warpgroups.  Each CTA
 // pools all 256 channels of its own X copy (thread tid: channel tid), then computes the outputs of its rank r from its
 // SE image (unit i in ring slot (u2 + i) % kW2Ring), each one sequential sum: ca_se hidden 64 r .. 64 r + 63 (threads
@@ -615,6 +630,11 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                 n_ca += B.se_type == 1;
             }
             RT_PROF(2);  // squeeze-excitation
+            // X is final for this block here (the SE above, else the previous block's exchange or the stem input):
+            // MMA1 reads it from registers, so that each wgmma reads only its W1 rows from shared memory
+            uint32_t xa[16][4];
+            rt_load_x_frags(aX, xa, w, lane);
+            RT_PROF(14);  // X -> registers
             int own = B.chunk0 + ((B.chunk0 & 1) != static_cast<int>(rank));  // the next own chunk without its H2
             for (int j = 0; j < nch; ++j) {
                 const int gc = B.chunk0 + j;
@@ -633,8 +653,8 @@ __global__ void __launch_bounds__(RtPairCfg::kThreads, 1) rise_trunk_pair_kernel
                     for (int p = 0; p < 4; ++p)
 #pragma unroll
                         for (int k = 0; k < 4; ++k)
-                            wgmma_f16<32>(acc1, wgmma_desc_k_sw128(aX + p * 8192 + k * 32, 1024),
-                                          wgmma_desc_k_sw128(aW1 + p * 8192 + k * 32, 1024), (p > 0 || k > 0) ? 1u : 0u);
+                            wgmma_f16_rs<32>(acc1, xa[4 * p + k], wgmma_desc_k_sw128(aW1 + p * 8192 + k * 32, 1024),
+                                             (p > 0 || k > 0) ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<0>();
                     wgmma_fence_regs(acc1);

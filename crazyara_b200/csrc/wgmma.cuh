@@ -53,6 +53,24 @@ __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t da, uin
         : "l"(da), "l"(db), "r"(accumulate));
 }
 
+// The same with A from registers (the RS form): a[4] is the fp16 m16k16 fragment of mma.sync that warp w of the
+// warpgroup holds for rows 16 w .. 16 w + 15.  With lane l, r = 16 w + l / 4, c = 2 (l % 4): a[0] = A[r][c, c + 1],
+// a[1] = A[r + 8][c, c + 1], a[2] = A[r][c + 8, c + 9], a[3] = A[r + 8][c + 8, c + 9], the lower column in the low half
+// (what ldmatrix.x4 returns for the four 8 x 8 tiles rows 0-7 | 8-15 of columns 0-7, then of columns 8-15).  B by
+// descriptor as above.
+template <int N>
+__device__ __forceinline__ void wgmma_f16_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : ARA_D8(0), ARA_D8(8)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+
 #undef ARA_D8
 
 }  // namespace ara

@@ -36,7 +36,7 @@ if any(out[i] for i in range(16)):
     names = ["X load + cluster barrier", "wait SE image", "squeeze-excitation (split)", "wait W1 image",
              "MMA1 (wgmma m64n32)", "epilogue 1 (relu + b1 -> H1)", "wait own H2 buffer free",
              "depthwise -> H2 + copy", "wait partner's H2", "wait W2 half", "MMA2 (wgmma m64n64)",
-             "wait partner's X free", "block epilogue + X panel copy", "wait partner's X"]
+             "wait partner's X free", "block epilogue + X panel copy", "wait partner's X", "X -> registers (ldmatrix)"]
 else:
     shape, base = "one / two boards per CTA", 16
     names = ["X load", "squeeze-excitation", "wait W1 image", "MMA1 (wgmma m64n64)", "epilogue 1 (relu + b1 -> H1)",
