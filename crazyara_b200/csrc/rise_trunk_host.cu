@@ -159,11 +159,18 @@ int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const
 
 namespace {
 
+// the squeeze-excitation arguments of ara_debug_trunk_se; all null: no block has one
+struct DebugSe {
+    const int *se_type = nullptr, *gate = nullptr, *flags = nullptr, *se_bias = nullptr;
+    const float *se_w1t = nullptr, *se_w2t = nullptr, *se_b = nullptr, *se_b1 = nullptr;
+};
+
 int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1, const float* b1,
-                    const float* wd, const float* bd, const float* w2, const float* b2, __half* out_h) {
+                    const float* wd, const float* bd, const float* w2, const float* b2, const DebugSe& se, __half* out_h, int* mx) {
     if (n < 1 || n_blocks < 1 || n_blocks > kTrunkMaxBlocks) return set_error("ara_debug_trunk: %d boards, %d blocks", n, n_blocks);
     const size_t x_count = static_cast<size_t>(n) * 64 * 256;
     std::vector<TrunkBlockHost> blocks(n_blocks);
+    const float *se_w1t = se.se_w1t, *se_w2t = se.se_w2t, *se_b = se.se_b, *se_b1 = se.se_b1;
     for (int i = 0; i < n_blocks; ++i) {
         TrunkBlockHost& h = blocks[i];
         const int c = c_op[i], kk = ksize[i] * ksize[i];
@@ -177,6 +184,28 @@ int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, con
         h.w2.assign(w2, w2 + static_cast<size_t>(256) * c);
         h.b2.assign(b2 + 256 * i, b2 + 256 * (i + 1));
         w1 += static_cast<size_t>(c) * 256, b1 += c, wd += static_cast<size_t>(c) * kk, bd += c, w2 += static_cast<size_t>(256) * c;
+        if (se.se_type == nullptr) continue;
+        // only what a weight blob can describe (net.cu): the kernels take a ca_se block's two biases together or not at all
+        const int type = se.se_type[i], bias = se.se_bias[i];
+        if (type < 0 || type > 2) return set_error("ara_debug_trunk_se: block %d has squeeze-excitation type %d", i, type);
+        if (se.gate[i] < kTrunkGateHard6 || se.gate[i] > kTrunkGateSigmoid) return set_error("ara_debug_trunk_se: block %d has gate %d", i, se.gate[i]);
+        if ((se.flags[i] & ~kTrunkShortcutPreSe) != 0) return set_error("ara_debug_trunk_se: block %d has flags %d", i, se.flags[i]);
+        const bool bias_ok = type == 0 ? bias == 0 : type == 2 ? bias == 1 : bias == 0 || bias == 3;
+        if (!bias_ok)
+            return set_error("ara_debug_trunk_se: block %d (squeeze-excitation type %d) has biases %d: eca_se takes se_b, ca_se "
+                             "both se_b and se_b1 or neither, a block without squeeze-excitation none", i, type, bias);
+        h.se_type = type;
+        h.gate = se.gate[i];
+        h.flags = se.flags[i];
+        if (type == 0) continue;
+        if (se_w1t == nullptr || (type == 1 && se_w2t == nullptr) || ((bias & 1) && se_b == nullptr) || ((bias & 2) && se_b1 == nullptr))
+            return set_error("ara_debug_trunk_se: block %d: a squeeze-excitation array is null", i);
+        const size_t n1 = type == 1 ? 256 * 128 : 256 * 256, n2 = type == 1 ? 128 * 256 : 0;
+        h.se_w1t.assign(se_w1t, se_w1t + n1);
+        h.se_w2t.assign(se_w2t, se_w2t + n2);
+        se_w1t += n1, se_w2t += n2;
+        if (bias & 1) h.se_b.assign(se_b, se_b + 256), se_b += 256;
+        if (bias & 2) h.se_b1.assign(se_b1, se_b1 + 128), se_b1 += 128;
     }
     DeviceBuffers mem;
     __half *d_x = nullptr, *d_out = nullptr;
@@ -184,6 +213,7 @@ int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, con
     ARA_CUDA_OK(cudaMemcpy(d_x, x_h, x_count * sizeof(__half), cudaMemcpyHostToDevice));
     RiseTrunk T;
     if (rise_trunk_init(&T, blocks, d_x, d_out)) return -1;
+    if (mx != nullptr) *mx = T.mx ? 1 : 0;
     if (rise_trunk_launch(&T, n, nullptr)) return -1;
     ARA_CUDA_OK(cudaStreamSynchronize(nullptr));
     ARA_CUDA_OK(cudaMemcpy(out_h, d_out, x_count * sizeof(__half), cudaMemcpyDeviceToHost));
@@ -199,6 +229,22 @@ int debug_trunk_run(const __half* x_h, int n, int n_blocks, const int* c_op, con
 // squeeze-excitation) one block after the other in the layouts of TrunkBlockHost; b2 [n_blocks][256].
 extern "C" int ara_debug_trunk(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1,
                                const float* b1, const float* wd, const float* bd, const float* w2, const float* b2, void* out_half) {
-    return ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2,
-                                static_cast<__half*>(out_half));
+    return ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2, {},
+                                static_cast<__half*>(out_half), nullptr);
+}
+
+// ara_debug_trunk with the squeeze-excitation and MXNet block fields of TrunkBlockHost: per block se_type, gate, flags
+// and se_bias (bit 0: se_b given, bit 1: se_b1 given); se_w1t, se_w2t, se_b and se_b1 concatenated over the blocks
+// that have them.  *mx_out (if not null): 1 when rise_trunk_init chose the kernels built for the MXNet semantics.
+extern "C" int ara_debug_trunk_se(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const int* se_type,
+                                  const int* gate, const int* flags, const int* se_bias, const float* w1, const float* b1,
+                                  const float* wd, const float* bd, const float* w2, const float* b2, const float* se_w1t,
+                                  const float* se_w2t, const float* se_b, const float* se_b1, void* out_half, int* mx_out) {
+    if (se_type == nullptr || gate == nullptr || flags == nullptr || se_bias == nullptr)
+        return ara::set_error("ara_debug_trunk_se: null per-block argument");
+    ara::DebugSe se;
+    se.se_type = se_type, se.gate = gate, se.flags = flags, se.se_bias = se_bias;
+    se.se_w1t = se_w1t, se.se_w2t = se_w2t, se.se_b = se_b, se.se_b1 = se_b1;
+    return ara::debug_trunk_run(static_cast<const __half*>(x_half), n, n_blocks, c_op, ksize, w1, b1, wd, bd, w2, b2, se,
+                                static_cast<__half*>(out_half), mx_out);
 }

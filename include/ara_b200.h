@@ -320,6 +320,17 @@ int ara_debug_choose_bn(int boards, int n_out);
  * w2 [256][c_op], b2 [256] (BN folded) */
 int ara_debug_trunk(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const float* w1,
                     const float* b1, const float* wd, const float* bd, const float* w2, const float* b2, void* out_half);
+/* ara_debug_trunk with squeeze-excitation and the MXNet block semantics.  Per block: se_type (0 none, 1 ca_se, 2 eca_se),
+ * gate (0 hard sigmoid x / 6 + 0.5, 1 hard sigmoid 0.2 x + 0.5, 2 logistic), flags (1: the shortcut is the block input
+ * before the squeeze-excitation) and se_bias (bit 0: se_b given, bit 1: se_b1 given).  Concatenated over the blocks
+ * that have them: se_w1t (ca_se [256][128], eca_se [256][256], transposed), se_w2t (ca_se [128][256]), se_b [256] (eca_se
+ * bias, ca_se fc2 bias), se_b1 [128] (ca_se fc1 bias).  eca_se takes se_b; ca_se both biases or neither; a gate out of
+ * range or other flags are refused.  A block with a flag, a gate other than 0 or se_b1 selects the kernels built for
+ * the MXNet semantics, and *mx_out (if not NULL) reports that choice (1) or the PyTorch one (0). */
+int ara_debug_trunk_se(const void* x_half, int n, int n_blocks, const int* c_op, const int* ksize, const int* se_type,
+                       const int* gate, const int* flags, const int* se_bias, const float* w1, const float* b1, const float* wd,
+                       const float* bd, const float* w2, const float* b2, const float* se_w1t, const float* se_w2t,
+                       const float* se_b, const float* se_b1, void* out_half, int* mx_out);
 /* the device build of the glibc powf / logf restatement the search uses for apply_temperature (util/blazeutil.h:78-88)
  * and the Dirichlet gamma sampler (:113-124): pow_out[i] = powf(x[i], y[i]), log_out[i] = logf(x[i]); host buffers,
  * either output may be NULL.  tests/test_glibc_flt32.py compares it with the host libm bit for bit. */
