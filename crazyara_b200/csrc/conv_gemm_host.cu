@@ -3,6 +3,8 @@
 
 #include <cstring>
 
+#include "ara_b200.h"
+
 namespace ara {
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -112,6 +114,17 @@ void conv_layer_set_precise(ConvLayer* L, const float* residual_f, int ldr, __ha
     L->args.split_cs = split_cs;
 }
 
+int conv_layer_build(ConvLayer* L, const __half* w, int w_rows, const float* bias, int n_out, int cin, int ksize, int relu,
+                     int precision, int boards_cap, int bn, const ConvIo& io) {
+    const int act_cin = precision == 0 ? (io.act_cin ? io.act_cin : cin) : 3 * ((cin + 63) / 64 * 64);
+    if (conv_layer_init(L, io.act, boards_cap, act_cin, w, w_rows, n_out, ksize, bias, relu, io.res_h, io.ldr, io.out_h, io.out_f,
+                        io.ldo, bn, io.act_pitch))
+        return -1;
+    if (precision == 1) conv_layer_set_precise(L, io.res_f, io.ldr, io.out_s, io.split_cs);
+    if (io.n_end) L->args.n_end = io.n_end;
+    return 0;
+}
+
 template <int BN>
 static int launch_bn(const ConvLayer* L, const ConvGemmArgs& a, dim3 grid, cudaStream_t stream) {
     ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN>, grid, dim3(kGemmThreads), ConvGemmCfg<BN>::kSmemBytes, stream, L->tm_a, L->tm_b, a));
@@ -133,16 +146,39 @@ int conv_layer_launch(const ConvLayer* L, int boards, cudaStream_t stream, const
 
 }  // namespace ara
 
-// Debug / unit-test entry: run one convolution layer on caller-provided device buffers.
-extern "C" int ara_debug_conv(const void* act_half, int boards_cap, int boards, int cin, const void* w_half, int w_rows,
-                              int n_out, int ksize, const float* bias, int relu, const void* residual, int ldr,
-                              void* out_half, float* out_f32, int ldo, int bn, void* stream) {
+// Debug / unit-test entry: one convolution layer on caller-provided device buffers, built and launched as a network's.
+extern "C" int ara_debug_conv(const ara_debug_conv_t* a, void* stream) {
+    if (a == nullptr) return ara::set_error("ara_debug_conv: null arguments");
+    // the argument block is read on the host: a device pointer in its place (e.g. a buffer handed over where the struct
+    // belongs) is refused here instead of being dereferenced
+    cudaPointerAttributes pa;
+    if (cudaPointerGetAttributes(&pa, a) != cudaSuccess) {
+        cudaGetLastError();
+        return ara::set_error("ara_debug_conv: the argument pointer is not a host address");
+    }
+    if (pa.type == cudaMemoryTypeDevice) return ara::set_error("ara_debug_conv: the arguments are in device memory, not on the host");
+    if (a->precision != ARA_PRECISION_FLOAT16 && a->precision != ARA_PRECISION_FLOAT32)
+        return ara::set_error("ara_debug_conv: precision %d (0 = float16, 1 = float32)", a->precision);
+    if (a->boards < 1 || a->boards > a->boards_cap) return ara::set_error("ara_debug_conv: %d boards of %d", a->boards, a->boards_cap);
+    ara::ConvIo io;
+    io.act = (const __half*)a->act;
+    io.act_cin = a->act_cin;
+    io.act_pitch = a->act_pitch;
+    io.res_h = (const __half*)a->res_h;
+    io.res_f = a->res_f;
+    io.ldr = a->ldr;
+    io.out_h = (__half*)a->out_h;
+    io.out_f = a->out_f;
+    io.out_s = (__half*)a->out_s;
+    io.ldo = a->ldo;
+    io.n_end = a->n_end;
+    io.split_cs = a->split_cs;
+    const int bn = a->bn ? a->bn : ara::conv_layer_choose_bn(a->boards, a->n_out);
     ara::ConvLayer L;
-    if (bn == 0) bn = ara::conv_layer_choose_bn(boards, n_out);
-    int rc = ara::conv_layer_init(&L, (const __half*)act_half, boards_cap, cin, (const __half*)w_half, w_rows, n_out,
-                                  ksize, bias, relu, (const __half*)residual, ldr, (__half*)out_half, out_f32, ldo, bn);
+    int rc = ara::conv_layer_build(&L, (const __half*)a->w, a->w_rows, a->bias, a->n_out, a->cin, a->ksize, a->relu, a->precision,
+                                   a->boards_cap, bn, io);
     if (rc != 0) return rc;
-    rc = ara::conv_layer_launch(&L, boards, (cudaStream_t)stream);
+    rc = ara::conv_layer_launch(&L, a->boards, (cudaStream_t)stream, a->boards_dev);
     if (rc != 0) return rc;
     cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
     if (e != cudaSuccess) return ara::set_error("ara_debug_conv: %s", cudaGetErrorString(e));

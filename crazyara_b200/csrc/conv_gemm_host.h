@@ -35,4 +35,26 @@ void conv_layer_set_precise(ConvLayer* L, const float* residual_f, int ldr, __ha
 // boards_dev (optional): device-side count of the boards in use, <= boards (see ConvGemmArgs::boards_dev)
 int conv_layer_launch(const ConvLayer* L, int boards, cudaStream_t stream, const int* boards_dev = nullptr);
 
+// Where one conv_gemm layer reads and writes.  act: the activations, rows act_pitch channels apart (0: act_cin); float16
+// reads channels 0 .. act_cin (0: the layer's cin), float32 the split [.., 3 * ceil64(cin)].  The epilogue adds the fp16
+// or fp32 residual (rows ldr apart) and writes columns 0 .. n_end (0: ldo) of the fp16, fp32 and / or split outputs
+// (rows ldo apart, split parts split_cs wide).
+struct ConvIo {
+    const __half* act = nullptr;
+    int act_cin = 0, act_pitch = 0;
+    const __half* res_h = nullptr;
+    const float* res_f = nullptr;
+    int ldr = 0;
+    __half* out_h = nullptr;
+    float* out_f = nullptr;
+    __half* out_s = nullptr;
+    int ldo = 0, n_end = 0, split_cs = 0;
+};
+
+// One layer of a network in `precision` (0 float16, 1 float32 = split operands): the weight image w [w_rows][taps *
+// parts * ceil64(cin)] (parts 1, or 3 for [hi | lo | hi], Net::upload_conv_w), bias [w_rows] or null, the activations and
+// outputs of io, N tile bn.  Net::build_conv and ara_debug_conv both build their layers here.
+int conv_layer_build(ConvLayer* L, const __half* w, int w_rows, const float* bias, int n_out, int cin, int ksize, int relu,
+                     int precision, int boards_cap, int bn, const ConvIo& io);
+
 }  // namespace ara

@@ -74,13 +74,7 @@ int Net::build_conv(ConvLayer* L, const std::vector<float>& w, const std::vector
     float* db = nullptr;
     if (upload_conv_w(w.data(), n_out, cin, ksize, precision == 0 ? 1 : 3, &dw)) return -1;
     if (!bias.empty() && upload_f32(bias.data(), bias.size(), rows, &db)) return -1;
-    const int act_cin = precision == 0 ? (io.act_cin ? io.act_cin : cin) : 3 * round_up(cin, 64);
-    if (conv_layer_init(L, io.act, batch_cap, act_cin, dw, rows, n_out, ksize, db, relu, io.res_h, io.ldr, io.out_h, io.out_f,
-                        io.ldo, conv_layer_choose_bn(batch, n_out), io.act_pitch))
-        return -1;
-    if (precision == 1) conv_layer_set_precise(L, io.res_f, io.ldr, io.out_s, io.split_cs);
-    if (io.n_end) L->args.n_end = io.n_end;
-    return 0;
+    return conv_layer_build(L, dw, rows, db, n_out, cin, ksize, relu, precision, batch_cap, conv_layer_choose_bn(batch, n_out), io);
 }
 
 template <typename... KArgs, typename... Args>

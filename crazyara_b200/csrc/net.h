@@ -50,22 +50,6 @@ struct PreciseBlock {
     ConvLayer conv1, conv2;
 };
 
-// Where one conv_gemm layer (conv_gemm.cuh) reads and writes.  act: the activations, rows act_pitch channels apart (0:
-// act_cin); float16 reads channels 0 .. act_cin (0: the layer's cin), float32 the split [.., 3 * ceil64(cin)].  The
-// epilogue adds the fp16 or fp32 residual (rows ldr apart) and writes columns 0 .. n_end (0: ldo) of the fp16, fp32 and /
-// or split outputs (rows ldo apart, split parts split_cs wide).
-struct ConvIo {
-    const __half* act = nullptr;
-    int act_cin = 0, act_pitch = 0;
-    const __half* res_h = nullptr;
-    const float* res_f = nullptr;
-    int ldr = 0;
-    __half* out_h = nullptr;
-    float* out_f = nullptr;
-    __half* out_s = nullptr;
-    int ldo = 0, n_end = 0, split_cs = 0;
-};
-
 // the tensors of a weight blob, host side, in blob order (weights.py)
 struct HostBlock {
     std::vector<float> se_a, se_b;  // ca_se: fc1 [128][256], fc2 [256][128]; eca_se: centre tap [256][256], bias [256]

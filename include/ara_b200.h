@@ -310,10 +310,45 @@ long long ara_search_launch_count(ara_search_t s); /* search kernels launched so
  * room left for another search on top of the dead siblings (instead of giving the tree up). */
 long long ara_search_compaction_count(ara_search_t s);
 
-/* ---- debug / unit-test entries (one wgmma convolution layer on caller-provided device buffers) */
-int ara_debug_conv(const void* act_half, int boards_cap, int boards, int cin, const void* w_half, int w_rows, int n_out,
-                   int ksize, const float* bias, int relu, const void* residual, int ldr, void* out_half,
-                   float* out_f32, int ldo, int bn, void* stream);
+/* ---- debug / unit-test entries
+ * ara_debug_conv: one wgmma convolution layer on caller-provided device buffers, built and launched as the network builds
+ * and launches each of its convolutions (Net::build_conv, Net::launch_conv); synchronous on `stream`.
+ *   act        fp16 activations [boards_cap][64][act_pitch]; float16 reads channels 0 .. act_cin (0: cin), float32 the
+ *              split [hi | hi | lo] of 3 * ceil64(cin) channels (act_cin ignored); act_pitch 0: as many as it reads
+ *   w          fp16 weight image [w_rows][ksize^2 * parts * ceil64(cin)], per tap w (parts 1) or, float32, hi | lo | hi
+ *   bias       fp32 [w_rows] zero padded, or NULL
+ *   res_h      fp16 residual (float16) / res_f fp32 residual (float32), rows ldr apart, added after the ReLU, or NULL
+ *   out_h, out_f, out_s   fp16, fp32 (rows ldo apart) and, float32 only, split outputs [rows][3 * split_cs], or NULL;
+ *              columns 0 .. n_end (0: ldo) are written, rows 0 .. 64 * boards
+ *   boards_dev device-side count of the boards in use (<= boards): M tiles beyond it leave at once; or NULL
+ *   bn         the N tile, 64, 128 or 256; 0: the one ara_debug_choose_bn(boards, n_out) gives */
+typedef struct ara_debug_conv_s {
+    const void* act;
+    const void* w;
+    const float* bias;
+    const void* res_h;
+    const float* res_f;
+    void* out_h;
+    float* out_f;
+    void* out_s;
+    const int* boards_dev;
+    int precision;
+    int boards_cap;
+    int boards;
+    int cin;
+    int n_out;
+    int ksize;
+    int relu;
+    int w_rows;
+    int act_cin;
+    int act_pitch;
+    int ldr;
+    int ldo;
+    int n_end;
+    int split_cs;
+    int bn;
+} ara_debug_conv_t;
+int ara_debug_conv(const ara_debug_conv_t* args, void* stream);
 int ara_debug_choose_bn(int boards, int n_out);
 /* the residual tower kernel alone on host buffers, on the shape ARA_TRUNK_ROWS selects: x_half, out_half [n][64][256]
  * fp16; per block (no squeeze-excitation), one after the other: w1 [c_op][256], b1 [c_op], wd [c_op][k*k], bd [c_op],

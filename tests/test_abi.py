@@ -93,9 +93,10 @@ def test_ctypes_structs_have_the_header_layout(tmp_path):
     mirror must sit at the offset and have the size the C compiler gives the field of the same name."""
     import subprocess
     from crazyara_b200 import engine
+    from tests.test_conv_gemm_gpu import DebugConv
     mirrors = {"ara_search_settings_t": engine.SearchSettings, "ara_search_result_t": engine.SearchResult,
                "ara_node_view_t": engine.NodeView, "ara_time_control_t": engine.TimeControl,
-               "ara_time_report_t": engine.TimeReport}
+               "ara_time_report_t": engine.TimeReport, "ara_debug_conv_t": DebugConv}
     fields = {t: _header_struct_fields(t) for t in mirrors}
     lines = ['#include <stddef.h>', '#include <stdio.h>', '#include "ara_b200.h"', 'int main(void) {']
     for t, names in fields.items():
