@@ -131,11 +131,18 @@ static int launch_bn(const ConvLayer* L, const ConvGemmArgs& a, dim3 grid, cudaS
     return 0;
 }
 
+static dim3 conv_layer_grid(const ConvLayer* L, int boards) { return dim3((boards + 1) / 2, (L->n_out + L->bn - 1) / L->bn, 1); }
+
+int conv_layer_ctas(const ConvLayer* L, int boards) {
+    const dim3 g = conv_layer_grid(L, boards);
+    return static_cast<int>(g.x * g.y);
+}
+
 int conv_layer_launch(const ConvLayer* L, int boards, cudaStream_t stream, const int* boards_dev) {
     ConvGemmArgs a = L->args;
     a.M = boards * 64;
     a.boards_dev = boards_dev;
-    dim3 grid((boards + 1) / 2, (L->n_out + L->bn - 1) / L->bn, 1);
+    const dim3 grid = conv_layer_grid(L, boards);
     switch (L->bn) {
         case 64: return launch_bn<64>(L, a, grid, stream);
         case 128: return launch_bn<128>(L, a, grid, stream);

@@ -34,6 +34,8 @@ void conv_layer_set_precise(ConvLayer* L, const float* residual_f, int ldr, __ha
 
 // boards_dev (optional): device-side count of the boards in use, <= boards (see ConvGemmArgs::boards_dev)
 int conv_layer_launch(const ConvLayer* L, int boards, cudaStream_t stream, const int* boards_dev = nullptr);
+// the CTAs of that launch
+int conv_layer_ctas(const ConvLayer* L, int boards);
 
 // Where one conv_gemm layer reads and writes.  act: the activations, rows act_pitch channels apart (0: act_cin); float16
 // reads channels 0 .. act_cin (0: the layer's cin), float32 the split [.., 3 * ceil64(cin)].  The epilogue adds the fp16

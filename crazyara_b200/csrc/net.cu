@@ -602,8 +602,13 @@ int Net::enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cud
     return 0;
 }
 
+bool Net::stem_beside_tower(int n) const {
+    return precision == 0 && d_x0_alt != nullptr &&
+           rise_trunk_ctas(trunks_[0].get(), n) + conv_layer_ctas(&stem_conv2, n) <= trunks_[0]->sm_count;
+}
+
 int Net::stem_device(int n, cudaStream_t s, const int* cnt, int io) {
-    if (!stem_splittable() || io < 0 || io > 1) return set_error("stem_device: needs Precision float16 and two input / output sets");
+    if (!stem_beside_tower(n) || io < 0 || io > 1) return set_error("stem_device: needs Precision float16, two input / output sets and room beside the tower");
     return launch_conv(io ? stem_conv2 : stem_conv, n, s, cnt);
 }
 
@@ -640,7 +645,7 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
 }
 
 int Net::forward_device(int n, cudaStream_t s, const int* cnt, int io, bool stem_done) {
-    if (stem_done && !stem_splittable()) return set_error("forward: stem_done needs Precision float16 and two input / output sets");
+    if (stem_done && !stem_beside_tower(n)) return set_error("forward: stem_done needs Precision float16, two input / output sets and room beside the tower");
     if (n < 1 || n > batch) return set_error("forward: n=%d outside [1,%d]", n, batch);
     if (io != 0 && (io != 1 || io_in_h[1] == nullptr)) return set_error("forward: input/output set %d not enabled", io);
     // two input / output sets = a search with Threads = 2: this forward runs on the network stream beside the other

@@ -85,11 +85,14 @@ class Net {
     // batches in flight -- one set is being written / read by the tree kernels while the other is at the network
     // stem_done: the stem convolution of this batch has already run (stem_device, on the caller's own stream)
     int forward_device(int n, cudaStream_t stream, const int* boards_dev = nullptr, int io = 0, bool stem_done = false);
-    // The stem convolution alone, into the stem-output buffer of input / output set `io` (Precision float16 with two
-    // sets enabled): a search with two logical threads runs it on its tree stream right behind the plane encoding, which
-    // takes it off the network stream's critical path.
+    // The stem convolution alone, into the stem-output buffer of input / output set `io` (stem_beside_tower(n)): a
+    // search with two logical threads runs it on its tree stream right behind the plane encoding, which takes it off the
+    // network stream's critical path.
     int stem_device(int n, cudaStream_t stream, const int* boards_dev, int io);
-    bool stem_splittable() const { return precision == 0 && d_x0_alt != nullptr; }
+    // Precision float16 with two sets enabled, and the stem of n boards fits on the SMs beside the tower of n boards.
+    // Where the tower fills the SMs (64 boards on 132 SMs) a stem on the tree stream would wait for the other set's
+    // tower and hold up this set's forward: then the forward starts at the stem.
+    bool stem_beside_tower(int n) const;
     __half* d_x0_alt = nullptr;  // stem output of set 1 (set 0: d_x[0])
     int enable_second_io();
     int forward_from_f32_device(int n, cudaStream_t stream);  // converts d_in_f32 -> in_h first

@@ -244,23 +244,30 @@ ARA_HD void encode_planes_nchw_f32(const Board& b, int mode, int version, bool n
     sink.flush();
 }
 
+// where the lanes of one warp trade the channel descriptors of a board (encode_planes_nhwc_f16): shared memory of the
+// calling kernel
+struct PlaneExchange {
+    uint64_t mask[96];
+    uint16_t val[96];
+};
+
 #if defined(__CUDACC__)
-// [64, cpad] fp16 rows (cpad = 64 or 128); channels >= C are written as zero.  Device only, warp-collective.
-__device__ __forceinline__ void encode_planes_nhwc_f16(const Board& b, int mode, int version, __half* out, int cpad) {
-    // (callers run at most four warps per thread block: encode_planes_f16_kernel, expand_kernel)
-    __shared__ uint64_t s_mask[4][96];
-    __shared__ uint16_t s_val[4][96];
+// [64, cpad] fp16 rows (cpad = 64 or 128); channels >= C are written as zero.  Device only, warp-collective; `x` is the
+// warp's own exchange in shared memory.
+__device__ __forceinline__ void encode_planes_nhwc_f16(const Board& b, int mode, int version, __half* out, int cpad, PlaneExchange& x) {
+    uint64_t* s_mask = x.mask;
+    uint16_t* s_val = x.val;
     const PlaneCtx p = make_plane_ctx(b, mode, true);
     LaneCaptureSink sink;
     sink.lane = threadIdx.x & 31;
     for_each_plane(p, version, sink);
-    const int lane = sink.lane, w = (threadIdx.x >> 5) & 3;
+    const int lane = sink.lane;
     // every lane has computed the descriptors (square mask, value) of three channels; a row of the output is written in
     // 16-byte pieces of eight channels, so the descriptors change hands through shared memory once per board ...
-    s_mask[w][lane] = sink.m0, s_mask[w][lane + 32] = sink.m1, s_mask[w][lane + 64] = sink.m2;
-    s_val[w][lane] = __half_as_ushort(__float2half_rn(sink.v0));
-    s_val[w][lane + 32] = __half_as_ushort(__float2half_rn(sink.v1));
-    s_val[w][lane + 64] = __half_as_ushort(__float2half_rn(sink.v2));
+    s_mask[lane] = sink.m0, s_mask[lane + 32] = sink.m1, s_mask[lane + 64] = sink.m2;
+    s_val[lane] = __half_as_ushort(__float2half_rn(sink.v0));
+    s_val[lane + 32] = __half_as_ushort(__float2half_rn(sink.v1));
+    s_val[lane + 64] = __half_as_ushort(__float2half_rn(sink.v2));
     __syncwarp();
     const int chunks = cpad >> 3;                                // pieces per row: 8 (cpad 64) or 16 (cpad 128)
     const int j = lane % chunks, s0 = lane / chunks, step = 32 / chunks;
@@ -269,8 +276,8 @@ __device__ __forceinline__ void encode_planes_nhwc_f16(const Board& b, int mode,
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int ch = 8 * j + i;
-        m[i] = ch < 96 ? s_mask[w][ch] : 0ull;
-        v[i] = ch < 96 ? s_val[w][ch] : 0u;
+        m[i] = ch < 96 ? s_mask[ch] : 0ull;
+        v[i] = ch < 96 ? s_val[ch] : 0u;
     }
     // ... and every store instruction of the warp writes 512 contiguous bytes (4 or 2 whole rows)
     for (int sq = s0; sq < 64; sq += step) {

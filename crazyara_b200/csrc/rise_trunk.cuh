@@ -402,7 +402,8 @@ struct RtPairCfg {
     static constexpr int kOffH1 = kOffH2 + kH2Bufs * 8192;    // [8 groups][64 squares][16 B]
     static constexpr int kOffSe = kOffH1 + 8192;              // pool[256] | hid[128] | scale[256] f32
     static constexpr int kOffBar = kOffSe + 2560;
-    static constexpr int kSmemBytes = kOffBar + 256 + 1024 /*align slack*/;
+    static constexpr int kSmemBytes = kTrunkPairSmemBytes;
+    static_assert(kOffBar + 256 + 1024 /*align slack*/ == kSmemBytes, "kTrunkPairSmemBytes must be the pair kernel's layout");
     static_assert(kSeUnits <= kW2Ring, "a block's SE image must fit the W2 ring");
     static_assert(kSmemBytes <= 232448, "pair trunk kernel shared memory exceeds the sm_90 limit of 227 KB per block");
 };

@@ -18,6 +18,9 @@ constexpr int kTrunkW2Image = 32768;
 //   ca_se:  fc1 columns 64 r .. 64 r + 63 as [256 k][64]  |  fc2 columns 128 r .. 128 r + 127 as [128 j][128]
 //   eca_se: columns 128 r .. 128 r + 127 as [256 k][128]
 constexpr int kTrunkSeImage = 65536;
+// Shared memory of one rise_trunk_pair_kernel CTA (RtPairCfg, rise_trunk.cuh).  In a two-thread search the tree kernels
+// of one logical thread run on what the other thread's tower leaves of the SMs: search.cu checks their layouts against it.
+constexpr int kTrunkPairSmemBytes = 216832;
 
 // the residual adds the block input as it was before the squeeze-excitation scaled it (MXNet RISE symbols)
 constexpr int kTrunkShortcutPreSe = 1;

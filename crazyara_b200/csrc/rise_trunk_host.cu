@@ -135,16 +135,25 @@ int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, con
     return 0;
 }
 
+// one board per CTA pair while every pair is resident at once, else one board per CTA while that fits one wave, else
+// two boards per CTA sharing a weight stream.  ARA_TRUNK_ROWS (trunk rows per CTA) forces a shape: 32 = the pair
+// (half of a board's channels per CTA), 64 = one board per CTA, any other value = two boards per CTA.
+static int trunk_rows(const RiseTrunk* T, int boards) {
+    const char* force = getenv("ARA_TRUNK_ROWS");
+    return force ? atoi(force) : boards <= T->pair_clusters ? 32 : boards <= T->sm_count ? 64 : 128;
+}
+
+int rise_trunk_ctas(const RiseTrunk* T, int boards) {
+    const int rows = trunk_rows(T, boards);
+    return rows == 32 ? 2 * boards : rows == 64 ? boards : (boards + 1) / 2;
+}
+
 int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const int* boards_dev, const __half* x_in) {
     TrunkArgs a = T->args;
     if (x_in != nullptr) a.x_in = x_in;
     a.M = boards * 64;
     a.boards_dev = boards_dev;
-    // one board per CTA pair while every pair is resident at once, else one board per CTA while that fits one wave, else
-    // two boards per CTA sharing a weight stream.  ARA_TRUNK_ROWS (trunk rows per CTA) forces a shape: 32 = the pair
-    // (half of a board's channels per CTA), 64 = one board per CTA, any other value = two boards per CTA.
-    const char* force = getenv("ARA_TRUNK_ROWS");
-    const int rows = force ? atoi(force) : boards <= T->pair_clusters ? 32 : boards <= T->sm_count ? 64 : 128;
+    const int rows = trunk_rows(T, boards);
     if (rows == 32)
         ARA_CUDA_OK(launch_pdl_cluster(T->mx ? rise_trunk_pair_kernel<true> : rise_trunk_pair_kernel<false>, dim3(2 * boards),
                                        dim3(RtPairCfg::kThreads), RtPairCfg::kSmemBytes, stream, 2u, a));

@@ -39,5 +39,7 @@ struct RiseTrunk {
 int rise_trunk_init(RiseTrunk* T, const std::vector<TrunkBlockHost>& blocks, const __half* x_in, __half* out);
 // x_in (optional): another stem-output buffer than the one given to rise_trunk_init (a second input / output set)
 int rise_trunk_launch(const RiseTrunk* T, int boards, cudaStream_t stream, const int* boards_dev = nullptr, const __half* x_in = nullptr);
+// the CTAs of that launch
+int rise_trunk_ctas(const RiseTrunk* T, int boards);
 
 }  // namespace ara

@@ -28,12 +28,13 @@ encode_planes_f32_kernel(const Board* boards, int n, int mode, int version, int 
 __global__ void __launch_bounds__(32 * kWarpsPerBlock)
 encode_planes_f16_kernel(const Board* boards, int n, int mode, int version, __half* out, int cpad) {
     __shared__ Board sb[kWarpsPerBlock];
+    __shared__ PlaneExchange xs[kWarpsPerBlock];
     const int w = threadIdx.x >> 5;
     const int i = blockIdx.x * kWarpsPerBlock + w;
     if (i >= n) return;
     if (ARA_LANE < 8) reinterpret_cast<uint4*>(&sb[w])[ARA_LANE] = reinterpret_cast<const uint4*>(&boards[i])[ARA_LANE];
     __syncwarp();
-    encode_planes_nhwc_f16(sb[w], mode, version, out + static_cast<size_t>(i) * 64 * cpad, cpad);
+    encode_planes_nhwc_f16(sb[w], mode, version, out + static_cast<size_t>(i) * 64 * cpad, cpad, xs[w]);
 }
 
 __global__ void __launch_bounds__(32 * kWarpsPerBlock)

@@ -23,6 +23,7 @@
 #include "abi_common.h"
 #include "ara_b200.h"
 #include "net.h"
+#include "rise_trunk_args.h"
 #include "search_dev.cuh"
 #include "search_wave.cuh"
 #include "time_manager.h"
@@ -33,21 +34,23 @@ struct DevWriterFactory {
     __half* base;
     int cpad;
     int split;  // Precision float32: rows of 3 * cpad halves, every channel as hi | hi | lo (conv_gemm.cuh)
+    PlaneExchange* xchg;  // the writing warp's, in shared memory
     struct Target {
         __half* out;
         int cpad;
         int split;
+        PlaneExchange* xchg;
         ARA_HD void encode(const Board& b, int mode, int version) const {
 #if defined(__CUDA_ARCH__)
             if (split)
                 encode_planes_nhwc_split(b, mode, version, out, cpad);
             else
-                encode_planes_nhwc_f16(b, mode, version, out, cpad);
+                encode_planes_nhwc_f16(b, mode, version, out, cpad, *xchg);
 #endif
         }
     };
     ARA_HD Target make(int slot) const {
-        return Target{base + static_cast<size_t>(slot) * 64 * cpad * (split ? 3 : 1), cpad, split};
+        return Target{base + static_cast<size_t>(slot) * 64 * cpad * (split ? 3 : 1), cpad, split, xchg};
     }
 };
 struct NullWriterFactory {  // fake backend: no planes needed
@@ -65,6 +68,15 @@ struct TreeLimits {
     int active;
     float q_value_weight, dirichlet_epsilon;
 };
+
+// With Threads = 2 one logical thread's tree kernels run while the other's tower holds all but a few SMs, one pair CTA
+// per SM.  A tree kernel's CTA that does not fit in what such an SM has left waits for the free SMs, and one sitting
+// there keeps the next tower from it.  Each CTA also takes kSmemReservedPerCta of the SM's shared memory.
+constexpr int kSmemPerSm = 233472, kSmemReservedPerCta = 1024;
+constexpr int kSmemBesideTower = kSmemPerSm - kTrunkPairSmemBytes - kSmemReservedPerCta;
+static_assert(sizeof(ExpandScratch) + kSmemReservedPerCta <= kSmemBesideTower, "expand_kernel no longer fits beside a tower CTA");
+static_assert(2 * (sizeof(UpdateScratch) + kSmemReservedPerCta) <= kSmemBesideTower, "two update_kernel CTAs no longer fit beside a tower CTA");
+static_assert(sizeof(WarpScratch) + kSmemReservedPerCta <= kSmemBesideTower, "select_kernel no longer fits beside a tower CTA");
 
 __global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const TreeLimits* limits) {
     __shared__ WarpScratch ws;
@@ -239,13 +251,13 @@ __global__ void __launch_bounds__(32) pack_kernel(TreeDev* trees, int n_trees, i
 // one warp per (tree, new leaf): move lists, edges, policy indices, input planes of all new leaves in parallel
 __global__ void __launch_bounds__(32) expand_kernel(const TreeDev* trees, SearchParams sp, int batch, __half* in_h, int cpad,
                                                     int split) {
-    __shared__ WarpScratch ws;
+    __shared__ ExpandScratch ws;
     const int tree = blockIdx.x / batch, b = blockIdx.x - tree * batch;
     const TreeDev t = trees[tree];
     if (b >= t.bs->n_new || t.st->error) return;
     const int nid = t.new_node[b];
     if (in_h != nullptr) {
-        const DevWriterFactory wf{in_h, cpad, split};
+        const DevWriterFactory wf{in_h, cpad, split, &ws.planes};
         const auto target = wf.make(t.slot_base + b);
         expand_pending(t, sp, ws, nid, &target);
     } else {
@@ -256,7 +268,7 @@ __global__ void __launch_bounds__(32) expand_kernel(const TreeDev* trees, Search
 // one warp per (tree, new leaf): priors of the legal moves out of the soft-maxed policy, temperature, sort, value
 __global__ void __launch_bounds__(32) scatter_kernel(const TreeDev* trees, SearchParams sp, int batch, const float* values,
                                                      const float* probs, int n_labels) {
-    __shared__ WarpScratch ws;
+    __shared__ ScatterScratch ws;
     const int tree = blockIdx.x / batch, b = blockIdx.x - tree * batch;
     const TreeDev t = trees[tree];
     if (b >= t.bs->n_new || t.st->error) return;
@@ -273,7 +285,7 @@ __global__ void __launch_bounds__(32) backup_kernel(const TreeDev* trees, Search
 
 // one warp per (tree, item): prepared-child slots of the new leaves and of the nodes expanded in the last mini-batch
 __global__ void __launch_bounds__(32) prepare_kernel(const TreeDev* trees, SearchParams sp, int items) {
-    __shared__ WarpScratch ws;
+    __shared__ PrepareScratch ws;
     const int tree = blockIdx.x / items, item = blockIdx.x - tree * items;
     const TreeDev t = trees[tree];
     prepare_item(t, sp, ws, item);
@@ -282,20 +294,20 @@ __global__ void __launch_bounds__(32) prepare_kernel(const TreeDev* trees, Searc
 // scatter and prepare in one warp (the iterations' path): warp `item` < B scatters leaf `item` and goes straight on to
 // prepare that leaf's first child; the other warps prepare the next children of the nodes expanded in the mini-batch,
 // which depend on neither.  Saves a dependent launch per iteration and takes the parents' work off the critical path.
-__device__ __forceinline__ void scatter_prepare_item(const TreeDev t, const SearchParams& sp, WarpScratch& ws, int item, int batch,
+__device__ __forceinline__ void scatter_prepare_item(const TreeDev t, const SearchParams& sp, UpdateScratch& ws, int item, int batch,
                                                      const float* values, const float* probs, int n_labels) {
     if (t.st->error) return;
     if (item < batch) {
         if (item >= t.bs->n_new) return;
-        scatter_pending(t, sp, ws, item, values, probs, n_labels);
+        scatter_pending(t, sp, ws.scatter, item, values, probs, n_labels);
         __syncwarp();
     }
-    prepare_item(t, sp, ws, item);
+    prepare_item(t, sp, ws.prepare, item);
 }
 
 __global__ void __launch_bounds__(32) scatter_prepare_kernel(const TreeDev* trees, SearchParams sp, int batch, int items,
                                                              const float* values, const float* probs, int n_labels) {
-    __shared__ WarpScratch ws;
+    __shared__ UpdateScratch ws;
     const int tree = blockIdx.x / items, item = blockIdx.x - tree * items;
     scatter_prepare_item(trees[tree], sp, ws, item, batch, values, probs, n_labels);
 }
@@ -306,7 +318,7 @@ __global__ void __launch_bounds__(32) scatter_prepare_kernel(const TreeDev* tree
 // join events either.
 __global__ void __launch_bounds__(32) update_kernel(const TreeDev* trees, SearchParams sp, int n_trees, int batch, int items,
                                                     const float* values, const float* probs, int n_labels) {
-    __shared__ WarpScratch ws;
+    __shared__ UpdateScratch ws;
     if (static_cast<int>(blockIdx.x) < n_trees) {
         backup_results(trees[blockIdx.x], sp, values);
         return;
@@ -806,9 +818,9 @@ int Search::enqueue_turn_tree_ops(const Slot& s, bool with_update) {
         return -1;
     // (one tree: its rows start at 0, the select kernel itself leaves the count)
     if (launch_select(s, n_trees == 1 ? s.d_count : nullptr) || pack_expand(s)) return -1;
-    // the stem convolution of the new batch right here, on the tree stream (which has the slack): the network stream's
-    // chain starts at the tower
-    if (net_ && net_->stem_splittable() && net_->stem_device(n_trees * B, stream_, s.d_count, s.io)) return -1;
+    // the stem convolution of the new batch right here, on the tree stream, when it fits beside the other thread's
+    // tower (Net::stem_beside_tower): the network stream's chain then starts at the tower
+    if (net_ && net_->stem_beside_tower(n_trees * B) && net_->stem_device(n_trees * B, stream_, s.d_count, s.io)) return -1;
     return 0;
 }
 
@@ -826,7 +838,7 @@ int Search::enqueue_turn(int k, bool with_update) {
         cudaEvent_t e = prof_event();  // (recorded on stream_; re-record it on the network stream)
         ARA_CUDA_OK(cudaEventRecord(e, net_stream_));
     }
-    if (evaluate(s, n_trees * sp.batch_size, net_stream_, s.d_count, net_ && net_->stem_splittable())) return -1;
+    if (evaluate(s, n_trees * sp.batch_size, net_stream_, s.d_count, net_ && net_->stem_beside_tower(n_trees * sp.batch_size))) return -1;
     if (profile) {
         cudaEvent_t e = prof_event();
         ARA_CUDA_OK(cudaEventRecord(e, net_stream_));

@@ -195,6 +195,36 @@ struct WarpScratch {  // per-warp shared memory (stack on the host)
     int bcast[4];
 };
 
+// The kernels that run while the other logical thread's forward occupies the SMs (Threads = 2) hold only what they use
+// in shared memory, so that a CTA fits beside a tower CTA (search.cu checks the sizes).  The functions they call are
+// templates over the layout; the select kernels and the host emulation pass a whole WarpScratch.
+struct ExpandScratch {  // expand_pending
+    Board child;
+    Move scratch[kMaxMoves];
+    Move legal[kMaxMoves];
+    MoveGenScratch mg;
+    PlaneExchange planes;
+    int bcast[4];
+};
+struct ScatterScratch {  // fill_nn_results
+    Move scratch[kMaxMoves];
+    Move legal[kMaxMoves];
+    float sort_p[kMaxMoves];
+    uint64_t path_key[kMaxDepth];  // the priors in policy-index order when a temperature applies (as in WarpScratch)
+};
+struct PrepareScratch {  // prepare_child
+    Board child;
+    Move scratch[kMaxMoves];
+    Move legal[kMaxMoves];
+    uint64_t path_key[kMaxDepth];
+    int16_t path_rep[kMaxDepth];
+    MoveGenScratch mg;
+};
+union UpdateScratch {  // one warp scatters a leaf, then prepares a child
+    ScatterScratch scatter;
+    PrepareScratch prepare;
+};
+
 // ------------------------------------------------------------------ small helpers
 ARA_HD int virtual_style_of(const SearchParams& sp, uint32_t visits) {  // node.h:87-95
     if (sp.virtual_style == VS_VIRTUAL_MIX) return visits > sp.virtual_mix_threshold ? VS_VIRTUAL_LOSS : VS_VIRTUAL_VISIT;
@@ -581,7 +611,8 @@ ARA_HD void revert_virtual_loss(const TreeDev& t, const SearchParams& sp, int ni
 
 // ------------------------------------------------------------------ repetition over (pre-root history + tree path)
 // ws.path_key/rep[0..depth) hold root..current; ws.child is the new position (depth plies below the root).
-ARA_HD int repetition_on_path(const TreeDev& t, const WarpScratch& ws, int depth) {
+template <class WS>
+ARA_HD int repetition_on_path(const TreeDev& t, const WS& ws, int depth) {
     const Board& b = ws.child;
     const int total = t.hist_len + depth;  // number of earlier positions
     int end = repetition_end(b);
@@ -623,7 +654,8 @@ ARA_HD int repetition_on_path(const TreeDev& t, const WarpScratch& ws, int depth
 //                     allocation + initialisation, policy indices, input planes.
 
 // Does the side to move have a legal move?  Warp-collective; *checked_out = side to move is in check.
-ARA_HD bool any_legal_move(const Board& b, WarpScratch& ws, bool* checked_out) {
+template <class WS>
+ARA_HD bool any_legal_move(const Board& b, WS& ws, bool* checked_out) {
     const int us = b.stm, them = us ^ 1;
     const uint64_t own = b.by_color[us], opp = b.by_color[them], occ = own | opp;
     const int ksq = king_square(b, us);
@@ -658,7 +690,8 @@ ARA_HD bool any_legal_move(const Board& b, WarpScratch& ws, bool* checked_out) {
 // Returns the new node id (uniform), or -1 on pool exhaustion.  *is_terminal receives the terminal verdict.
 // Repetition state and terminal verdict of ws.child (already moved), `depth` plies below the root with the keys of the
 // path in ws.path_key / path_rep.  Warp-collective; writes b.repetition.
-ARA_HD int leaf_verdict(const TreeDev& t, WarpScratch& ws, int depth) {
+template <class WS>
+ARA_HD int leaf_verdict(const TreeDev& t, WS& ws, int depth) {
     Board& b = ws.child;
     const int rep = repetition_on_path(t, ws, depth);
     if (ARA_LANE == 0) b.repetition = static_cast<int16_t>(rep);
@@ -738,7 +771,8 @@ ARA_HD int expand_node_seq(const TreeDev& t, const SearchParams& sp, WarpScratch
 // of nodes of any trees concurrently; runs after the backup of a mini-batch, when nothing else touches the tree.
 // Children are expanded in index order, so the slots hold the next kPrepSlots unexpanded children (slot = index mod
 // kPrepSlots): a node that is expanded twice within one mini-batch still finds its second child prepared.
-ARA_HD void prepare_child(const TreeDev& t, WarpScratch& ws, int X) {
+template <class WS>
+ARA_HD void prepare_child(const TreeDev& t, WS& ws, int X) {
     const NodeHdr& hx = t.hdr[X];
     if (!(hx.flags & NF_HAS_NN) || (hx.flags & NF_TERMINAL)) return;
     const int first = static_cast<int>(hx.no_visit_idx) - 1;
@@ -777,7 +811,8 @@ ARA_HD void prepare_child(const TreeDev& t, WarpScratch& ws, int X) {
     }
 }
 // item < B: the new leaves of the last mini-batch (their first child); item >= B: the nodes expanded in it
-ARA_HD void prepare_item(const TreeDev& t, const SearchParams& sp, WarpScratch& ws, int item) {
+template <class WS>
+ARA_HD void prepare_item(const TreeDev& t, const SearchParams& sp, WS& ws, int item) {
     const TreeState& st = *t.st;
     const BatchState& bs = *t.bs;
     if (st.error) return;
@@ -791,8 +826,8 @@ ARA_HD void prepare_item(const TreeDev& t, const SearchParams& sp, WarpScratch& 
 
 // Second half of the expansion of node `nid` (non-terminal, freshly created by expand_node_seq).  Warp-collective;
 // different nodes are processed by different warps concurrently, the edge pool is claimed with one atomic.
-template <class PlaneTarget>
-ARA_HD void expand_pending(const TreeDev& t, const SearchParams& sp, WarpScratch& ws, int nid, const PlaneTarget* target) {
+template <class WS, class PlaneTarget>
+ARA_HD void expand_pending(const TreeDev& t, const SearchParams& sp, WS& ws, int nid, const PlaneTarget* target) {
     copy_board(&ws.child, &t.board[nid]);
     const Board& b = ws.child;
     const int n_moves = gen_legal(b, ws.mg, ws.scratch, ws.legal);
@@ -848,7 +883,8 @@ ARA_HD void expand_pending(const TreeDev& t, const SearchParams& sp, WarpScratch
 
 // ------------------------------------------------------------------ scatter of network results into a new node
 // prob: this node's row of the soft-maxed policy; value: its value output.  Warp-collective.
-ARA_HD void fill_nn_results(const TreeDev& t, const SearchParams& sp, WarpScratch& ws, int nid, float value,
+template <class WS>
+ARA_HD void fill_nn_results(const TreeDev& t, const SearchParams& sp, WS& ws, int nid, float value,
                             const float* prob) {
     NodeHdr& h = t.hdr[nid];
     const int n = h.n_moves;
@@ -1353,7 +1389,8 @@ ARA_HD void create_mini_batch(const TreeDev& t_in, const SearchParams& sp, WarpS
 }
 
 // set_nn_results_to_child_nodes (searchthread.cpp:301-310) for new leaf `b` of the tree: one warp per leaf.
-ARA_HD void scatter_pending(const TreeDev& t, const SearchParams& sp, WarpScratch& ws, int b, const float* values,
+template <class WS>
+ARA_HD void scatter_pending(const TreeDev& t, const SearchParams& sp, WS& ws, int b, const float* values,
                             const float* probs, int n_labels) {
     const int slot = t.slot_base + b;
     fill_nn_results(t, sp, ws, t.new_node[b], values[slot], probs + static_cast<size_t>(slot) * n_labels);
