@@ -27,6 +27,9 @@ int conv_layer_init(ConvLayer* L, const __half* act, int boards_cap, int cin, co
 // activations [boards_cap, 8, 8, cin] fp16 as the 4-D map the A operand is fetched through (conv_layer_init builds the
 // same one): lets a layer be re-pointed at another input buffer
 int make_act_tensor_map(CUtensorMap* m, const __half* act, int boards_cap, int cin, int pitch = 0);
+// a K-major fp16 matrix [rows][k_total] as the 2-D map with box {64 k, box_rows} and the 128-byte swizzle the wgmma
+// operand descriptors read (the layers' weights; the fully-connected policy head's operands)
+int make_weight_tensor_map(CUtensorMap* m, const __half* w, int k_total, int rows, int box_rows);
 
 // Precision float32: fp32 residual [M, ldr] instead of the fp16 one, and / or the hi | hi | lo split output
 // [M, 3 * split_cs] (see conv_gemm.cuh); call after conv_layer_init.

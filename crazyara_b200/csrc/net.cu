@@ -122,10 +122,23 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     // ARAB2001: the networks of the reference's PyTorch definition.  ARAB2002 (the MXNet symbols) adds the header flags
     // stem_act and policy_bias, and per block flags and the squeeze-excitation gate.  ARAB2003 (AlphaVile) has the header
     // of ARAB2002 with trunks of 64..256 channels and a type word per block: 0 an ARAB2001 bottleneck block, 1 an NTB.
+    // ARAB2004 is one of the three with a fully-connected policy head (the trainer's select_policy_from_plane = False): the
+    // base format (1, 2 or 3) and the label count L, the base blob from its header on, then the head's tensors.
     char magic[8];
-    if (!rd.read(magic, 8) || (memcmp(magic, "ARAB2001", 8) != 0 && memcmp(magic, "ARAB2002", 8) != 0 && memcmp(magic, "ARAB2003", 8) != 0))
-        return set_error("ara_net_create: '%s' is not an ARAB2001 / ARAB2002 / ARAB2003 weight blob", blob_path);
-    const bool v2 = magic[7] == '2', v3 = magic[7] == '3';
+    if (!rd.read(magic, 8) || memcmp(magic, "ARAB200", 7) != 0 || magic[7] < '1' || magic[7] > '4')
+        return set_error("ara_net_create: '%s' is not an ARAB2001 / ARAB2002 / ARAB2003 / ARAB2004 weight blob", blob_path);
+    int base = magic[7] - '0';
+    hdr.n_classic = 0;
+    if (base == 4) {
+        int w[2];
+        if (!rd.read(w, sizeof(w))) return set_error("ara_net_create: truncated header");
+        base = w[0];
+        hdr.n_classic = w[1];
+        if (base < 1 || base > 3) return set_error("ara_net_create: ARAB2004 wraps base format %d (1, 2 or 3)", base);
+        if (hdr.n_classic != 1968 && hdr.n_classic != 2272 && hdr.n_classic != 2316)
+            return set_error("ara_net_create: %d policy labels (the classic label lists have 1968, 2272 or 2316)", hdr.n_classic);
+    }
+    const bool v2 = base == 2, v3 = base == 3;
     int h[10] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 0};
     if (!rd.read(h, (v2 || v3 ? 10 : 8) * sizeof(int))) return set_error("ara_net_create: truncated header");
     hdr.in_channels = h[0];
@@ -140,6 +153,8 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     hdr.policy_bias = h[9];
     if ((hdr.stem_act != 0 && hdr.stem_act != 1) || (hdr.policy_bias != 0 && hdr.policy_bias != 1))
         return set_error("ara_net_create: header flags stem_act %d policy_bias %d", hdr.stem_act, hdr.policy_bias);
+    if (hdr.n_classic && hdr.policy_bias)
+        return set_error("ara_net_create: ARAB2004 carries the policy convolution's bias with its head, not in the base header");
     if (v3 ? (hdr.channels % 32 != 0 || hdr.channels < 64 || hdr.channels > 256 || hdr.value_channels != 8 || hdr.value_fc < 1 ||
               hdr.value_fc > 256)
            : (hdr.channels != 256 || hdr.value_channels != 8 || hdr.value_fc != 256))
@@ -224,6 +239,10 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
     if (!rd.tensor(hw->pol_w1, static_cast<size_t>(C) * C * 9) || !rd.tensor(hw->pol_b1, C) ||
         !rd.tensor(hw->pol_w2, static_cast<size_t>(hdr.policy_channels) * C * 9) ||
         (hdr.policy_bias && !rd.tensor(hw->pol_b2, hdr.policy_channels)))
+        return -1;
+    if (hdr.n_classic && (!rd.tensor(hw->pol_b2, hdr.policy_channels) ||
+                          !rd.tensor(hw->fc_w, static_cast<size_t>(hdr.n_classic) * hdr.policy_channels * 64) ||
+                          !rd.tensor(hw->fc_b, hdr.n_classic)))
         return -1;
     char tail;
     if (fread(&tail, 1, 1, rd.f) != 0) return set_error("ara_net_create: trailing bytes in weight blob");
@@ -391,8 +410,13 @@ int Net::build_half(const HostWeights& hw) {
         if (bd.se_type == 1) t.se_b1 = hb.se_b1, t.se_b = hb.se_b2;
     }
     if (flush()) return -1;
-    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_x[1], .out_h = d_p1, .ldo = C}) ||
-        build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp}))
+    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_x[1], .out_h = d_p1, .ldo = C})) return -1;
+    if (!is_policy_map()) {  // relu(conv2) in fp16 for the fully-connected layer
+        if (mem_.dalloc(&d_pol_x, rows * ldp)) return -1;
+        return build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 1, {.act = d_p1, .out_h = d_pol_x, .ldo = ldp}) ||
+               build_policy_fc(hw);
+    }
+    if (build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp}))
         return -1;
     return 0;
 }
@@ -452,9 +476,17 @@ int Net::build_precise(const HostWeights& hw) {
                        {.act = d_h2s, .res_f = d_xf[in], .ldr = C, .out_f = d_xf[out], .out_s = d_xs[out], .ldo = C, .split_cs = C}))
             return -1;
     }
-    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_xs[hdr.n_blocks & 1], .out_s = d_p1, .ldo = C, .split_cs = C}) ||
-        build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp}))
+    if (build_conv(&pol_conv1, hw.pol_w1, hw.pol_b1, C, C, 3, 1, {.act = d_xs[hdr.n_blocks & 1], .out_s = d_p1, .ldo = C, .split_cs = C}))
         return -1;
+    if (!is_policy_map()) {  // relu(conv2) split for the fully-connected layer
+        const int cs = round_up(hdr.policy_channels, 64);
+        if (mem_.dalloc(&d_pol_x, rows * 3 * cs) ||
+            build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 1, {.act = d_p1, .out_s = d_pol_x, .ldo = cs, .split_cs = cs}) ||
+            build_policy_fc(hw))
+            return -1;
+    } else if (build_conv(&pol_conv2, hw.pol_w2, hw.pol_b2, hdr.policy_channels, C, 3, 0, {.act = d_p1, .out_f = d_logits, .ldo = ldp})) {
+        return -1;
+    }
     ARA_CUDA_OK(cudaFuncSetAttribute(value_head_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      value_head_smem<float>()));
     ARA_CUDA_OK(cudaFuncSetAttribute(nchw_f32_to_nhwc_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -480,6 +512,65 @@ int Net::build_ntb_precise(const BlockDesc& bd, const HostBlock& hb, int in, int
                    {.act = d_hs, .res_f = d_x2f, .ldr = 256, .out_f = d_xf[out], .out_s = d_xs[out], .ldo = 256, .split_cs = 256}))
         return -1;
     return 0;
+}
+
+// The fully-connected policy head: W_fc [L][P * 64] (the trainer's NCHW flatten c * 64 + sq) -> fp16 [lp][K] with the
+// columns in the order of a board's row of d_pol_x: float16 sq * ldp + c (K = 64 ldp); float32 per square hi | lo | hi
+// parts cs wide (K = 64 * 3 cs) against the activations' hi | hi | lo.  Padding rows and columns are zero.
+int Net::build_policy_fc(const HostWeights& hw) {
+    const int L = hdr.n_classic, P = hdr.policy_channels;
+    const int lp = round_up(L, 64);
+    const int parts = precision == 0 ? 1 : 3;
+    const int cs = precision == 0 ? ldp : round_up(P, 64);
+    const int K = 64 * parts * cs;
+    std::vector<__half> h(static_cast<size_t>(lp) * K, __float2half(0.0f));
+    for (int l = 0; l < L; ++l)
+        for (int c = 0; c < P; ++c)
+            for (int sq = 0; sq < 64; ++sq) {
+                const float v = hw.fc_w[(static_cast<size_t>(l) * P + c) * 64 + sq];
+                const __half hi = __float2half_rn(v);
+                __half* col = &h[static_cast<size_t>(l) * K + static_cast<size_t>(sq) * parts * cs];
+                col[c] = hi;
+                if (parts == 3) {
+                    col[cs + c] = __float2half_rn(v - __half2float(hi));
+                    col[2 * cs + c] = hi;
+                }
+            }
+    if (mem_.dalloc(&fc_w, h.size())) return -1;
+    ARA_CUDA_OK(cudaMemcpy(fc_w, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    if (upload_f32(hw.fc_b.data(), L, lp, &fc_b)) return -1;
+    // the split count depends on L and K only, never on the batch: the partial sums of a board are the same in any batch
+    const int m_tiles = lp / 64, num_kb = K / 64;
+    const int want = (kFcTargetCtas + m_tiles - 1) / m_tiles;
+    const int kb_per = (num_kb + want - 1) / want;
+    fc_splits_ = (num_kb + kb_per - 1) / kb_per;
+    fc_bn_ = batch <= 32 ? 32 : batch <= 64 ? 64 : 128;
+    if (mem_.dalloc(&d_fc_part, static_cast<size_t>(fc_splits_) * batch_cap * lp)) return -1;
+    fc_args = PolicyFcArgs{kb_per, num_kb, lp, batch_cap, d_fc_part, nullptr};
+    if (make_weight_tensor_map(&fc_tm_w, fc_w, K, lp, 64) || make_weight_tensor_map(&fc_tm_x, d_pol_x, K, batch_cap, fc_bn_)) return -1;
+    switch (fc_bn_) {
+        case 32: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<32>::kSmemBytes)); break;
+        case 64: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<64>::kSmemBytes)); break;
+        default: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<128>::kSmemBytes));
+    }
+    return 0;
+}
+
+// The policy head after the first convolution: the second convolution, then the softmax over its P * 64 logits, or the
+// fully-connected layer and the softmax over its L logits
+int Net::launch_policy_head(int n, cudaStream_t s, const int* cnt, int io) {
+    if (launch_conv(pol_conv2, n, s, cnt)) return -1;
+    if (is_policy_map())
+        return launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt);
+    PolicyFcArgs a = fc_args;
+    a.boards_dev = cnt;
+    const dim3 grid(a.lp / 64, fc_splits_, (n + fc_bn_ - 1) / fc_bn_);
+    const int rc = fc_bn_ == 32 ? launch(policy_fc_kernel<32>, grid, dim3(kFcThreads), PolicyFcCfg<32>::kSmemBytes, s, fc_tm_w, fc_tm_x, a)
+                 : fc_bn_ == 64 ? launch(policy_fc_kernel<64>, grid, dim3(kFcThreads), PolicyFcCfg<64>::kSmemBytes, s, fc_tm_w, fc_tm_x, a)
+                                : launch(policy_fc_kernel<128>, grid, dim3(kFcThreads), PolicyFcCfg<128>::kSmemBytes, s, fc_tm_w, fc_tm_x, a);
+    if (rc) return -1;
+    return launch(policy_fc_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_fc_part, fc_b, io_prob[io], n_labels(), a.lp,
+                  fc_splits_, batch_cap, cnt);
 }
 
 int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
@@ -518,8 +609,10 @@ int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
     io_in_h[0] = d_in_h, io_prob[0] = d_prob, io_value[0] = d_value, io_aux[0] = d_aux;
     ARA_CUDA_OK(cudaFuncSetAttribute(value_head_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      value_head_smem<__half>()));
-    ARA_CUDA_OK(cudaFuncSetAttribute(policy_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     n_labels() * 4));
+    if (is_policy_map())
+        ARA_CUDA_OK(cudaFuncSetAttribute(policy_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n_labels() * 4));
+    else
+        ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n_labels() * 4));
     ARA_CUDA_OK(cudaFuncSetAttribute(nchw_f32_to_nhwc_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      hdr.in_channels * 65 * 4));
     ARA_CUDA_OK(cudaDeviceSynchronize());
@@ -571,8 +664,7 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
     const float* xfinal = d_xf[hdr.n_blocks & 1];
     ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
     if (launch(value_head_kernel<float>, dim3(n), dim3(256), value_head_smem<float>(), s, xfinal, vw, io_value[io], io_aux[io], cnt) ||
-        launch_conv(pol_conv1, n, s, cnt) || launch_conv(pol_conv2, n, s, cnt) ||
-        launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt))
+        launch_conv(pol_conv1, n, s, cnt) || launch_policy_head(n, s, cnt, io))
         return -1;
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
@@ -636,9 +728,7 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
     value_head_kernel<__half><<<dim3(n), dim3(256), value_head_smem<__half>(), head_stream>>>(xfinal, vw, io_value[io], io_aux[io], cnt);
     ++launches;
     ARA_CUDA_OK(cudaEventRecord(ev_join, head_stream));
-    if (launch_conv(pol_conv1, n, s, cnt) || launch_conv(pol_conv2, n, s, cnt) ||
-        launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt))
-        return -1;
+    if (launch_conv(pol_conv1, n, s, cnt) || launch_policy_head(n, s, cnt, io)) return -1;
     ARA_CUDA_OK(cudaStreamWaitEvent(s, ev_join, 0));
     ARA_CUDA_OK(cudaGetLastError());
     return 0;
@@ -762,8 +852,9 @@ extern "C" int ara_net_shape(ara_net_t h, int* in_channels, int* n_labels, int* 
     if (in_channels) *in_channels = net->hdr.in_channels;
     if (n_labels) *n_labels = net->n_labels();
     if (n_aux) *n_aux = net->n_aux();
-    if (is_policy_map) *is_policy_map = 1;  // the policy head is a convolution onto P x 8 x 8 planes (builder_util.py:206-243,
-                                            // select_policy_from_plane): every blob this loader accepts is a policy map
+    // 1: the policy head is a convolution onto P x 8 x 8 planes; 0: a fully-connected layer onto the classic label list
+    // (builder_util.py:206-243, select_policy_from_plane)
+    if (is_policy_map) *is_policy_map = net->is_policy_map() ? 1 : 0;
     if (input_version) *input_version = net->hdr.input_version;
     if (batch_size) *batch_size = net->batch;
     return 0;

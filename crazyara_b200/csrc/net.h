@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "conv_gemm_host.h"
+#include "policy_fc.cuh"
 #include "rise_trunk_host.h"
 
 namespace ara {
@@ -36,6 +37,7 @@ struct NetHeader {
     int input_version;   // e.g. 10 = v1.0, 30 = v3.0
     int stem_act;        // 1: ReLU behind the stem convolution (ARAB2001: always)
     int policy_bias;     // 1: the last policy convolution has a bias (ARAB2001: never)
+    int n_classic;       // ARAB2004: the fully-connected policy head's label count L (0: a policy-map head)
 };
 
 // One NTB as GEMM launches (conv_gemm.cuh) around the attention kernel (ntb_attention.cuh), both precisions
@@ -63,7 +65,8 @@ struct HostWeights {
     std::vector<float> stem_w, stem_b;
     std::vector<HostBlock> blocks;
     std::vector<float> vh_wv, vh_bv, vh_a, vh_ab, vh_b, vh_bb;  // standard: fc1 / b1 / fc2 / b2; WDL: wdl w / b, plys w / b
-    std::vector<float> pol_w1, pol_b1, pol_w2, pol_b2;  // pol_b2: [policy_channels] when hdr.policy_bias
+    std::vector<float> pol_w1, pol_b1, pol_w2, pol_b2;  // pol_b2: [policy_channels] when hdr.policy_bias or hdr.n_classic
+    std::vector<float> fc_w, fc_b;                      // ARAB2004: [L][policy_channels * 64] (NCHW flatten), [L]
 };
 
 class Net {
@@ -105,7 +108,9 @@ class Net {
     int batch_cap = 0;  // even, >= 2
     int cin_pad = 0;
     int ldp = 0;  // padded policy channels (multiple of 32)
-    int n_labels() const { return hdr.policy_channels * 64; }
+    int n_labels() const { return hdr.n_classic ? hdr.n_classic : hdr.policy_channels * 64; }
+    // the policy is P x 64 planes (the convolution's output); false: the classic label list of a fully-connected head
+    bool is_policy_map() const { return hdr.n_classic == 0; }
     int n_aux() const { return hdr.wdl_mode ? 4 : 0; }
     int trunk_cycles(unsigned long long* out32);  // -DARA_TRUNK_PROF builds: per-role cycle counters of CTA 0 (first segment)
     cudaStream_t stream = nullptr;
@@ -182,6 +187,18 @@ class Net {
     float *vh_wv = nullptr, *vh_bv = nullptr, *vh_w1t = nullptr, *vh_b1 = nullptr, *vh_w2 = nullptr, *vh_b2 = nullptr;
     float *vh_wdl_w = nullptr, *vh_wdl_b = nullptr, *vh_plys_w = nullptr, *vh_plys_b = nullptr;
     ConvLayer pol_conv1, pol_conv2;
+    // fully-connected policy head (policy_fc.cuh): relu(conv2) as fp16 (float32: split) rows, one board per row, weights
+    // [lp][K] with their tensor maps, bias, split-K partial sums.  Like d_logits, shared by both input / output sets: their
+    // forwards follow each other on the network stream.
+    __half* d_pol_x = nullptr;
+    __half* fc_w = nullptr;
+    float* fc_b = nullptr;
+    float* d_fc_part = nullptr;
+    CUtensorMap fc_tm_w, fc_tm_x;
+    PolicyFcArgs fc_args{};
+    int fc_bn_ = 0, fc_splits_ = 0;
+    int build_policy_fc(const HostWeights& hw);
+    int launch_policy_head(int n, cudaStream_t s, const int* boards_dev, int io);
     struct Captured {
         cudaGraphExec_t exec;
         long long launches;  // the kernel launches the capture enqueued

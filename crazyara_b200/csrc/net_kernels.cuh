@@ -262,6 +262,43 @@ template <typename T>
 constexpr int value_head_smem() { return 64 * (256 + 16 / static_cast<int>(sizeof(T))) * static_cast<int>(sizeof(T)); }
 
 // ---------------------------------------------------------------------------------------------
+// The softmax of the policy heads over one board's L logits staged in shared memory (s_l, overwritten), mx their maximum
+// as this thread saw it; writes prob[0 .. L).  One CTA of 256 threads.
+__device__ __forceinline__ void block_softmax_256(float* s_l, int L, float mx, float* __restrict__ prob, float* s_red, float* s_bcast) {
+    const int t = threadIdx.x;
+    const int warp = t >> 5, lane = t & 31;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    if (lane == 0) s_red[warp] = mx;
+    __syncthreads();
+    if (t == 0) {
+        float m = s_red[0];
+        for (int i = 1; i < 8; ++i) m = fmaxf(m, s_red[i]);
+        *s_bcast = m;
+    }
+    __syncthreads();
+    mx = *s_bcast;
+    float sum = 0.0f;
+    for (int i = t; i < L; i += 256) {
+        const float e = expf(s_l[i] - mx);
+        s_l[i] = e;
+        sum += e;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+    __syncthreads();
+    if (lane == 0) s_red[warp] = sum;
+    __syncthreads();
+    if (t == 0) {
+        float s = 0.0f;
+        for (int i = 0; i < 8; ++i) s += s_red[i];
+        *s_bcast = 1.0f / s;
+    }
+    __syncthreads();
+    const float inv = *s_bcast;
+    for (int i = t; i < L; i += 256) prob[i] = s_l[i] * inv;
+}
+
 // Policy softmax over all P*64 logits of a board (illegal moves included, as the reference backend does).
 // logits: [boards*64, ldp] fp32 (NHWC, channel = policy plane), prob: [boards, P*64] fp32 with index ch*64+sq
 // (the reference's NCHW flatten, builder_util.py:229).  One CTA (256 threads) per board.
@@ -284,38 +321,29 @@ __global__ void __launch_bounds__(256) policy_softmax_kernel(const float* __rest
         s_l[ch * 64 + sq] = v;
         mx = fmaxf(mx, v);
     }
-    const int warp = t >> 5, lane = t & 31;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    if (lane == 0) s_red[warp] = mx;
-    __syncthreads();
-    if (t == 0) {
-        float m = s_red[0];
-        for (int i = 1; i < 8; ++i) m = fmaxf(m, s_red[i]);
-        s_bcast = m;
+    block_softmax_256(s_l, L, mx, prob + static_cast<size_t>(b) * L, s_red, &s_bcast);
+}
+
+// logits[b, l] = b_fc[l] + part[0][b][l] + part[1][b][l] + ... (split order), then the softmax over the L labels into
+// prob [boards, L].  One CTA (256 threads) per board.
+__global__ void __launch_bounds__(256) policy_fc_softmax_kernel(const float* __restrict__ part, const float* __restrict__ bias,
+                                                                  float* __restrict__ prob, int L, int lp, int splits, int rows_cap,
+                                                                  const int* __restrict__ boards_dev) {
+    extern __shared__ float s_l[];  // [L]
+    __shared__ float s_red[8];
+    __shared__ float s_bcast;
+    if (boards_dev != nullptr && static_cast<int>(blockIdx.x) >= *boards_dev) return;  // row without input
+    pdl_wait();
+    pdl_launch_dependents();
+    const int b = blockIdx.x;
+    float mx = -INFINITY;
+    for (int i = threadIdx.x; i < L; i += 256) {
+        float v = __ldg(bias + i);
+        for (int s = 0; s < splits; ++s) v += part[(static_cast<size_t>(s) * rows_cap + b) * lp + i];
+        s_l[i] = v;
+        mx = fmaxf(mx, v);
     }
-    __syncthreads();
-    mx = s_bcast;
-    float sum = 0.0f;
-    for (int i = t; i < L; i += 256) {
-        const float e = expf(s_l[i] - mx);
-        s_l[i] = e;
-        sum += e;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
-    __syncthreads();
-    if (lane == 0) s_red[warp] = sum;
-    __syncthreads();
-    if (t == 0) {
-        float s = 0.0f;
-        for (int i = 0; i < 8; ++i) s += s_red[i];
-        s_bcast = 1.0f / s;
-    }
-    __syncthreads();
-    const float inv = s_bcast;
-    float* pb = prob + static_cast<size_t>(b) * L;
-    for (int i = t; i < L; i += 256) pb[i] = s_l[i] * inv;
+    block_softmax_256(s_l, L, mx, prob + static_cast<size_t>(b) * L, s_red, &s_bcast);
 }
 
 // Node::set_probabilities_for_moves (node.cpp:961-979) for a whole batch: out[b][i] = prob[b][idx[b][i]], i < counts[b].

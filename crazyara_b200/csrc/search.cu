@@ -617,6 +617,9 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     if (net_ != nullptr) {
         if (net_->batch < n_trees * sp.batch_size)
             return set_error("ara_search_create: network batch %d < trees %d x Batch_Size %d", net_->batch, n_trees, sp.batch_size);
+        if (!net_->is_policy_map())  // the tree kernels park policy-map indices in the children's priors
+            return set_error("ara_search_create: the network has a fully-connected policy head (classic labels); the search "
+                             "runs policy-map networks");
         if (net_->n_labels() != n_labels_ || net_->hdr.in_channels != planes_channels(sp.mode, sp.input_version))
             return set_error("ara_search_create: network shape (C=%d, L=%d) does not match mode/version (C=%d, L=%d)",
                              net_->hdr.in_channels, net_->n_labels(), planes_channels(sp.mode, sp.input_version), n_labels_);

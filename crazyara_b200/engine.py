@@ -299,6 +299,9 @@ class RawNetAgent:
     def __init__(self, net, mode, input_version):
         if net is None:
             raise AraError("RawNetAgent needs a network")
+        if not net.is_policy_map():  # legal_moves_gpu gives policy-map indices; classic labels are not mapped yet
+            raise AraError("RawNetAgent: the network has a fully-connected policy head (classic labels); only policy-map "
+                           "networks are supported")
         self.net, self.mode, self.input_version = net, mode, input_version
 
     def predict(self, states):

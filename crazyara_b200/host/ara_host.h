@@ -364,6 +364,10 @@ class RawNetAgent {
             evalInfo.centipawns = value_to_centipawn(0.0f, param);
             return;
         }
+        // ara_legal_moves gives policy-map indices: the classic labels of a fully-connected policy head are not mapped yet
+        if (!net_->is_policy_map())
+            throw std::runtime_error("RawNetAgent: the network has a fully-connected policy head (classic labels); only "
+                                     "policy-map networks are supported");
         ara_board_t board;
         ara_state_board(state.handle(), &board);
         Action moves[512];

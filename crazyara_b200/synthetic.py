@@ -115,7 +115,30 @@ def random_state_dict(arch, seed=0):
     sd["policy_head.body.0.weight"] = normal((C, C, 3, 3), np.sqrt(2.0 / (9 * C)))
     batchnorm("policy_head.body.1", C)
     sd["policy_head.body.3.weight"] = normal((arch["policy_channels"], C, 3, 3), 2.0 * np.sqrt(2.0 / (9 * C)))
+    if arch.get("n_labels"):
+        sd.update(classic_head(arch, arch["n_labels"], seed))
     return sd
+
+
+def classic(arch, n_labels):
+    """the same network with a fully-connected policy head onto the n_labels classic labels (the trainer's
+    select_policy_from_plane=False, builder_util.py _PolicyHead): 1968 chess, 2272 crazyhouse, 2316 lichess variants"""
+    return dict(arch, name=f"{arch['name']}_fc{n_labels}", n_labels=n_labels)
+
+
+def classic_head(arch, n_labels, seed=0):
+    """Seeded parameters of the fully-connected policy head under the state_dict names (policy_head.body2.0 BatchNorm2d,
+    policy_head.body3.0 Linear), from a generator of their own so that the rest of a state_dict stays as it is.  The
+    logits come out with a spread of a few units, as a trained head's do."""
+    g = np.random.default_rng([seed, n_labels])
+    P, f32 = arch["policy_channels"], np.float32
+    k = P * 64
+    return {"policy_head.body2.0.weight": g.uniform(0.8, 1.2, P).astype(f32),
+            "policy_head.body2.0.bias": (g.standard_normal(P) * 0.1).astype(f32),
+            "policy_head.body2.0.running_mean": (g.standard_normal(P) * 0.1).astype(f32),
+            "policy_head.body2.0.running_var": g.uniform(0.5, 1.5, P).astype(f32),
+            "policy_head.body3.0.weight": (g.standard_normal((n_labels, k)) * 2.0 / np.sqrt(k)).astype(f32),
+            "policy_head.body3.0.bias": (g.standard_normal(n_labels) * 0.1).astype(f32)}
 
 
 def mx_twin(arch):

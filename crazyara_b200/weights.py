@@ -17,6 +17,9 @@ AlphaVile (alpha_vile.py: RiseV3 with a 192 / 224 channel trunk and NextViT tran
 ARAB2003: the header of ARAB2002 with any trunk width from 64 to 256, and a type word in front of every block record
 (0: a bottleneck block as in ARAB2001, 1: an NTB with its widths M, Ca, H).  The NTB's pre-norms norm1 and norm2 are
 folded into q / k / v and mlp.conv1 the way the reference's merge_pre_bn does before its ONNX export.
+
+A network with a fully-connected policy head (the trainer's select_policy_from_plane=False: policy_head.body2 BatchNorm
++ ReLU and policy_head.body3 Linear onto the classic labels) is written as ARAB2004 around one of the three (write_blob).
 """
 import struct
 
@@ -95,7 +98,12 @@ def export_blob(sd, arch, path, input_version=10):
         put(_np(sd["value_head.body_final.2.weight"])), put(_np(sd["value_head.body_final.2.bias"]))
     w, b = _fold(sd, "policy_head.body.0.weight", "policy_head.body.1")
     put(w), put(b)
-    put(_np(sd["policy_head.body.3.weight"]))
+    if arch.get("n_labels"):  # select_policy_from_plane=False: BatchNorm + ReLU behind the last convolution, then the Linear
+        w, b = _fold(sd, "policy_head.body.3.weight", "policy_head.body2.0")
+        put(w), put(b)
+        put(_np(sd["policy_head.body3.0.weight"])), put(_np(sd["policy_head.body3.0.bias"]))
+    else:
+        put(_np(sd["policy_head.body.3.weight"]))
     return write_blob(path, arch, tensors, input_version)
 
 
@@ -125,18 +133,32 @@ def ntb_tensors(sd, p):
     return out
 
 
+CLASSIC_LABELS = (1968, 2272, 2316)  # NB_LABELS of chess, crazyhouse and the lichess variants (crazyara_b200.labels)
+
+
 def write_blob(path, arch, tensors, input_version):
     """Header, block table and the float32 tensors (flattened, in net.cu's order).  ARAB2001 for the PyTorch semantics;
     ARAB2002 when arch["semantics"] == "mxnet" (every block's shortcut from its input before the SE, ca_se with biases);
-    ARAB2003 for a trunk narrower than 256 channels or with NTB blocks (arch["ntb"], widths mhsa / mhca / mlp)."""
+    ARAB2003 for a trunk narrower than 256 channels or with NTB blocks (arch["ntb"], widths mhsa / mhca / mlp).
+
+    A network with a fully-connected policy head (arch["n_labels"] = L, the trainer's select_policy_from_plane=False) is
+    ARAB2004: the magic, the base format's number (1, 2 or 3) and L, then the base blob from its header on.  Its last
+    policy convolution has the BatchNorm of the head folded in, so the tensors end with that convolution's weight and
+    bias [P], W_fc [L][P * 64] (the trainer's NCHW flatten) and b_fc [L]; the base header's policy_bias stays 0."""
     mx = arch.get("semantics") == "mxnet"
     ntb = arch.get("ntb") or [False] * len(arch["kernels"])
     C = arch.get("channels", 256)
     v3 = any(ntb) or C != 256
     if mx and v3:
         raise ValueError("ARAB2003 has no blocks with the MXNet semantics")
+    n_labels = arch.get("n_labels")
+    if n_labels and arch.get("policy_bias"):
+        raise ValueError("ARAB2004 carries the policy convolution's bias with its head (policy_bias must be False)")
     with open(path, "wb") as f:
-        f.write(b"ARAB2003" if v3 else b"ARAB2002" if mx else b"ARAB2001")
+        if n_labels:
+            f.write(b"ARAB2004" + struct.pack("<2i", 3 if v3 else 2 if mx else 1, n_labels))
+        else:
+            f.write(b"ARAB2003" if v3 else b"ARAB2002" if mx else b"ARAB2001")
         f.write(struct.pack("<8i", arch["in_channels"], arch["policy_channels"], len(arch["kernels"]), C, 8,
                             arch.get("value_fc", 256) if v3 else 256, 1 if arch["wdl"] else 0, input_version))
         if mx or v3:
@@ -158,23 +180,35 @@ def write_blob(path, arch, tensors, input_version):
 
 
 def read_blob(path):
-    """The inverse of write_blob: an ARAB2001 / 2002 / 2003 blob -> (arch, tensors [flat float32], input_version).  arch
+    """The inverse of write_blob: an ARAB2001 / 2002 / 2003 / 2004 blob -> (arch, tensors [flat float32], input_version).  arch
     holds what the header and block table say, under write_blob's keys; write_blob(path2, *read_blob(path)) rewrites the
     file byte for byte.  A blob write_blob cannot have written (ARAB2002 block flags other than the ones it sets, an unknown
     block type, a tensor past the end of the file) is refused."""
     buf = open(path, "rb").read()
     magic = buf[:8]
-    if magic not in (b"ARAB2001", b"ARAB2002", b"ARAB2003"):
-        raise ValueError(f"{path}: not an ARAB2001 / 2002 / 2003 blob")
+    if magic not in (b"ARAB2001", b"ARAB2002", b"ARAB2003", b"ARAB2004"):
+        raise ValueError(f"{path}: not an ARAB2001 / 2002 / 2003 / 2004 blob")
+    off, n_labels = 8, 0
+    if magic == b"ARAB2004":
+        base, n_labels = struct.unpack_from("<2i", buf, 8)
+        if base not in (1, 2, 3):
+            raise ValueError(f"{path}: ARAB2004 wraps base format {base}")
+        if n_labels not in CLASSIC_LABELS:
+            raise ValueError(f"{path}: {n_labels} policy labels (the classic label lists have {CLASSIC_LABELS})")
+        magic, off = b"ARAB200%d" % base, 16
     mx, v3 = magic == b"ARAB2002", magic == b"ARAB2003"
-    cin, pch, n, C, vc, fc, wdl, version = struct.unpack_from("<8i", buf, 8)
+    cin, pch, n, C, vc, fc, wdl, version = struct.unpack_from("<8i", buf, off)
     arch = dict(in_channels=cin, policy_channels=pch, channels=C, value_channels=vc, value_fc=fc, wdl=bool(wdl),
                 kernels=[], se_types=[], c_ops=[])
-    off = 40
+    if n_labels:
+        arch["n_labels"] = n_labels
+    off += 32
     if mx or v3:
         stem_act, policy_bias = struct.unpack_from("<2i", buf, off)
         arch.update(stem_act=bool(stem_act), policy_bias=bool(policy_bias))
         off += 8
+        if n_labels and policy_bias:
+            raise ValueError(f"{path}: ARAB2004 carries the policy convolution's bias with its head, not in the base header")
     if mx:
         arch.update(semantics="mxnet", se_gates=[])
     if v3:
@@ -323,6 +357,8 @@ def arch_from_state_dict(sd):
                 channels=C, kernels=kernels, se_types=se_types, c_ops=c_ops,
                 wdl="value_head.body_wdl.0.weight" in keys, value_channels=int(sd["value_head.body.0.weight"].shape[0]),
                 value_fc=256)
+    if "policy_head.body3.0.weight" in keys:  # select_policy_from_plane=False (builder_util.py _PolicyHead body2 / body3)
+        arch["n_labels"] = int(sd["policy_head.body3.0.weight"].shape[0])
     if any(ntb) or C != 256:
         if len(widths) > 1:
             raise ValueError(f"NTB blocks of different widths {sorted(widths)}")

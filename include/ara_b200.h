@@ -32,7 +32,8 @@ const char* ara_last_error(void);
  * ara_net_predict <-> NeuralNetAPI::predict(float* inputPlanes, float* valueOutput, float* probOutputs,
  *                     float* auxiliaryOutputs) (nn/neuralnetapi.h:237, nn/tensorrtapi.cpp:195-237):
  *                     planes [n, C, 8, 8] fp32 host -> value [n], prob [n, L] (softmax over ALL L labels, policy-map
- *                     order channel*64+square), aux [n, A].  Synchronous.  n <= batch_size rows are evaluated
+ *                     order channel*64+square; with is_policy_map = 0, a fully-connected policy head's, the order of
+ *                     the classic label list, crazyara_b200/labels.py), aux [n, A].  Synchronous.  n <= batch_size rows are evaluated
  *                     (the reference always runs the full batch; n < B just skips the unused rows).
  */
 #define ARA_PRECISION_FLOAT16 0
