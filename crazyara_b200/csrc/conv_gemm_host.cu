@@ -69,9 +69,24 @@ int conv_layer_choose_bn(int boards, int n_out) {
     return 64;
 }
 
+// N tiles up to 128: at 256 the accumulators (128 registers) leave no room beside them for the fragment sets of the
+// resident loop under the 168-register ceiling of a 288-thread block, and groups of half a k block ran slower than streaming
+bool conv_resident_a(int ksize, int c_chunks, int bn) {
+    if (ksize != 3) return false;
+    if (bn == 64) return c_chunks <= ConvGemmCfg<64>::kResidentMaxChunks;
+    if (bn == 128) return c_chunks <= ConvGemmCfg<128>::kResidentMaxChunks;
+    return false;
+}
+
 template <int BN>
 static cudaError_t allow_smem() {
-    return cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvGemmCfg<BN>::kSmemBytes);
+    using Cfg = ConvGemmCfg<BN>;
+    cudaError_t e = cudaFuncSetAttribute(conv_gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if constexpr (BN <= 128)
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(conv_gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     Cfg::resident_smem_bytes(Cfg::kResidentMaxChunks));
+    return e;
 }
 
 int conv_layer_init(ConvLayer* L, const __half* act, int boards_cap, int cin, const __half* w, int w_rows,
@@ -127,7 +142,14 @@ int conv_layer_build(ConvLayer* L, const __half* w, int w_rows, const float* bia
 
 template <int BN>
 static int launch_bn(const ConvLayer* L, const ConvGemmArgs& a, dim3 grid, cudaStream_t stream) {
-    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN>, grid, dim3(kGemmThreads), ConvGemmCfg<BN>::kSmemBytes, stream, L->tm_a, L->tm_b, a));
+    using Cfg = ConvGemmCfg<BN>;
+    if constexpr (BN <= 128)
+        if (conv_resident_a(a.ksize, a.c_chunks, BN)) {
+            ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN, true>, grid, dim3(kGemmThreads), Cfg::resident_smem_bytes(a.c_chunks),
+                                   stream, L->tm_a, L->tm_b, a));
+            return 0;
+        }
+    ARA_CUDA_OK(launch_pdl(conv_gemm_kernel<BN, false>, grid, dim3(kGemmThreads), Cfg::kSmemBytes, stream, L->tm_a, L->tm_b, a));
     return 0;
 }
 

@@ -15,6 +15,10 @@ struct ConvLayer {
 
 // Heuristic N-tile: biggest tile that still yields >= 120 CTAs, else 64.
 int conv_layer_choose_bn(int boards, int n_out);
+// Which main loop a layer runs: true for the 3x3 layers whose c_chunks A tiles fit in shared memory beside the B ring
+// of N tile bn (each CTA loads its activations once and feeds every tap from them); false for the streaming loop, which
+// fetches the shifted A tile of every (tap, chunk) by TMA and runs any layer.
+bool conv_resident_a(int ksize, int c_chunks, int bn);
 
 // act:  [boards_cap, 8, 8, cin] fp16 (boards_cap even), w: [w_rows, taps*ceil64(cin)] fp16 (w_rows % bn == 0),
 // bias: [ldo] fp32 zero padded (or null), out: [boards*64, ldo].  act_pitch (0: cin): the activation rows are act_pitch
