@@ -16,16 +16,23 @@ graph input, block by block, to the heads, looking through shape-only nodes.
   is the `Add` fed by the block input, traced back through BatchNormalization / Relu / Conv to its first convolution,
   whose input is the block input or its `Mul` with the gate (`Sigmoid`, or `HardSigmoid` with alpha 0.2).
 Both trace the gate back to `Gemm, Relu, Gemm` (ca_se) or to a 1-D `Conv` over the channels (eca_se).
+A fully-connected policy head (the trainer's select_policy_from_plane=False) is the last policy convolution's output
+(an MXNet export: through its BatchNormalization policy_bn1) followed by Relu, a flatten and Gemm (or MatMul + Add) onto
+a classic label list; it is written as ARAB2004 around the base format.  Such a layer that does not take the flattened
+ReLU, has another label count or another width is refused, as are a bias or a Relu behind a folded policy-map
+convolution and a policy_bn1 with no such layer behind it: no blob format holds them, and dropping them would change
+the network.
 
 PARITY UNPINNED: the reference tree holds no .onnx file and no `onnx` / `onnxsim` package is installed, so the readers are
-checked against files written by tests/onnx_writer.py, tests/onnx_mx_writer.py and tests/onnx_alphavile_writer.py.
+checked against files written by tests/onnx_writer.py, tests/onnx_mx_writer.py and tests/onnx_alphavile_writer.py
+(tests/onnx_classic_writer.py adds the fully-connected policy head to them).
 """
 import struct
 from collections import defaultdict
 
 import numpy as np
 
-from .weights import export_mx_blob, input_version_of, write_blob
+from .weights import CLASSIC_LABELS, export_mx_blob, input_version_of, write_blob
 
 _SHAPE_OPS = ("Reshape", "Flatten", "Squeeze", "Unsqueeze", "Identity")
 # a torch export also has the NTB's token transposes and the Expand of the SE gate (x * y.view(b, c, 1, 1).expand_as(x))
@@ -217,6 +224,27 @@ class _Graph:
             self.fail(f"no bias behind MatMul '{mm[2][0]}'")
         return self.weight(mm), b, add[2][0]
 
+    def policy_fc(self, t, P):
+        """The fully-connected policy head behind tensor t, the last policy convolution's output (an MXNet export: its
+        BatchNorm's): Relu, a flatten (Flatten, or the Reshape of torch's view()), then Gemm or MatMul + Add onto the
+        classic labels -> (W_fc [L][P * 64], b_fc [L]); None when no fully-connected layer follows t (a policy map)"""
+        fc = self.downstream(t, ("Gemm", "MatMul"))
+        if fc is None:
+            return None
+        relu = self.prod.get(fc[1][0])
+        while relu is not None and relu[0] in self.skip:
+            relu = self.prod.get(relu[1][0])
+        if relu is None or relu[0] != "Relu" or relu[1][0] != t or len(fc[1]) < 2 or fc[1][1] not in self.inits:
+            self.fail(f"policy head: the {fc[0]} behind the last policy convolution does not take its flattened ReLU")
+        w, b = (self.weight(fc), self.bias(fc)) if fc[0] == "Gemm" else self.linear(fc)[:2]
+        if w.shape[0] not in CLASSIC_LABELS:
+            self.fail(f"policy head: a fully-connected layer onto {w.shape[0]} labels (the classic label lists have "
+                      f"{CLASSIC_LABELS})")
+        if w.shape[1] != P * 64:
+            self.fail(f"policy head: the fully-connected layer takes {w.shape[1]} features, not the {P} x 64 of the flattened "
+                      f"convolution")
+        return w, b
+
     def stem(self):  # the convolution on the graph input
         return next((nd for nd in self.nodes if nd[0] == "Conv" and nd[1][0] not in self.prod and nd[1][0] not in self.inits), None)
 
@@ -239,7 +267,8 @@ def import_onnx(onnx_path, blob_path, input_version=None, channels=256):
 
 
 def _import_mxnet_graph(g, blob_path, input_version, channels):
-    """a graph with unfolded BatchNormalization nodes (an MXNet export) -> ARAB2002 blob"""
+    """a graph with unfolded BatchNormalization nodes (an MXNet export) -> ARAB2002 blob (ARAB2004 around it with a
+    fully-connected policy head)"""
     params, eps = {}, {}
 
     def take_bn(nd, name):
@@ -311,17 +340,31 @@ def _import_mxnet_graph(g, blob_path, input_version, channels):
     take(g0, "value_fc0"), take(g1, "value_fc1")
     take(pconv[0], "policy_conv0")
     take_bn(g.first(pconv[0][2][0], "BatchNormalization"), "policy_bn0")
-    take(g.downstream(pconv[0][2][0], ("Conv",)), "policy_conv1")
+    pc1 = g.downstream(pconv[0][2][0], ("Conv",))
+    take(pc1, "policy_conv1")
+    P = int(params["policy_conv1_weight"].shape[0])
+    # select_policy_from_plane=False (builder_util_symbol.py policy_head): policy_bn1, the activation, Flatten, policy_out
+    bn1 = g.first(pc1[2][0], "BatchNormalization")
+    head = g.policy_fc(bn1[2][0] if bn1 is not None else pc1[2][0], P)
+    if head is not None and bn1 is None:
+        g.fail("policy head: no BatchNormalization (policy_bn1) between the last policy convolution and its ReLU")
+    if head is None and bn1 is not None:
+        g.fail("policy head: a BatchNormalization behind the last policy convolution but no fully-connected layer")
     arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(g.weight(stem).shape[1]),
-                policy_channels=int(params["policy_conv1_weight"].shape[0]), channels=channels, kernels=kernels,
+                policy_channels=P, channels=channels, kernels=kernels,
                 se_types=se_types, se_gates=se_gates, c_ops=c_ops, wdl=False, value_channels=int(params["value_conv0_weight"].shape[0]),
                 value_fc=256, stem_act=stem_act, policy_bias="policy_conv1_bias" in params)
+    if head is not None:  # the convolution's bias is folded with policy_bn1 into the head (ARAB2004)
+        take_bn(bn1, "policy_bn1")
+        params["policy_out_weight"], params["policy_out_bias"] = head
+        arch.update(policy_bias=False, n_labels=int(head[0].shape[0]))
     export_mx_blob(params, arch, blob_path, input_version_of(arch, input_version), eps=eps, fix_gamma=False)
     return arch
 
 
 def _import_folded_graph(g, blob_path, input_version, channels):
-    """a BatchNorm-folded export: a RISE network (256-channel trunk) -> ARAB2001 blob, an AlphaVile one -> ARAB2003"""
+    """a BatchNorm-folded export: a RISE network (256-channel trunk) -> ARAB2001 blob, an AlphaVile one -> ARAB2003 (ARAB2004
+    around either with a fully-connected policy head)"""
     W, bias = g.weight, g.bias
     mat = lambda a: a.reshape(a.shape[0], -1)
     stem = g.stem()
@@ -446,6 +489,16 @@ def _import_folded_graph(g, blob_path, input_version, channels):
         (M, Ca, H), = widths
         arch.update(name=f"alphavile_{len(kernels)}b", ntb=ntb, mhsa=M, mhca=Ca, mlp=H,
                     value_fc=C if wdl else int(W(fc[0]).shape[0]))
+    # select_policy_from_plane=False: the exporter has folded the head's BatchNorm (body2) into p2, ReLU, view(), Linear
+    head = g.policy_fc(p2[2][0], arch["policy_channels"])
+    if head is not None:
+        tensors += [bias(p2), *head]
+        arch["n_labels"] = int(head[0].shape[0])
+    elif np.any(bias(p2) != 0):
+        g.fail("policy head: the last policy convolution has a bias but no fully-connected layer behind it (a policy map's "
+               "convolution has none)")
+    elif g.first(p2[2][0], "Relu") is not None:
+        g.fail("policy head: a Relu behind the last policy convolution but no fully-connected layer")
     write_blob(blob_path, arch, tensors, input_version_of(arch, input_version))
     return arch
 
@@ -455,4 +508,5 @@ if __name__ == "__main__":
     if len(sys.argv) < 3:
         raise SystemExit("usage: python -m crazyara_b200.onnx_import <model.onnx> <out.arab> [input_version]")
     a = import_onnx(sys.argv[1], sys.argv[2], int(sys.argv[3]) if len(sys.argv) > 3 else None)
-    print(f"{sys.argv[2]}: {len(a['kernels'])} blocks, {a['in_channels']} -> {a['policy_channels']}x64, wdl={a['wdl']}")
+    policy = f"{a['n_labels']} labels" if a.get("n_labels") else f"{a['policy_channels']}x64"
+    print(f"{sys.argv[2]}: {len(a['kernels'])} blocks, {a['in_channels']} -> {policy}, wdl={a['wdl']}")

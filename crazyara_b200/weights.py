@@ -19,7 +19,8 @@ ARAB2003: the header of ARAB2002 with any trunk width from 64 to 256, and a type
 folded into q / k / v and mlp.conv1 the way the reference's merge_pre_bn does before its ONNX export.
 
 A network with a fully-connected policy head (the trainer's select_policy_from_plane=False: policy_head.body2 BatchNorm
-+ ReLU and policy_head.body3 Linear onto the classic labels) is written as ARAB2004 around one of the three (write_blob).
++ ReLU and policy_head.body3 Linear onto the classic labels; in the MXNet symbols policy_bn1, the activation and
+FullyConnected policy_out) is written as ARAB2004 around one of the three (write_blob).
 """
 import struct
 
@@ -281,7 +282,10 @@ def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamm
     arch: as oracle.net_mx.arch_mx_risev2 / arch_mx_risev33 (semantics "mxnet", se_gates, stem_act, policy_bias).
     eps: BatchNorm epsilon, one value or {BatchNorm name: eps} (missing names: MXNet's default 1e-3).  fix_gamma: the
     BatchNorm gammas are fixed to 1 (mx.sym.BatchNorm's default), whatever values the parameters hold.  ca_se hidden
-    widths below 128 are zero-padded to 128; the eca_se convolution becomes its banded 256 x 256 matrix."""
+    widths below 128 are zero-padded to 128; the eca_se convolution becomes its banded 256 x 256 matrix.
+    arch["n_labels"] set (select_policy_from_plane=False, builder_util_symbol.py policy_head): policy_conv1 is folded with
+    policy_bn1, its bias included, and FullyConnected policy_out follows; the blob is ARAB2004 around ARAB2002, and
+    arch["policy_bias"] has to be False (the bias goes with the head)."""
     assert arch.get("semantics") == "mxnet"
     tensors = []
     put = tensors.append
@@ -316,9 +320,14 @@ def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamm
         put(_np(params[n + "_weight"])), put(_np(params[n + "_bias"]))
     w, b = fold("policy_conv0", "policy_bn0")
     put(w), put(b)
-    put(_np(params["policy_conv1_weight"]))
-    if arch["policy_bias"]:
-        put(_np(params["policy_conv1_bias"]))
+    if arch.get("n_labels"):  # select_policy_from_plane=False: policy_bn1 and the activation, Flatten, policy_out
+        w, b = fold("policy_conv1", "policy_bn1")  # (with the convolution's bias, which the v3 symbol has)
+        put(w), put(b)
+        put(_np(params["policy_out_weight"])), put(_np(params["policy_out_bias"]))
+    else:
+        put(_np(params["policy_conv1_weight"]))
+        if arch["policy_bias"]:
+            put(_np(params["policy_conv1_bias"]))
     return write_blob(path, arch, tensors, input_version)
 
 
