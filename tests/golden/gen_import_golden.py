@@ -23,7 +23,7 @@ from oracle import net_mx  # noqa: E402
 from tests.onnx_alphavile_writer import write_alphavile_onnx  # noqa: E402
 from tests.onnx_mx_writer import write_mx_onnx  # noqa: E402
 from tests.onnx_writer import add_shape_concat, write_rise_onnx  # noqa: E402
-from tests.test_net_mx_gpu import mixed_arch  # noqa: E402
+from tests.net_harness import mixed_arch  # noqa: E402
 
 PATH = os.path.join(ROOT, "tests", "golden", "import_golden.json")
 RISE = {"risev2": (lambda: synthetic.risev2(34, 81), 10), "risev33": (lambda: synthetic.risev33(52, 76), 30)}

@@ -1,127 +1,57 @@
-"""GPU network vs the fp32 oracle (oracle/net.py, pinned to the reference's torch module), through the C-ABI with host
-buffers, in both settings of the reference's UCI option `Precision` (engine/src/uci/optionsuci.cpp:144):
-
-  float16 (the reference's default): fp16 tensor-core operands and activations, fp32 accumulation -> value within
-          4e-3, probabilities within 3 % of the fp32 oracle;
-  float32: the same wgmma GEMMs with fp16 hi + lo operand splitting and fp32 activations between the layers ->
-          value and every probability within 1e-4 (north_star's float tolerance), in practice ~1e-6."""
-import os
-
+"""GPU networks against their fp32 oracles through the C-ABI with host buffers, in both settings of the reference's UCI
+option `Precision`, within the bounds of tests/net_harness.py.  One table holds every network family's comparisons:
+the torch RISE networks (ARAB2001, oracle/net.py), the reference's MXNet symbols (ARAB2002, oracle/net_mx.py),
+AlphaVile (ARAB2003, oracle/net_alphavile.py) and the fully-connected policy head on top of each (ARAB2004,
+tests/classic_head.py, tests/classic_mx_head.py)."""
 import numpy as np
 import pytest
 
-from oracle import net as onet
-from oracle import net_mx
-from tests.golden.gen_net_golden import golden_input
+from tests import net_harness as nh
 
-VALUE_ATOL = 4e-3
-LOGIT_ATOL = 2.5e-2
-PROB_RTOL = 3e-2
-
-
-F32_ATOL = 1e-4  # north_star: "floats within 1e-4"
-
-
-def _make_net(tmp_path, arch, batch, version, precision="float16"):
-    from crazyara_b200.nn import NeuralNetAPI
-    from crazyara_b200.weights import export_blob
-    sd = onet.make_state_dict(arch, 0)
-    blob = export_blob(sd, arch, str(tmp_path / f"{arch['name']}.arab"), input_version=version)
-    return NeuralNetAPI("gpu", 0, batch, blob, precision=precision), sd
-
-
-CASES = [("risev2", 34, 81, 8, 8), ("risev2", 34, 81, 64, 64), ("risev2", 34, 81, 1, 1), ("risev33", 52, 76, 64, 64),
-         ("risev33", 52, 76, 8, 5), ("risev2", 63, 84, 16, 16)]
+P16, P32 = "float16", "float32"
+# (kind, batch, n): batches from 1 to 128, 66 a partial last board tile of the fully-connected head
+RISE = [("risev2", 8, 8), ("risev2", 64, 64), ("risev2", 1, 1), ("risev33", 64, 64), ("risev33", 8, 5),
+        ("risev2_63_84", 16, 16)]
+FC = [("fc_risev2_81_2272", 1, 1), ("fc_risev2_81_2272", 8, 5), ("fc_risev2_81_2272", 64, 64),
+      ("fc_risev2_81_2272", 66, 66), ("fc_risev2_81_2272", 128, 128), ("fc_risev33_76_1968", 8, 8),
+      ("fc_risev2_2_2316", 8, 8), ("fc_risev2_16_1968", 64, 64), ("fc_av_tiny_2316", 8, 8)]
+FC_MX = [("fc_mx_risev2_2272", 1, 1), ("fc_mx_risev2_2272", 8, 5), ("fc_mx_risev2_2272", 66, 66),
+         ("fc_mx_risev2_2272", 128, 128), ("fc_mx_risev33_1968", 1, 1), ("fc_mx_risev33_1968", 16, 16),
+         ("fc_mx_risev33_1968", 128, 128)]
+# (kind, batch, n, precision, input seed), grouped by kind
+CASES = sorted([(k, b, n, P16, 5) for k, b, n in RISE] +
+               [(k, b, n, P32, 5) for k, b, n in RISE + [("risev2_63_84", 128, 128), ("risev33_64_81", 16, 16)]] +
+               [(k, n, n, p, seed) for k in ("mx_risev2", "mx_risev33", "mx_mixed", "av_tiny", "av_normal")
+                for p, seed, sizes in ((P16, 21, (1, 5, 64, 66, 128)), (P32, 22, (1, 16))) for n in sizes] +
+               [(k, b, n, p, 5) for k, b, n in FC for p in (P16, P32)] +
+               [(k, b, n, p, 31) for k, b, n in FC_MX for p in (P16, P32)], key=lambda c: c[0])
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("name,cin,pch,batch,n", CASES)
-def test_net_predict_matches_oracle(tmp_path, name, cin, pch, batch, n):
-    arch = onet.arch_risev2(cin, pch) if name == "risev2" else onet.arch_risev33(cin, pch, True)
-    net, sd = _make_net(tmp_path, arch, batch, 10 if name == "risev2" else 30)
-    assert net.get_nb_policy_values() == pch * 64 and net.get_nb_input_values_total() == cin * 64
-    x = golden_input(arch, n=n, seed=5)
-    value = np.full(batch, np.nan, np.float32)
-    prob = np.full((batch, pch * 64), np.nan, np.float32)
-    aux = np.full((batch, 4), np.nan, np.float32)
-    xin = np.zeros((batch, cin, 8, 8), np.float32)
-    xin[:n] = x
-    net.predict(xin, value, prob, aux if arch["wdl"] else None, n=n)
-    ref = onet.forward(sd, arch, x)
-    assert np.isfinite(value[:n]).all() and np.isfinite(prob[:n]).all()
-    np.testing.assert_allclose(prob[:n].sum(1), 1.0, atol=1e-4)
-    np.testing.assert_allclose(value[:n], ref["value"], atol=VALUE_ATOL)
-    logit_gpu = np.log(prob[:n]) - np.log(prob[:n]).mean(1, keepdims=True)
-    logit_ref = ref["policy_logits"] - ref["policy_logits"].mean(1, keepdims=True)
-    assert np.abs(logit_gpu - logit_ref).max() < LOGIT_ATOL
-    np.testing.assert_allclose(prob[:n], ref["prob"], rtol=PROB_RTOL, atol=1e-7)
-    if arch["wdl"]:
-        np.testing.assert_allclose(aux[:n], ref["aux"], atol=6e-3)
-    # second call must give bit-identical results (graph replay, no stale state)
-    value2, prob2 = value.copy(), prob.copy()
-    net.predict(xin, value2, prob2, None, n=n)
-    assert np.array_equal(value2[:n], value[:n]) and np.array_equal(prob2[:n], prob[:n])
-    net.close()
-
-
-F32_CASES = CASES + [("risev2", 63, 84, 128, 128), ("risev33", 64, 81, 16, 16)]
+@pytest.fixture(scope="module")
+def nets(tmp_path_factory):
+    yield from nh.module_nets(tmp_path_factory)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,cin,pch,batch,n", F32_CASES)
-def test_net_predict_float32_within_1e4_of_oracle(tmp_path, name, cin, pch, batch, n):
-    """Precision float32: value, probabilities (and WDL / plys auxiliary outputs) within 1e-4 of the fp32 oracle."""
-    arch = onet.arch_risev2(cin, pch) if name == "risev2" else onet.arch_risev33(cin, pch, True)
-    net, sd = _make_net(tmp_path, arch, batch, 10 if name == "risev2" else 30, precision="float32")
-    x = golden_input(arch, n=n, seed=5)
-    value = np.full(batch, np.nan, np.float32)
-    prob = np.full((batch, pch * 64), np.nan, np.float32)
-    aux = np.full((batch, 4), np.nan, np.float32)
-    xin = np.zeros((batch, cin, 8, 8), np.float32)
-    xin[:n] = x
-    net.predict(xin, value, prob, aux if arch["wdl"] else None, n=n)
-    ref = onet.forward(sd, arch, x)
-    np.testing.assert_allclose(value[:n], ref["value"], atol=F32_ATOL, rtol=0)
-    np.testing.assert_allclose(prob[:n], ref["prob"], atol=F32_ATOL, rtol=0)
-    np.testing.assert_allclose(prob[:n], ref["prob"], rtol=2e-3, atol=1e-8)   # and small probabilities relatively
-    logit_gpu = np.log(prob[:n]) - np.log(prob[:n]).mean(1, keepdims=True)
-    logit_ref = ref["policy_logits"] - ref["policy_logits"].mean(1, keepdims=True)
-    assert np.abs(logit_gpu - logit_ref).max() < 1e-3
-    if arch["wdl"]:
-        np.testing.assert_allclose(aux[:n], ref["aux"], atol=F32_ATOL)
-    value2, prob2 = value.copy(), prob.copy()
-    net.predict(xin, value2, prob2, None, n=n)
-    assert np.array_equal(value2[:n], value[:n]) and np.array_equal(prob2[:n], prob[:n])
-    net.close()
+@pytest.mark.parametrize("kind,batch,n,precision,seed", CASES)
+def test_net_predict_matches_oracle(nets, kind, batch, n, precision, seed):
+    kn = nets(kind)
+    net, arch = kn.net(batch, precision), kn.arch
+    assert net.is_policy_map() == ("n_labels" not in arch) and net.get_nb_policy_values() == nh.n_labels(arch)
+    assert net.get_nb_input_values_total() == arch["in_channels"] * 64
+    x, ref = kn.ref(n, seed)
+    out = nh.predict(net, arch, x)
+    (nh.check_float16 if precision == P16 else nh.check_float32)(out, ref)
+    nh.check_replay_bits(net, arch, x, out)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("precision", ["float16", "float32"])
-@pytest.mark.parametrize("name", ["risev33", "mx_risev2"])
-def test_launch_bookkeeping_matches_the_launches(tmp_path, name, precision):
-    """The first forward of a size runs eagerly (every launch counted) before it is captured; a graph replay then adds
-    the launches its capture enqueued.  Both must agree with the layer plan: input conversion, stem, the tower kernel
-    (float16) or per block the squeeze-excitation if any, conv1, depthwise and conv2 (float32), value head, two policy
-    convolutions, softmax.  (AlphaVile: tests/test_net_alphavile_gpu.py)"""
-    from crazyara_b200.nn import NeuralNetAPI
-    from crazyara_b200.weights import export_mx_blob
-    if name == "risev33":
-        arch = onet.arch_risev33(52, 76, True)
-        net, _ = _make_net(tmp_path, arch, 4, 30, precision)
-    else:
-        arch = net_mx.arch_mx_risev2(34, 81)
-        blob = export_mx_blob(net_mx.make_mx_params(arch, 7), arch, str(tmp_path / f"{name}.arab"), input_version=10)
-        net = NeuralNetAPI("gpu", 0, 4, blob, precision=precision)
-    x = golden_input(arch, n=4, seed=25)
-    v, p = np.zeros(4, np.float32), np.zeros((4, arch["policy_channels"] * 64), np.float32)
-    net.predict(x, v, p, None, n=4)
-    first = net.launch_count()
-    net.predict(x, v, p, None, n=4)
-    per_forward = net.launch_count() - first
-    net.close()
-    assert first == 2 * per_forward
-    tower = 1 if precision == "float16" else sum(3 + (se is not None) for se in arch["se_types"])
-    assert per_forward == 1 + 1 + tower + 4
+@pytest.mark.parametrize("precision", [P16, P32])
+@pytest.mark.parametrize("kind", ["risev33", "mx_risev2"])
+def test_launch_bookkeeping_matches_the_launches(nets, kind, precision):
+    """input conversion, stem, the tower kernel (float16) or per block the squeeze-excitation if any, conv1, depthwise
+    and conv2 (float32), value head, two policy convolutions, softmax"""
+    nh.check_launch_count(nets(kind), precision, n=4, seed=25)
 
 
 @pytest.mark.gpu
@@ -136,80 +66,37 @@ def test_net_create_fails_loudly_on_bad_blob(tmp_path):
         NeuralNetAPI("gpu", 0, 8, str(tmp_path / "missing.arab"))
 
 
-def _assert_rows_independent(tmp_path, precision):
-    """A board's value / policy bits at a row of a batch of 3 equal its bits at its row of a batch of 64."""
-    arch = onet.arch_risev2(34, 81)
-    x = golden_input(arch, n=64, seed=9)
-    net64, _ = _make_net(tmp_path, arch, 64, 10, precision)
-    v64, p64 = np.zeros(64, np.float32), np.zeros((64, 81 * 64), np.float32)
-    net64.predict(x, v64, p64, None, n=64)
-    net64.close()
-    net3, _ = _make_net(tmp_path, arch, 3, 10, precision)
-    for src in (0, 37, 63):
-        xin = np.zeros((3, 34, 8, 8), np.float32)
-        xin[1] = x[src]
-        xin[0] = x[(src + 5) % 64]
-        v, p = np.zeros(3, np.float32), np.zeros((3, 81 * 64), np.float32)
-        net3.predict(xin, v, p, None, n=2)
-        assert v[1] == v64[src] and np.array_equal(p[1], p64[src]), (precision, src)
-    net3.close()
-
-
 @pytest.mark.gpu
-def test_net_output_of_a_position_does_not_depend_on_its_batch(tmp_path):
+def test_net_output_of_a_position_does_not_depend_on_its_batch(nets):
     """The search relies on this: a leaf's value / policy are the same bits whichever mini-batch evaluates it."""
-    _assert_rows_independent(tmp_path, "float16")
+    nh.check_rows_independent(nets("risev2"), 64, (0, 37, 63), seed=9)
 
 
 @pytest.mark.gpu
-def test_float32_net_output_of_a_position_does_not_depend_on_its_batch(tmp_path):
+def test_float32_net_output_of_a_position_does_not_depend_on_its_batch(nets):
     """The same in Precision float32, where the 1x1 convolutions of the tower are GEMM launches whose tile width follows
     the batch (conv_layer_choose_bn): packed multi-tree float32 searches put a leaf at any row of a batch of any size."""
-    _assert_rows_independent(tmp_path, "float32")
+    nh.check_rows_independent(nets("risev2"), 64, (0, 37, 63), seed=9, precision=P32)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,cin,pch", [("risev2", 34, 81), ("risev33", 52, 76)])
-def test_float16_and_float32_networks_agree(tmp_path, monkeypatch, name, cin, pch):
-    """Persistent tower kernel (Precision float16: one board per CTA, then two boards per CTA) against the layer-by-layer
-    Precision float32 network: same weights, fp16 tolerance."""
-    arch = onet.arch_risev2(cin, pch) if name == "risev2" else onet.arch_risev33(cin, pch, True)
-    x = golden_input(arch, n=6, seed=3)
-    outs = []
-    for env, precision in (({}, "float32"), ({}, "float16"), ({"ARA_TRUNK_ROWS": "128"}, "float16")):
-        monkeypatch.delenv("ARA_TRUNK_ROWS", raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
-        net, _ = _make_net(tmp_path, arch, 6, 10 if name == "risev2" else 30, precision=precision)
-        v, p = np.zeros(6, np.float32), np.zeros((6, pch * 64), np.float32)
-        net.predict(x, v, p, None, n=6)
-        net.close()
-        outs.append((v, p))
-    for v, p in outs[1:]:
-        np.testing.assert_allclose(v, outs[0][0], atol=VALUE_ATOL)
-        np.testing.assert_allclose(p, outs[0][1], rtol=PROB_RTOL, atol=1e-6)
+@pytest.mark.parametrize("kind", ["risev2", "risev33"], ids=["risev2-34-81", "risev33-52-76"])
+def test_float16_and_float32_networks_agree(nets, monkeypatch, kind):
+    """The tower kernel in each shape (Precision float16) against the layer-by-layer Precision float32 network: same
+    weights, fp16 tolerance."""
+    kn = nets(kind)
+    x = nh.inputs(kn.arch, 6, 3)
+    f16 = nh.check_tower_shapes(kn, x, monkeypatch)
+    f32 = nh.predict(kn.net(6, P32), kn.arch, x)
+    np.testing.assert_allclose(f16.value, f32.value, atol=nh.VALUE_ATOL)
+    np.testing.assert_allclose(f16.prob, f32.prob, rtol=nh.PROB_RTOL, atol=1e-6)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,cin,pch", [("risev2", 34, 81), ("risev33", 52, 76)])
-def test_tower_variants_are_bit_identical(tmp_path, monkeypatch, name, cin, pch):
-    """The tower kernel's two shapes (one / two boards per CTA) must give the same bits: a search with many trees evaluates
-    the same positions in bigger batches.  At 140 boards the default is two boards per CTA."""
-    arch = onet.arch_risev2(cin, pch) if name == "risev2" else onet.arch_risev33(cin, pch, True)
-    for n, variants in ((5, [{"ARA_TRUNK_ROWS": "128"}, {"ARA_TRUNK_ROWS": "64"}]),
-                        (64, [{"ARA_TRUNK_ROWS": "128"}, {"ARA_TRUNK_ROWS": "64"}]),
-                        (140, [{}, {"ARA_TRUNK_ROWS": "64"}])):
-        x = golden_input(arch, n=n, seed=11)
-        outs = []
-        for env in variants:
-            monkeypatch.delenv("ARA_TRUNK_ROWS", raising=False)
-            for k, v in env.items():
-                monkeypatch.setenv(k, v)
-            net, _ = _make_net(tmp_path, arch, n, 10 if name == "risev2" else 30)
-            v, p = np.zeros(n, np.float32), np.zeros((n, pch * 64), np.float32)
-            for _ in range(3):  # (repeated: a race in the weight ring would not show every time)
-                net.predict(x, v, p, None, n=n)
-                outs.append((v.copy(), p.copy()))
-            net.close()
-        for v, p in outs[1:]:
-            assert np.array_equal(v, outs[0][0]) and np.array_equal(p, outs[0][1])
+@pytest.mark.parametrize("kind", ["risev2", "risev33"], ids=["risev2-34-81", "risev33-52-76"])
+def test_tower_variants_are_bit_identical(nets, monkeypatch, kind):
+    """The tower kernel's shapes must give the same bits: a search with many trees evaluates the same positions in
+    bigger batches.  At 140 boards (more than the SMs) the default is two boards per CTA."""
+    kn = nets(kind)
+    for n, rows in ((5, ("32", "64", "128")), (64, ("32", "64", "128")), (140, ("64", "128"))):
+        nh.check_tower_shapes(kn, nh.inputs(kn.arch, n, 11), monkeypatch, rows, repeats=3)

@@ -8,7 +8,7 @@ from crazyara_b200.onnx_import import import_onnx
 from crazyara_b200.weights import export_mx_blob
 from oracle import net_mx
 from tests.onnx_mx_writer import write_mx_onnx
-from tests.test_net_mx_gpu import mixed_arch
+from tests.net_harness import mixed_arch
 
 ARCHS = {"mx_risev2": lambda: net_mx.arch_mx_risev2(34, 81), "mx_risev33": lambda: net_mx.arch_mx_risev33(52, 76),
          "mx_mixed": mixed_arch}
