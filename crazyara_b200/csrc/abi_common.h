@@ -1,5 +1,6 @@
 // Shared host-side plumbing for the C-ABI: last-error string, CUDA error checks, device buffers, graph capture.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdarg>
 #include <cstdio>
@@ -40,6 +41,39 @@ class DeviceBuffers {
 
    private:
     std::vector<void*> ptrs_;
+};
+
+// Owner of device memory that is reserved as a virtual address range and mapped piece by piece as it is needed (the
+// CUDA virtual memory management calls, reached through cudaGetDriverEntryPoint).  An array placed in a reserved range
+// keeps its address for the range's life while memory is mapped in behind it, so pointers held by the device and by
+// captured graphs stay valid.  Every mapped piece is zero-filled on the given stream before any later work on that
+// stream can reach it.  Reservations and mappings are released with the owner, on every return path.
+class DeviceRanges {
+   public:
+    DeviceRanges() = default;
+    ~DeviceRanges();
+    DeviceRanges(const DeviceRanges&) = delete;
+    DeviceRanges& operator=(const DeviceRanges&) = delete;
+    // the mapping granularity of `device` (every reservation and piece is a multiple of it)
+    int init(int device);
+    size_t granularity() const { return gran_; }
+    int reserve(size_t bytes, CUdeviceptr* base);
+    // maps [at, at + bytes) (multiples of the granularity, inside a reservation); 1: the device has not that much free
+    // memory (nothing mapped, no error set)
+    int map(CUdeviceptr at, size_t bytes, cudaStream_t zero_on);
+    // unmaps and releases every piece inside [lo, hi); the caller makes sure the device no longer reads it
+    void unmap(CUdeviceptr lo, CUdeviceptr hi);
+
+   private:
+    struct Piece {
+        CUdeviceptr at;
+        size_t bytes;
+        CUmemGenericAllocationHandle h;
+    };
+    std::vector<Piece> pieces_;
+    std::vector<Piece> reserved_;  // (h unused)
+    int device_ = 0;
+    size_t gran_ = 0;
 };
 
 // Captures the work enqueue() (0 or -1 with the error set) puts on stream s into *exec.

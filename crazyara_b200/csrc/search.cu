@@ -18,6 +18,7 @@
 #include <cmath>
 #include <cstring>
 #include <memory>
+#include <type_traits>
 #include <vector>
 
 #include "abi_common.h"
@@ -74,11 +75,17 @@ struct TreeLimits {
 // there keeps the next tower from it.  Each CTA also takes kSmemReservedPerCta of the SM's shared memory.
 constexpr int kSmemPerSm = 233472, kSmemReservedPerCta = 1024;
 constexpr int kSmemBesideTower = kSmemPerSm - kTrunkPairSmemBytes - kSmemReservedPerCta;
+// A tree whose pools are mapped as it grows stops growing where a mapping would leave the device less than this much
+// free memory: room kept for the network's buffers and graphs, a second handle (Threads 2, a match) and whatever else
+// shares the GPU.  A chosen margin, not a measured one.
+constexpr size_t kFreeMemoryMargin = size_t(4) << 30;
 static_assert(sizeof(ExpandScratch) + kSmemReservedPerCta <= kSmemBesideTower, "expand_kernel no longer fits beside a tower CTA");
 static_assert(2 * (sizeof(UpdateScratch) + kSmemReservedPerCta) <= kSmemBesideTower, "two update_kernel CTAs no longer fit beside a tower CTA");
 static_assert(sizeof(WarpScratch) + kSmemReservedPerCta <= kSmemBesideTower, "select_kernel no longer fits beside a tower CTA");
 
-__global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const TreeLimits* limits) {
+// room: -1, the pools' own test of room for another search on top of a kept subtree (reuse_root); else the host's verdict
+__global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchParams sp, const Board* roots, const TreeLimits* limits,
+                                                 int room) {
     __shared__ WarpScratch ws;
     const TreeDev t = trees[blockIdx.x];
     const TreeLimits lim = limits[blockIdx.x];
@@ -87,7 +94,8 @@ __global__ void __launch_bounds__(32) root_kernel(const TreeDev* trees, SearchPa
         return;
     }
     // the subtree kept by ara_search_apply_move is searched on if it is this position, else a new tree starts
-    if (!reuse_root(t, sp, &roots[blockIdx.x])) create_root(t, sp, ws, &roots[blockIdx.x]);
+    const bool reused = room < 0 ? reuse_root(t, sp, &roots[blockIdx.x]) : reuse_root(t, sp, &roots[blockIdx.x], room != 0);
+    if (!reused) create_root(t, sp, ws, &roots[blockIdx.x]);
     __syncwarp();
     if (threadIdx.x == 0) {
         t.st->limit_simulations = lim.simulations;
@@ -106,15 +114,16 @@ __global__ void __launch_bounds__(32) advance_kernel(const TreeDev* trees, int t
 // A kept subtree lives wherever its nodes were allocated: after a few searches the pools are full of the dead siblings
 // of the moves that were played, and reuse_root would have to start a new tree.  Instead the subtree behind the new
 // root is copied to the front of a second set of pools (node ids and edge ranges keep their relative order, so the new
-// root becomes node 0), the pool pointers are swapped and the search goes on with every statistic it had.
+// root becomes node 0), the pool pointers are swapped and the search goes on with every statistic it had.  Pools mapped
+// as the tree grows compact every kept subtree, and then give back what the old set held.
 struct CompactInfo {
-    int need;    // the kept subtree is the searched position but the pools have no room left for another search
+    int need;    // the kept subtree is the searched position and (always, or) the pools have no room left for another search
     int cand;    // its root
     int n_nodes, n_edges;
 };
 // (an idle tree is not searched in this go, and its roots[] entry may be stale: it is left alone)
 __global__ void __launch_bounds__(32) compact_decide_kernel(const TreeDev* trees, SearchParams sp, const Board* roots,
-                                                            const TreeLimits* limits, CompactInfo* info) {
+                                                            const TreeLimits* limits, int always, CompactInfo* info) {
     if (threadIdx.x != 0) return;
     const TreeDev t = trees[blockIdx.x];
     const int cand = limits[blockIdx.x].active ? kept_subtree_root(t, &roots[blockIdx.x]) : -1;
@@ -122,7 +131,7 @@ __global__ void __launch_bounds__(32) compact_decide_kernel(const TreeDev* trees
     c.cand = cand;
     c.n_nodes = t.st->n_nodes;
     c.n_edges = t.st->n_edges;
-    c.need = cand >= 0 && !pools_have_room(sp, t.max_nodes, t.max_edges, c.n_nodes, c.n_edges);
+    c.need = cand >= 0 && (always || !pools_have_room(sp, t.max_nodes, t.max_edges, c.n_nodes, c.n_edges));
     info[blockIdx.x] = c;
 }
 // keep_n[i] = 1 if node i lies in the subtree of `cand`, keep_e[i] = its number of edges then
@@ -354,6 +363,16 @@ __global__ void fake_eval_kernel(const TreeDev* trees, int n_trees, int batch, f
     for (int i = threadIdx.x; i < n_labels; i += blockDim.x) probs[static_cast<size_t>(slot) * n_labels + i] = fake_prob(key, i);
 }
 
+// Room for another search on top of a kept subtree of n_nodes / n_edges in pools that grow with the tree: the subtree
+// takes at most half of the reservation, its nodes and its edges measured separately.  (pools_have_room sizes a
+// budget-less search by half the nodes times the per-node edge bound, more edges than a reservation sized by the
+// device's memory has: those are capped at 2^31 - 1.)
+static bool growing_pools_have_room(const SearchParams& sp, long long max_nodes, long long max_edges, long long n_nodes,
+                                    long long n_edges) {
+    const long long slack = 4LL * sp.batch_size + 64;
+    return n_nodes + slack <= max_nodes / 2 && n_edges + slack * pool_edge_bound(sp) <= max_edges / 2;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 class Search {
    public:
@@ -369,6 +388,7 @@ class Search {
     int fetch_results();
     int apply_move(int tree, unsigned short move);
     int node_view(int tree, int node_id, NodeView* out);
+    int pool_info(int tree, ara_search_pool_t* out);
     void request_stop() { stop_requested_.store(true, std::memory_order_relaxed); }
     int debug_cycles(int tree, unsigned long long* out8) {
         TreeState st;
@@ -381,6 +401,7 @@ class Search {
     std::vector<SearchResult> results;
     long long launches = 0;  // kernels launched so far, each counted by launch() (bench bookkeeping)
     long long compactions = 0;
+    long long grows = 0;  // times the pools of a growing tree were mapped further
     long long net_forwards = 0;
     double last_go_ms = 0.0;
     double movetime_ms = 0.0;  // > 0: stop issuing iterations once this much wall time has passed (UCI `go movetime`)
@@ -411,15 +432,19 @@ class Search {
         long long search_launches = 0, net_launches = 0;
     };
 
-    // The arrays of TreeDev, listed once: f(member, length) for each.  A tree's node, edge and prepared-child pools
-    // (the compaction swaps them for its second set) ...
+    // The arrays of TreeDev, listed once.  A tree's node, edge and prepared-child pools (the compaction swaps them for
+    // its second set): f(member, entries per node or edge, is an edge array) for each ...
+    static constexpr int kPoolArrays = 13;
     template <typename F>
-    void for_each_pool(F&& f) const {
-        const size_t nodes = max_nodes_, edges = max_edges_, slots = nodes * kPrepSlots;
-        f(&TreeDev::hdr, nodes), f(&TreeDev::board, nodes);
-        f(&TreeDev::P, edges), f(&TreeDev::Q, edges), f(&TreeDev::N, edges), f(&TreeDev::child, edges), f(&TreeDev::cbase, edges);
-        f(&TreeDev::move, edges), f(&TreeDev::vl, edges), f(&TreeDev::etype, edges);
-        f(&TreeDev::prep_board, slots), f(&TreeDev::prep_ci, slots), f(&TreeDev::prep_term, slots);
+    static void for_each_pool(F&& f) {
+        f(&TreeDev::hdr, 1, false), f(&TreeDev::board, 1, false);
+        f(&TreeDev::P, 1, true), f(&TreeDev::Q, 1, true), f(&TreeDev::N, 1, true), f(&TreeDev::child, 1, true), f(&TreeDev::cbase, 1, true);
+        f(&TreeDev::move, 1, true), f(&TreeDev::vl, 1, true), f(&TreeDev::etype, 1, true);
+        f(&TreeDev::prep_board, kPrepSlots, false), f(&TreeDev::prep_ci, kPrepSlots, false), f(&TreeDev::prep_term, kPrepSlots, false);
+    }
+    template <typename T>
+    static size_t entry_bytes(T* TreeDev::*) {
+        return sizeof(T);
     }
     // ... and the batch arrays of one view of a tree (Threads = 2: each logical thread's view has its own)
     template <typename F>
@@ -429,11 +454,28 @@ class Search {
         f(&TreeDev::traj_node, traj), f(&TreeDev::traj_ci, traj), f(&TreeDev::traj_edge, traj);
         f(&TreeDev::traj_len, 2 * B), f(&TreeDev::traj_start, 2 * B);
     }
-    int alloc_pools(TreeDev& t) {
-        int rc = 0;
-        for_each_pool([&](auto m, size_t n) { rc = rc ? rc : mem_.dalloc(&(t.*m), n); });
-        return rc;
+    // One tree's set of pools: a reserved address range that holds every pool array at pool_off_, and what is mapped of
+    // each.  A handle with a visit budget, or of several trees, packs the arrays and maps the whole set at once; one tree
+    // without a budget (grow_) gives each array room for the reservation, in whole granules, and maps it as it grows.
+    struct PoolSet {
+        CUdeviceptr base = 0;  // 0: not reserved yet
+        size_t mapped[kPoolArrays] = {};
+        int nodes = 0, edges = 0;  // the capacity mapped: TreeDev::max_nodes / max_edges of the tree living in the set
+        long long bytes() const {
+            long long b = 0;
+            for (size_t m : mapped) b += static_cast<long long>(m);
+            return b;
+        }
+    };
+    void point_at(TreeDev& t, const PoolSet& p) const {
+        int i = 0;
+        for_each_pool([&](auto m, size_t, bool) { t.*m = reinterpret_cast<std::remove_reference_t<decltype(t.*m)>>(p.base + pool_off_[i++]); });
     }
+    int reserve_pools(PoolSet& p) { return vm_.reserve(pool_span_, &p.base); }
+    int map_pools(PoolSet& p, long long nodes, long long edges);
+    int grow_pools(PoolSet& p, long long nodes, long long edges);
+    int release_pools(PoolSet& p);
+    int map_ahead(int batches);
     int alloc_batch_arrays(TreeDev& t) {
         int rc = 0;
         for_each_batch_array([&](auto m, size_t n) { rc = rc ? rc : mem_.dalloc(&(t.*m), n); });
@@ -479,9 +521,16 @@ class Search {
     bool searched_ = false;  // a go has run: the device holds trees that apply_move may keep
     // UCI `stop` (SearchThread::stop): set from another host thread while go() runs; go() leaves its loop at the next poll
     std::atomic<bool> stop_requested_{false};
+    // the pools' size: what a budget needs, or the cap (max_nodes) of a growing tree, or what the device's memory holds
     int max_nodes_ = 0, max_edges_ = 0, n_labels_ = 0, hist_cap_ = 512;
     int cin_pad_ = 0, split_ = 0;  // the network input's rows (expand_kernel)
     DeviceBuffers mem_;
+    DeviceRanges vm_;  // the pools' reservations and mappings
+    bool grow_ = false;  // one tree without a visit budget: its pools are mapped as the tree grows (map_ahead)
+    size_t pool_off_[kPoolArrays] = {}, pool_span_ = 0;  // where each pool array lies in a set's range, its length
+    std::vector<PoolSet> live_, spare_;  // per tree: the set the tree lives in, and compaction's second set
+    long long used_nodes_ = 0, used_edges_ = 0;  // grow_: the tree's entries in use (exact after each poll), or a bound
+    bool grow_room_ = true;  // grow_: a kept subtree was compacted (or there is none), so the next go may search on it
     Slot slots_[2];
     cudaStream_t stream_ = nullptr;
     bool own_stream_ = false;
@@ -498,10 +547,12 @@ class Search {
     bool warm_ = false;  // iterations and turns may be captured from now on (run_captured)
     Captured iter_graph_;        // Threads = 1: an iteration
     Captured turn_graph_[2][2];  // Threads = 2: a turn [slot][with update]
-    // node-pool compaction: the second set of pools per tree (allocated at the first compaction), scan scratch
+    // node-pool compaction: the second set of pools per tree (reserved and mapped at its first use), scan scratch
     std::vector<TreeDev> shadow_;
     std::vector<char> advanced_;  // ara_search_apply_move since the last go
     CompactInfo* d_cinfo_ = nullptr;
+    CUdeviceptr keep_base_ = 0;  // d_keep_n_ and d_keep_e_, room for max_nodes_ + 1 entries each, mapped for the nodes in use
+    size_t keep_span_ = 0, keep_mapped_ = 0;
     int* d_keep_n_ = nullptr;
     int* d_keep_e_ = nullptr;
     int* d_ctotal_ = nullptr;
@@ -632,19 +683,47 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
         if (mem_.dalloc(&s0.values, static_cast<size_t>(n_trees) * sp.batch_size)) return -1;
         if (mem_.dalloc(&s0.probs, static_cast<size_t>(n_trees) * sp.batch_size * n_labels_)) return -1;
     }
+    if (vm_.init(device_)) return -1;
+    const unsigned budget = sp.simulations ? sp.simulations : (sp.nodes ? sp.nodes * 2 : 0);
+    // Without a visit budget a single tree's pools are reserved for max_nodes (a cap), or for what the device's memory
+    // could hold, and mapped as the tree grows.  Trees of a handle of several only grow within pools mapped whole.
+    grow_ = budget == 0 && n_trees == 1;
+    bool device_sized = false;
     if (max_nodes <= 0) {
-        const unsigned budget = sp.simulations ? sp.simulations : (sp.nodes ? sp.nodes * 2 : 0);
-        if (budget == 0) return set_error("ara_search_create: max_nodes must be given when neither Simulations nor Nodes is set");
-        max_nodes = static_cast<int>(budget) + 4 * sp.batch_size * sp.threads + 64;
+        if (budget != 0) {
+            max_nodes = static_cast<int>(budget) + 4 * sp.batch_size * sp.threads + 64;
+        } else if (n_trees > 1) {
+            return set_error("ara_search_create: %d trees without Simulations or Nodes need max_nodes: only a single tree's pools "
+                             "grow to what the device's memory holds", n_trees);
+        } else {  // the node arrays for what the device's memory could hold; the edges are bounded by their int32 indices
+            size_t free_b = 0, total_b = 0;
+            ARA_CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+            size_t per_node = 0;
+            for_each_pool([&](auto m, size_t per, bool edge) { per_node += edge ? 0 : entry_bytes(m) * per; });
+            max_nodes = static_cast<int>(std::min<size_t>(total_b / per_node, 2147483647u / 2));
+            device_sized = true;
+        }
     }
     max_nodes_ = max_nodes;
     // edge pool: average legal moves per node is ~35 (chess) but drop-heavy crazyhouse positions reach 200-300
     {
         // sized for the worst case per node; computed in 64 bits: 2^24 nodes x 320 edges does not fit an int
-        const long long want = static_cast<long long>(max_nodes) * (sp.mode == MODE_CHESS ? 128 : 320) + 1024;
+        long long want = static_cast<long long>(max_nodes) * pool_edge_bound(sp) + 1024;
+        if (device_sized) want = std::min(want, 2147483647LL);
         if (want > 2147483647LL)
             return set_error("ara_search_create: a pool of %d nodes needs %lld edge slots (more than 2^31 - 1); lower max_nodes", max_nodes, want);
         max_edges_ = static_cast<int>(want);
+    }
+    {   // where each pool array lies in a set's range
+        const size_t g = vm_.granularity(), align = grow_ ? g : 512;
+        size_t off = 0;
+        int i = 0;
+        for_each_pool([&](auto m, size_t per, bool edge) {
+            pool_off_[i++] = off;
+            const size_t bytes = entry_bytes(m) * per * static_cast<size_t>(edge ? max_edges_ : max_nodes_);
+            off += (bytes + align - 1) / align * align;
+        });
+        pool_span_ = (off + g - 1) / g * g;
     }
     const int B = sp.batch_size;
     // cput look-up table with the HOST libm: bit-identical to the reference's scalar code (node.cpp:1243-1246)
@@ -666,17 +745,27 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     d_states_.resize(n_trees);
     d_hist_keys_.resize(n_trees);
     d_hist_reps_.resize(n_trees);
+    live_.resize(n_trees);
+    spare_.resize(n_trees);
     for (int i = 0; i < n_trees; ++i) {
         TreeDev& t = s0.h_trees[i];
-        if (alloc_pools(t) || alloc_batch_arrays(t) || mem_.dalloc(&t.st, 1)) return -1;
+        PoolSet& p = live_[i];
+        // (a growing tree starts with what its root and its first mini-batches need; map_ahead grows it from there)
+        if (reserve_pools(p) || grow_pools(p, 4LL * (3 * sp.batch_size + 8), 4LL * (3 * sp.batch_size + 8) * pool_edge_bound(sp)))
+            return -1;
+        if (p.nodes == 0)
+            return set_error("ara_search_create: less than %zu GiB of device memory free beside the first mapping of a growing "
+                             "pool", kFreeMemoryMargin >> 30);
+        point_at(t, p);
+        if (alloc_batch_arrays(t) || mem_.dalloc(&t.st, 1)) return -1;
         if (mem_.dalloc(&d_hist_keys_[i], hist_cap_) || mem_.dalloc(&d_hist_reps_[i], hist_cap_)) return -1;
         t.hist_keys = d_hist_keys_[i];
         t.hist_reps = d_hist_reps_[i];
         t.hist_len = 0;
         t.cput_lut = d_lut_;
         t.sqrt_lut = d_sqrt_lut_;
-        t.max_nodes = max_nodes_;
-        t.max_edges = max_edges_;
+        t.max_nodes = p.nodes;
+        t.max_edges = p.edges;
         t.slot_base = i * B;
         d_states_[i] = t.st;
     }
@@ -730,6 +819,100 @@ int Search::init(Net* net, const SearchParams& params, int device, int trees, in
     ARA_CUDA_OK(cudaMallocHost(&h_tstats_, sizeof(RootTimeStats)));
     ARA_CUDA_OK(cudaEventCreate(&ev0_));
     ARA_CUDA_OK(cudaEventCreate(&ev1_));
+    ARA_CUDA_OK(cudaStreamSynchronize(stream_));  // (the pools' zero fill)
+    grows = 0;
+    return 0;
+}
+
+// Maps `p` for `nodes` / `edges` entries (a set mapped whole: all of it).  1: the device has too little free memory
+// (nothing more is mapped past what fitted; capacity as before or in between), -1: error.
+int Search::map_pools(PoolSet& p, long long nodes, long long edges) {
+    if (!grow_) {
+        if (p.nodes > 0) return 0;
+        const int rc = vm_.map(p.base, pool_span_, stream_);
+        if (rc) return rc < 0 ? -1 : set_error("ara_search: out of device memory for %zu bytes of node and edge pools", pool_span_);
+        int i = 0;
+        for_each_pool([&](auto, size_t, bool) {
+            p.mapped[i] = (i + 1 < kPoolArrays ? pool_off_[i + 1] : pool_span_) - pool_off_[i];
+            ++i;
+        });
+        p.nodes = max_nodes_;
+        p.edges = max_edges_;
+        return 0;
+    }
+    const size_t g = vm_.granularity();
+    size_t want[kPoolArrays], extra = 0;
+    int i = 0;
+    for_each_pool([&](auto m, size_t per, bool edge) {
+        want[i] = (entry_bytes(m) * per * static_cast<size_t>(edge ? edges : nodes) + g - 1) / g * g;
+        if (want[i] > p.mapped[i]) extra += want[i] - p.mapped[i];
+        ++i;
+    });
+    if (extra == 0) return 0;
+    size_t free_b = 0, total_b = 0;
+    ARA_CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+    if (free_b < extra + kFreeMemoryMargin) return 1;
+    int rc = 0;
+    for (i = 0; i < kPoolArrays && rc == 0; ++i)
+        if (want[i] > p.mapped[i]) {
+            rc = vm_.map(p.base + pool_off_[i] + p.mapped[i], want[i] - p.mapped[i], stream_);
+            if (rc == 0) p.mapped[i] = want[i];
+        }
+    if (rc < 0) return -1;
+    // the capacity: what every array of its kind holds, within the reservation
+    long long n = max_nodes_, e = max_edges_;
+    i = 0;
+    for_each_pool([&](auto m, size_t per, bool edge) {
+        long long& c = edge ? e : n;
+        c = std::min(c, static_cast<long long>(p.mapped[i++] / (entry_bytes(m) * per)));
+    });
+    p.nodes = static_cast<int>(n);
+    p.edges = static_cast<int>(e);
+    ++grows;
+    return rc;
+}
+
+// `p` grown to hold `nodes` / `edges` entries (within the reservation): doubled at least, so that a tree of N nodes is
+// mapped in O(log N) steps, or where that does not fit beside kFreeMemoryMargin, just what is asked.  Where that does
+// not fit either the set stays as it is; the device's pool test then ends the search as a full pool ends it.
+int Search::grow_pools(PoolSet& p, long long nodes, long long edges) {
+    nodes = std::min<long long>(nodes, max_nodes_);
+    edges = std::min<long long>(edges, max_edges_);
+    if (nodes <= p.nodes && edges <= p.edges) return 0;
+    const long long gn = nodes > p.nodes ? std::min<long long>(max_nodes_, std::max(nodes, 2LL * p.nodes)) : p.nodes;
+    const long long ge = edges > p.edges ? std::min<long long>(max_edges_, std::max(edges, 2LL * p.edges)) : p.edges;
+    int rc = map_pools(p, gn, ge);
+    if (rc == 1) rc = map_pools(p, nodes, edges);
+    return rc < 0 ? -1 : 0;
+}
+
+// gives back all memory mapped for `p` (its reservation stays); the device must be done with it
+int Search::release_pools(PoolSet& p) {
+    ARA_CUDA_OK(cudaStreamSynchronize(stream_));
+    vm_.unmap(p.base, p.base + pool_span_);
+    for (size_t& m : p.mapped) m = 0;
+    p.nodes = p.edges = 0;
+    return 0;
+}
+
+// A growing tree, before `batches` more mini-batches (of all logical threads together) are enqueued: its pools cover
+// the entries in use plus what those mini-batches can add at most -- 3B + 8 nodes each (the slack of the device's pool
+// test), each node with the per-node edge bound -- and every view of the tree on the device has the new capacity.
+int Search::map_ahead(int batches) {
+    const long long add = static_cast<long long>(batches) * (3 * sp.batch_size + 8);
+    PoolSet& p = live_[0];
+    const int n0 = p.nodes, e0 = p.edges;
+    if (grow_pools(p, used_nodes_ + add, used_edges_ + add * pool_edge_bound(sp))) return -1;
+    used_nodes_ += add;  // (a bound until the next poll reads the counters)
+    used_edges_ += add * pool_edge_bound(sp);
+    if (p.nodes == n0 && p.edges == e0) return 0;
+    for (int k = 0; k < threads_; ++k) {
+        TreeDev& t = slots_[k].h_trees[0];
+        t.max_nodes = p.nodes;
+        t.max_edges = p.edges;
+        if (slots_[k].d_trees)  // (the two adjacent ints)
+            ARA_CUDA_OK(cudaMemcpyAsync(&slots_[k].d_trees[0].max_nodes, &t.max_nodes, 2 * sizeof(int), cudaMemcpyHostToDevice, stream_));
+    }
     return 0;
 }
 
@@ -855,6 +1038,7 @@ int Search::enqueue_turn(int k, bool with_update) {
 // S0 S1 (nothing to back up yet: the root's batch was applied by the root phase).  The handle is warm after its first
 // iteration (which warmed the network's graph up) or its first S0 S1.
 int Search::iterate(int count) {
+    if (grow_ && map_ahead(threads_ == 2 ? 2 * ((count + 1) / 2) : count)) return -1;
     if (threads_ == 2) {
         for (int c = 0; c < (count + 1) / 2; ++c) {
             if (enqueue_turn(0, primed_) || enqueue_turn(1, primed_)) return -1;
@@ -879,15 +1063,18 @@ int Search::compact_pools() {
     for (size_t i = 0; i < advanced_.size(); ++i)
         if (advanced_[i] && h_limits_[i].active) any = true, advanced_[i] = 0;  // (an idle tree's move waits for its next go)
     if (!any) return 0;
+    const size_t g = vm_.granularity();
     if (d_cinfo_ == nullptr) {
-        if (mem_.dalloc(&d_cinfo_, n_trees) || mem_.dalloc(&d_keep_n_, static_cast<size_t>(max_nodes_) + 1) ||
-            mem_.dalloc(&d_keep_e_, static_cast<size_t>(max_nodes_) + 1) || mem_.dalloc(&d_ctotal_, 2))
-            return -1;
+        if (mem_.dalloc(&d_cinfo_, n_trees) || mem_.dalloc(&d_ctotal_, 2)) return -1;
+        keep_span_ = ((static_cast<size_t>(max_nodes_) + 1) * sizeof(int) + g - 1) / g * g;
+        if (vm_.reserve(2 * keep_span_, &keep_base_)) return -1;
+        d_keep_n_ = reinterpret_cast<int*>(keep_base_);
+        d_keep_e_ = reinterpret_cast<int*>(keep_base_ + keep_span_);
         shadow_.resize(n_trees);
         for (auto& t : shadow_) t.hdr = nullptr;
     }
     Slot& s0 = slots_[0];
-    if (launch(compact_decide_kernel, n_trees, 32, 0, stream_, s0.d_trees, sp, d_roots_, d_limits_, d_cinfo_)) return -1;
+    if (launch(compact_decide_kernel, n_trees, 32, 0, stream_, s0.d_trees, sp, d_roots_, d_limits_, grow_ ? 1 : 0, d_cinfo_)) return -1;
     std::vector<CompactInfo> info(n_trees);
     ARA_CUDA_OK(cudaMemcpyAsync(info.data(), d_cinfo_, sizeof(CompactInfo) * n_trees, cudaMemcpyDeviceToHost, stream_));
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
@@ -895,6 +1082,16 @@ int Search::compact_pools() {
         const CompactInfo& c = info[i];
         if (!c.need || c.n_nodes <= 0) continue;
         TreeDev& t = s0.h_trees[i];
+        {   // the scan scratch, mapped for the nodes in use
+            const size_t want = ((static_cast<size_t>(c.n_nodes) + 1) * sizeof(int) + g - 1) / g * g;
+            if (want > keep_mapped_) {
+                const int rc0 = vm_.map(keep_base_ + keep_mapped_, want - keep_mapped_, stream_);
+                const int rc1 = rc0 ? rc0 : vm_.map(keep_base_ + keep_span_ + keep_mapped_, want - keep_mapped_, stream_);
+                if (rc1 < 0) return -1;
+                if (rc1) return set_error("ara_search: out of device memory for the compaction of %d nodes", c.n_nodes);
+                keep_mapped_ = want;
+            }
+        }
         if (launch(compact_mark_kernel, (c.n_nodes + 255) / 256, 256, 0, stream_, t, c.cand, c.n_nodes, d_keep_n_, d_keep_e_) ||
             launch(compact_scan_kernel, 1, 1024, 0, stream_, d_keep_n_, c.n_nodes, d_ctotal_) ||
             launch(compact_scan_kernel, 1, 1024, 0, stream_, d_keep_e_, c.n_nodes, d_ctotal_ + 1))
@@ -902,18 +1099,38 @@ int Search::compact_pools() {
         int total[2] = {0, 0};
         ARA_CUDA_OK(cudaMemcpyAsync(total, d_ctotal_, sizeof(total), cudaMemcpyDeviceToHost, stream_));
         ARA_CUDA_OK(cudaStreamSynchronize(stream_));
-        if (!pools_have_room(sp, max_nodes_, max_edges_, total[0], total[1])) continue;  // even the subtree alone is too big: new tree
+        // even the subtree alone is too big: new tree
+        if (!(grow_ ? growing_pools_have_room(sp, max_nodes_, max_edges_, total[0], total[1])
+                    : pools_have_room(sp, max_nodes_, max_edges_, total[0], total[1]))) {
+            grow_room_ = false;
+            continue;
+        }
         TreeDev& d = shadow_[i];
+        PoolSet& spare = spare_[i];
+        if (spare.base == 0 && reserve_pools(spare)) return -1;
+        if (grow_pools(spare, total[0], total[1])) return -1;
+        if (spare.nodes < total[0] || spare.edges < total[1]) {  // no device memory for the copy: a new tree
+            grow_room_ = false;
+            continue;
+        }
         if (d.hdr == nullptr) {
             d = t;
-            if (alloc_pools(d)) return -1;
+            point_at(d, spare);
         }
         if (launch(compact_gather_kernel, (c.n_nodes + 7) / 8, 256, 0, stream_, t, d, c.cand, c.n_nodes, d_keep_n_, d_keep_e_) ||
             launch(compact_finish_kernel, 1, 1, 0, stream_, t.st, total[0], total[1]))
             return -1;
         // swap the pools: the tree now lives in what was the second set
-        for_each_pool([&](auto m, size_t) { std::swap(t.*m, d.*m); });
+        for_each_pool([&](auto m, size_t, bool) { std::swap(t.*m, d.*m); });
+        std::swap(live_[i], spare_[i]);
+        t.max_nodes = live_[i].nodes;
+        t.max_edges = live_[i].edges;
         ++compactions;
+        if (grow_) {  // what the tree grows from now on is the subtree; the old set's memory goes back to the device
+            if (release_pools(spare_[i])) return -1;
+            used_nodes_ = total[0];
+            used_edges_ = total[1];
+        }
     }
     ARA_CUDA_OK(cudaGetLastError());
     ARA_CUDA_OK(cudaMemcpyAsync(s0.d_trees, s0.h_trees.data(), sizeof(TreeDev) * n_trees, cudaMemcpyHostToDevice, stream_));
@@ -934,7 +1151,9 @@ int Search::begin() {
     ARA_CUDA_OK(cudaMemcpyAsync(d_limits_, h_limits_.data(), sizeof(TreeLimits) * n_trees, cudaMemcpyHostToDevice, stream_));
     n_active_ = 0;
     for (const TreeLimits& l : h_limits_) n_active_ += l.active ? 1 : 0;
+    grow_room_ = true;
     if (compact_pools()) return -1;
+    if (grow_ && map_ahead(1)) return -1;  // the root phase: less than one mini-batch
     if (threads_ == 2) {  // the second thread's views of the trees: same pools, its own batch arrays
         Slot& s1 = slots_[1];
         for (int i = 0; i < n_trees; ++i) {
@@ -948,7 +1167,7 @@ int Search::begin() {
     }
     const int B = sp.batch_size;
     // root: create, expand, evaluate (set_root_node_predictions), scatter, prepare_node_for_visits (+ Dirichlet)
-    if (launch(root_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, d_roots_, d_limits_)) return -1;
+    if (launch(root_kernel, n_trees, 32, 0, stream_, s.d_trees, sp, d_roots_, d_limits_, grow_ ? (grow_room_ ? 1 : 0) : -1)) return -1;
     if (n_active_ == 0) {  // every tree idle: root_kernel has marked them done, nothing goes to the network
         ARA_CUDA_OK(cudaGetLastError());
         return 0;
@@ -971,12 +1190,14 @@ int Search::poll_running() {
     ARA_CUDA_OK(cudaStreamSynchronize(stream_));
     int running = 0;
     for (int i = 0; i < n_trees; ++i) running += h_done_[i] == 0;
-    if (running) {
+    if (running || grow_) {
         for (int i = 0; i < n_trees; ++i) {
             TreeState st;
             ARA_CUDA_OK(cudaMemcpy(&st, d_states_[i], sizeof(st), cudaMemcpyDeviceToHost));
-            if (st.error)
+            if (running && st.error)
                 return set_error("ara_search: device search error %d (1 node pool, 2 edge pool, 3 depth > %d)", st.error, kMaxDepth);
+            used_nodes_ = st.n_nodes;  // (grow_: one tree)
+            used_edges_ = st.n_edges;
         }
     }
     return running;
@@ -991,6 +1212,25 @@ int Search::step(int n_batches) {
     const int running = poll_running();
     if (running < 0 || fetch_results()) return -1;  // ara_search_result between steps shows the tree as it is now
     return running;
+}
+
+int Search::pool_info(int tree, ara_search_pool_t* out) {
+    if (tree < 0 || tree >= n_trees) return set_error("ara_search_pool: tree %d out of range", tree);
+    ARA_CUDA_OK(cudaSetDevice(device_));
+    TreeState st;
+    ARA_CUDA_OK(cudaStreamSynchronize(stream_));
+    ARA_CUDA_OK(cudaMemcpy(&st, d_states_[tree], sizeof(st), cudaMemcpyDeviceToHost));
+    out->nodes = st.n_nodes;
+    out->edges = st.n_edges;
+    out->mapped_nodes = live_[tree].nodes;
+    out->mapped_edges = live_[tree].edges;
+    out->cap_nodes = max_nodes_;
+    out->cap_edges = max_edges_;
+    out->mapped_bytes = live_[tree].bytes() + spare_[tree].bytes();
+    out->spare_bytes = spare_[tree].bytes();
+    out->grows = grows;
+    out->growing = grow_ ? 1 : 0;
+    return 0;
 }
 
 int Search::node_view(int tree, int node_id, NodeView* out) {
@@ -1203,6 +1443,11 @@ extern "C" int ara_search_step(ara_search_t h, int n_batches) {
 extern "C" int ara_search_node(ara_search_t h, int tree, int node_id, ara_node_view_t* out) {
     if (h == nullptr || out == nullptr) return ara::set_error("ara_search_node: null argument");
     return reinterpret_cast<Search*>(h)->node_view(tree, node_id, out);
+}
+
+extern "C" int ara_search_pool(ara_search_t h, int tree, ara_search_pool_t* out) {
+    if (h == nullptr || out == nullptr) return ara::set_error("ara_search_pool: null argument");
+    return reinterpret_cast<Search*>(h)->pool_info(tree, out);
 }
 
 extern "C" int ara_search_result(ara_search_t h, int tree, ara_search_result_t* out) {

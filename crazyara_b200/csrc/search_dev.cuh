@@ -1175,6 +1175,9 @@ ARA_HD void apply_tree_settings(TreeState& st, float q_value_weight, float diric
     if (dirichlet_epsilon >= 0) st.dirichlet_epsilon = dirichlet_epsilon;
 }
 
+// the most edges one node can have: the legal-move bound the edge pools are sized by (chess, else drop variants)
+ARA_HD int pool_edge_bound(const SearchParams& sp) { return sp.mode == 1 ? 128 : 320; }
+
 // run_search_thread loop condition (searchthread.cpp:326-340, :418-426), checked before every mini-batch.  True: this
 // thread makes no mini-batch now and its counters are cleared.  A thread whose condition fails leaves its loop for good,
 // like a returning run_search_thread; the search is over when the last thread has left.  Stores on lane 0.
@@ -1189,9 +1192,12 @@ ARA_HD bool thread_loop_ends(const TreeDev& t, const SearchParams& sp) {
     const uint32_t node_count = r.visit_sum - r.free_visits;
     const bool limits_ok = (st.limit_nodes == 0 || node_count < st.limit_nodes) &&
                            (st.limit_simulations == 0 || r.visit_sum < st.limit_simulations);
-    // (a pool sized for a visit budget can never trip the last test before the budget does; it only ends
-    // time-limited searches whose pool is exhausted before their time)
-    const bool pool_ok = st.n_nodes + 3 * sp.batch_size + 8 <= t.max_nodes;
+    // Room for another mini-batch: at most 3B + 8 new nodes, each with at most the per-node edge bound.  (A pool sized
+    // for a visit budget can never trip this before the budget does, and there the edge test follows from the node
+    // test.  It ends time-limited searches whose pools are full: at their size or cap, or, for pools mapped as the tree
+    // grows, where growth stopped short of the device's free memory.)
+    const int grow = 3 * sp.batch_size + 8;
+    const bool pool_ok = st.n_nodes + grow <= t.max_nodes && st.n_edges <= t.max_edges - grow * pool_edge_bound(sp);
     if (!(limits_ok && r.node_type == NT_UNSOLVED) || r.n_moves <= 1 || !pool_ok) {
         if (ARA_LANE == 0) {
             bs.done = 1;
@@ -1594,7 +1600,7 @@ ARA_HD bool pools_have_room(const SearchParams& sp, int max_nodes, int max_edges
     const unsigned limit = sp.simulations ? sp.simulations : sp.nodes;
     const unsigned budget = limit ? limit : static_cast<unsigned>(max_nodes / 2);
     return n_nodes + static_cast<long long>(budget) + 4 * sp.batch_size + 64 <= max_nodes &&
-           n_edges + (static_cast<long long>(budget) + 4 * sp.batch_size + 64) * (sp.mode == 1 ? 128 : 320) <= max_edges;
+           n_edges + (static_cast<long long>(budget) + 4 * sp.batch_size + 64) * pool_edge_bound(sp) <= max_edges;
 }
 // the candidate root of the next search (ara_search_apply_move) if it is the searched position and a playout node with
 // visits of its own, else -1
@@ -1606,10 +1612,12 @@ ARA_HD int kept_subtree_root(const TreeDev& t, const Board* root_board) {
     const bool ok = h.key == root_board->key && (h.flags & NF_HAS_D) && (h.flags & NF_HAS_NN) && h.visit_sum - h.free_visits > 0;
     return ok ? cand : -1;
 }
-ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* root_board) {
+// (room: whether the pools have room for another search on top of the subtree -- decided by the host for pools mapped
+// as the tree grows, which measure it against their reservation)
+ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* root_board, bool room) {
     TreeState& st = *t.st;
     const int cand = kept_subtree_root(t, root_board);
-    const int ok = cand >= 0 && pools_have_room(sp, t.max_nodes, t.max_edges, st.n_nodes, st.n_edges) ? 1 : 0;
+    const int ok = cand >= 0 && room ? 1 : 0;
     ARA_WARP_SYNC();
     if (ARA_LANE == 0) {
         st.next_root = -1;
@@ -1624,6 +1632,10 @@ ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* roo
     }
     ARA_WARP_SYNC();
     return ok;
+}
+
+ARA_HD int reuse_root(const TreeDev& t, const SearchParams& sp, const Board* root_board) {
+    return reuse_root(t, sp, root_board, pools_have_room(sp, t.max_nodes, t.max_edges, t.st->n_nodes, t.st->n_edges));
 }
 
 // The root phase of a tree left out of a go (ara_search_set_active), in place of reuse_root / create_root: the tree, its

@@ -46,6 +46,12 @@ class TimeReport(ctypes.Structure):
                 ("elapsed_ms", ctypes.c_double), ("value_eval", ctypes.c_float)]
 
 
+class SearchPool(ctypes.Structure):
+    _fields_ = [("nodes", ctypes.c_longlong), ("edges", ctypes.c_longlong), ("mapped_nodes", ctypes.c_longlong),
+                ("mapped_edges", ctypes.c_longlong), ("cap_nodes", ctypes.c_longlong), ("cap_edges", ctypes.c_longlong),
+                ("mapped_bytes", ctypes.c_longlong), ("spare_bytes", ctypes.c_longlong), ("grows", ctypes.c_longlong), ("growing", ctypes.c_int)]
+
+
 def early_stopping(tc, remaining_ms, node_count, max_q_is_max_visits, first_visits, second_visits, q_first, q_second):
     """ThreadManager::early_stopping as a pure function: 0 keep searching, 1 'max nodes' rule, 2 'cannot catch up' rule."""
     return _L().ara_time_early_stopping(ctypes.byref(tc), float(remaining_ms), int(node_count), int(max_q_is_max_visits),
@@ -136,6 +142,7 @@ def _L():
         L.ara_search_launch_count.argtypes = [vp]
         L.ara_search_compaction_count.restype = ctypes.c_longlong
         L.ara_search_compaction_count.argtypes = [vp]
+        L.ara_search_pool.argtypes = [vp, ci, vp]
         _SIGS = True
     return L
 
@@ -485,6 +492,13 @@ class MCTSAgent:
     def compaction_count(self):
         """kept subtrees moved to the front of the node pools so far (ara_search_compaction_count)"""
         return _L().ara_search_compaction_count(self._h)
+
+    def pool(self, tree=0):
+        """The tree's pools (ara_search_pool): nodes / edges in use, the capacity mapped, the reservation (cap), the device
+        bytes mapped for both sets, how often the handle's pools grew, and whether they grow with the tree."""
+        r = SearchPool()
+        check(_L().ara_search_pool(self._h, int(tree), ctypes.byref(r)))
+        return {n: getattr(r, n) for n, _ in SearchPool._fields_}
 
     def close(self):
         if getattr(self, "_h", None):

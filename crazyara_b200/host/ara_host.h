@@ -251,6 +251,12 @@ class MCTSAgent {
     }
     ~MCTSAgent() { ara_search_destroy(search_); }
     MCTSAgent(const MCTSAgent&) = delete;
+    // the tree's pools: nodes in use, capacity mapped, cap, device bytes (ara_search_pool)
+    ara_search_pool_t pool() const {
+        ara_search_pool_t p{};
+        if (ara_search_pool(search_, 0, &p) != 0) throw std::runtime_error(ara_last_error());
+        return p;
+    }
     void evaluate_board_state(const BoardState& state, EvalInfo& evalInfo) {
         ara_board_t root;
         const unsigned long long* keys = nullptr;

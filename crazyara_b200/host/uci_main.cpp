@@ -33,7 +33,7 @@ struct Options {
                                              {"MCTS_Solver", "true"},       {"Virtual_Style", "virtual_mix"},
                                              {"Virtual_Mix_Threshold", "1000"}, {"First_Device_ID", "0"},
                                              {"UCI_Chess960", "false"},     {"Input_Version", "0"},    {"Dirichlet_Seed", "42"},
-                                             {"Move_Overhead", "20"},       {"Timed_Search_Nodes", "1000000"},
+                                             {"Move_Overhead", "20"},       {"Timed_Search_Nodes", "0"},
                                              {"Reuse_Tree", "true"},           {"Use_NPS_Time_Manager", "true"},
                                              {"Precision", "float16"},      {"Use_Raw_Network", "false"},
                                              // the reference's defaults (optionsuci.cpp:89-90, :182); Threads 1 and both epsilons 0
@@ -56,7 +56,7 @@ int mode_of_variant(int variant) { return variant == 0 ? 1 : (variant == 1 ? 0 :
 // proportional system from move 35 with 14 moves to go, increment factor 0.7, safety buffer 30 x overhead
 struct GoLimits {
     long movetime = 0, time[2] = {0, 0}, inc[2] = {0, 0}, movestogo = 0;
-    bool infinite = false;  // `go infinite`: search until `stop` (or until the node pool is full)
+    bool infinite = false;  // `go infinite`: search until `stop` (or until the device's memory, or Timed_Search_Nodes, is used)
     bool any() const { return movetime || time[0] || time[1] || infinite; }
 };
 long time_for_move(const GoLimits& g, int me, int move_number, long overhead) {
@@ -113,9 +113,10 @@ int main() {
                                        opt.kv["Precision"]));
             rawAgent.reset(new RawNetAgent(net.get(), mode, s.input_version));
         }
-        // a time-limited search has no visit budget to size the node pool from
-        // a kept subtree lives in the same pools as the next search: room for a few searches, then the library compacts
-        // the subtree to the front of its second set of pools (ara_search_apply_move)
+        // a time-limited search has no visit budget: its pools grow with the tree, up to Timed_Search_Nodes nodes (0: as
+        // many as the device's memory holds); a kept subtree is compacted into fresh pools at the start of every search
+        // (ara_search_apply_move).  A budget sizes the pools: room for a few searches, then the library compacts the
+        // subtree to the front of its second set of pools.
         const long budget = s.simulations ? s.simulations : s.nodes;
         const int pool = timed ? opt.i("Timed_Search_Nodes")
                                : (opt.b("Reuse_Tree") ? static_cast<int>(std::min(8 * budget + 4L * s.batch_size + 64, 1L << 24)) : 0);

@@ -182,15 +182,23 @@ typedef struct ara_search_result_s {
 void ara_search_default_settings(ara_search_settings_t* s, int mode);
 /* net: handle whose batch size is >= n_trees * batch_size, or NULL to run the hash-derived fake backend (search-parity
  * tests).  n_trees independent positions are searched concurrently, one warp per tree, sharing each network batch.
- * max_nodes <= 0 sizes the node pool from the Simulations / Nodes limit. */
+ * Each tree's node, edge and prepared-child pools are reserved as device address ranges:
+ *   - with Simulations or Nodes set, max_nodes <= 0 sizes them from that budget, max_nodes > 0 gives their size; they are
+ *     mapped whole at creation;
+ *   - without either, one tree's pools are reserved for max_nodes > 0 (a cap: the search ends when the tree reaches it)
+ *     or, for max_nodes <= 0, for what the device's memory could hold (at most 2^31 - 1 edges), and mapped as the tree
+ *     grows, ahead of every chunk of mini-batches.  Growth stops at the reservation or where it would leave the device
+ *     less than a fixed margin of free memory; the search then ends as a full pool ends it, with its result.  Several
+ *     trees without a budget need max_nodes (their pools are mapped whole). */
 ara_search_t ara_search_create(ara_net_t net, const ara_search_settings_t* settings, int device, int n_trees, int max_nodes);
 void ara_search_destroy(ara_search_t s);
 /* root position of tree `tree` plus the (key, repetition) history of the game before it, oldest first */
 int ara_search_set_position(ara_search_t s, int tree, const ara_board_t* root, const unsigned long long* hist_keys,
                             const short* hist_reps, int hist_len);
 /* SearchLimits of the following go calls (searchlimits.h:37-61): simulations / nodes of tree `tree` (-1 = every tree)
- * instead of the settings' values.  The node pool is sized at creation, so the limits must stay within the budget the
- * handle was created for (ara_search_create max_nodes).  Self-play jitters the node budget of every search
+ * instead of the settings' values.  Pools mapped whole at creation hold what the handle was created for, so the limits
+ * must stay within that budget (ara_search_create max_nodes); pools that grow with the tree hold what their cap or the
+ * device's memory allows.  Self-play jitters the node budget of every search
  * (SelfPlay::adjust_node_count, rl/selfplay.cpp:146-152). */
 int ara_search_set_limits(ara_search_t s, int tree, unsigned simulations, unsigned nodes);
 /* The Q-value weight of the posterior (Centi_Q_Value_Weight / 100, 0..999.99) and the Dirichlet epsilon of the root
@@ -257,8 +265,9 @@ int ara_search_node(ara_search_t s, int tree, int node_id, ara_node_view_t* out)
  * (init_root_node / get_root_node_from_tree, :113-160) instead of starting a new tree -- provided the subtree's root is
  * that position, has been visited, and the node pool (ara_search_create max_nodes) has room for another search.  When
  * the dead siblings of the played moves have eaten that room, the kept subtree is first copied to the front of a second
- * set of pools (compaction; allocated at the first need), so a long game keeps its statistics as long as the subtree
- * itself plus one search fits.
+ * set of pools (compaction; mapped at the first need), so a long game keeps its statistics as long as the subtree
+ * itself plus one search fits.  Pools that grow with the tree compact every kept subtree at the start of the next go
+ * and give the old set's memory back: such a handle holds the kept subtree plus what one search adds.
  * `move` is the engine's 16-bit move code (ara_search_result_t.moves). */
 int ara_search_apply_move(ara_search_t s, int tree, unsigned short move);
 /* ThreadManager's time stop (manager/threadmanager.cpp, SearchLimits::movetime): ms > 0 makes the following go calls
@@ -310,6 +319,20 @@ long long ara_search_launch_count(ara_search_t s); /* search kernels launched so
 /* How often a kept subtree (ara_search_apply_move) was moved to the front of the node / edge pools because they had no
  * room left for another search on top of the dead siblings (instead of giving the tree up). */
 long long ara_search_compaction_count(ara_search_t s);
+/* The pools of one tree (ara_search_pool). */
+typedef struct {
+    long long nodes;        /* nodes in use */
+    long long edges;        /* edges in use */
+    long long mapped_nodes; /* node capacity mapped: the device's pool test ends a search that reaches it */
+    long long mapped_edges; /* edge capacity mapped */
+    long long cap_nodes;    /* the reservation: max_nodes, the budget's pool, or what the device's memory could hold */
+    long long cap_edges;
+    long long mapped_bytes; /* device memory mapped for the tree's pools, both sets */
+    long long spare_bytes;  /* of which the compaction's second set (0 after a growing tree's compaction) */
+    long long grows;        /* times pools of the handle were mapped further since its creation */
+    int growing;            /* 1: mapped as the tree grows; 0: mapped whole at creation */
+} ara_search_pool_t;
+int ara_search_pool(ara_search_t s, int tree, ara_search_pool_t* out);
 
 /* ---- debug / unit-test entries
  * ara_debug_conv: one wgmma convolution layer on caller-provided device buffers, built and launched as the network builds
