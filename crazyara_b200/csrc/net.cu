@@ -155,9 +155,16 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
         return set_error("ara_net_create: header flags stem_act %d policy_bias %d", hdr.stem_act, hdr.policy_bias);
     if (hdr.n_classic && hdr.policy_bias)
         return set_error("ara_net_create: ARAB2004 carries the policy convolution's bias with its head, not in the base header");
+    // the value head's kind: 0 standard, 1 WDL + plies (value P(win) - P(loss)), 2 the same feeding the value MLP, 3 / 4
+    // the MXNet symbols' head: a hidden layer of value_fc units (any base format) in front of the outputs of 1 / 2
+    const int kind = hdr.wdl_mode;
+    const bool mx_head = kind == kValueHeadMxWdl || kind == kValueHeadMxWdlMlp;
+    if (kind < kValueHeadStandard || kind > kValueHeadMxWdlMlp) return set_error("ara_net_create: value head of unknown kind %d", kind);
+    if (mx_head && (hdr.value_fc < 1 || hdr.value_fc > 256))
+        return set_error("ara_net_create: value head: hidden layer of %d units (1 .. 256)", hdr.value_fc);
     if (v3 ? (hdr.channels % 32 != 0 || hdr.channels < 64 || hdr.channels > 256 || hdr.value_channels != 8 || hdr.value_fc < 1 ||
               hdr.value_fc > 256)
-           : (hdr.channels != 256 || hdr.value_channels != 8 || hdr.value_fc != 256))
+           : (hdr.channels != 256 || hdr.value_channels != 8 || (hdr.value_fc != 256 && !mx_head)))
         return set_error("ara_net_create: unsupported trunk geometry (channels %d, value %d/%d)", hdr.channels,
                          hdr.value_channels, hdr.value_fc);
     if (hdr.n_blocks < 1 || hdr.n_blocks > 64) return set_error("ara_net_create: %d blocks (1 .. 64)", hdr.n_blocks);
@@ -233,8 +240,23 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
             !rd.tensor(hw->vh_bb, 1))
             return -1;
     } else {
-        if (!rd.tensor(hw->vh_a, 3 * 512) || !rd.tensor(hw->vh_ab, 3) || !rd.tensor(hw->vh_b, 512) || !rd.tensor(hw->vh_bb, 1))
+        const size_t hid = mx_head ? fc : 512;  // the features the WDL and plies outputs take
+        if (mx_head && (!rd.tensor(hw->vh_hid_w, static_cast<size_t>(fc) * 512) || !rd.tensor(hw->vh_hid_b, fc))) return -1;
+        if (!rd.tensor(hw->vh_a, 3 * hid) || !rd.tensor(hw->vh_ab, 3) || !rd.tensor(hw->vh_b, hid) || !rd.tensor(hw->vh_bb, 1))
             return -1;
+        if (kind == kValueHeadWdlMlp || kind == kValueHeadMxWdlMlp) {
+            long long count = 0;
+            if (!rd.read(&count, 8)) return set_error("ara_net_create: truncated value head");
+            if (count != 4 * kValueMlp)
+                return set_error("ara_net_create: value head: MLP of width %g (the trainers' MLP has %d)", count / 4.0, kValueMlp);
+            std::vector<float> w0(4 * kValueMlp), b0, w1, b1;
+            if (!rd.read(w0.data(), w0.size() * 4) || !rd.tensor(b0, kValueMlp) || !rd.tensor(w1, kValueMlp) || !rd.tensor(b1, 1))
+                return -1;
+            hw->vh_mlp = w0;
+            hw->vh_mlp.insert(hw->vh_mlp.end(), b0.begin(), b0.end());
+            hw->vh_mlp.insert(hw->vh_mlp.end(), w1.begin(), w1.end());
+            hw->vh_mlp.insert(hw->vh_mlp.end(), b1.begin(), b1.end());
+        }
     }
     if (!rd.tensor(hw->pol_w1, static_cast<size_t>(C) * C * 9) || !rd.tensor(hw->pol_b1, C) ||
         !rd.tensor(hw->pol_w2, static_cast<size_t>(hdr.policy_channels) * C * 9) ||
@@ -270,6 +292,11 @@ int Net::read_blob(const char* blob_path, HostWeights* hw) {
             pad3(&hw->vh_a, fc, 512, 1, 256, 512);
             pad3(&hw->vh_ab, fc, 1, 1, 256, 1);
             pad3(&hw->vh_b, fc, 1, 1, 256, 1);
+        } else if (mx_head) {  // zero hidden units: relu(0) = 0, and zero weights behind them
+            pad3(&hw->vh_hid_w, fc, 512, 1, 256, 512);
+            pad3(&hw->vh_hid_b, fc, 1, 1, 256, 1);
+            pad3(&hw->vh_a, 3, fc, 1, 3, 256);
+            pad3(&hw->vh_b, fc, 1, 1, 256, 1);
         }
         pad3(&hw->pol_w1, C, C, 9, 256, 256);
         pad3(&hw->pol_b1, C, 1, 1, 256, 1);
@@ -301,19 +328,24 @@ static void se_transposed(const BlockDesc& bd, const HostBlock& hb, std::vector<
 int Net::upload_value_head(const HostWeights& hw) {
     if (upload_f32(hw.vh_wv.data(), hw.vh_wv.size(), hw.vh_wv.size(), &vh_wv)) return -1;
     if (upload_f32(hw.vh_bv.data(), 8, 8, &vh_bv)) return -1;
-    if (!hdr.wdl_mode) {
-        std::vector<float> t2(512 * 256, 0.f);  // fc1 [256][512] -> [512][256]
+    // fc1 [256][512] -> [512][256]: the standard head's first layer, or the MXNet WDL heads' hidden layer value_fc0
+    auto upload_w1t = [&](const std::vector<float>& w, const std::vector<float>& b) {
+        std::vector<float> t2(512 * 256, 0.f);
         for (int o = 0; o < 256; ++o)
-            for (int i = 0; i < 512; ++i) t2[i * 256 + o] = hw.vh_a[o * 512 + i];
-        if (upload_f32(t2.data(), t2.size(), t2.size(), &vh_w1t)) return -1;
-        if (upload_f32(hw.vh_ab.data(), 256, 256, &vh_b1)) return -1;
+            for (int i = 0; i < 512; ++i) t2[i * 256 + o] = w[o * 512 + i];
+        return upload_f32(t2.data(), t2.size(), t2.size(), &vh_w1t) || upload_f32(b.data(), 256, 256, &vh_b1);
+    };
+    if (!hdr.wdl_mode) {
+        if (upload_w1t(hw.vh_a, hw.vh_ab)) return -1;
         if (upload_f32(hw.vh_b.data(), 256, 256, &vh_w2)) return -1;
         if (upload_f32(hw.vh_bb.data(), 1, 1, &vh_b2)) return -1;
     } else {
+        if (!hw.vh_hid_w.empty() && upload_w1t(hw.vh_hid_w, hw.vh_hid_b)) return -1;
         if (upload_f32(hw.vh_a.data(), hw.vh_a.size(), hw.vh_a.size(), &vh_wdl_w)) return -1;
         if (upload_f32(hw.vh_ab.data(), 3, 4, &vh_wdl_b)) return -1;
-        if (upload_f32(hw.vh_b.data(), 512, 512, &vh_plys_w)) return -1;
+        if (upload_f32(hw.vh_b.data(), hw.vh_b.size(), hw.vh_b.size(), &vh_plys_w)) return -1;
         if (upload_f32(hw.vh_bb.data(), 1, 1, &vh_plys_b)) return -1;
+        if (!hw.vh_mlp.empty() && upload_f32(hw.vh_mlp.data(), hw.vh_mlp.size(), hw.vh_mlp.size(), &vh_mlp)) return -1;
     }
     return 0;
 }
@@ -662,7 +694,7 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
         if (launch_conv(w.conv2, n, s)) return -1;
     }
     const float* xfinal = d_xf[hdr.n_blocks & 1];
-    ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
+    ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, vh_mlp, hdr.wdl_mode};
     if (launch(value_head_kernel<float>, dim3(n), dim3(256), value_head_smem<float>(), s, xfinal, vw, io_value[io], io_aux[io], cnt) ||
         launch_conv(pol_conv1, n, s, cnt) || launch_policy_head(n, s, cnt, io))
         return -1;
@@ -721,7 +753,7 @@ int Net::enqueue(int n, cudaStream_t s, bool from_f32, const int* cnt, int io, b
         if (st.ntb ? enqueue_ntb_half(blocks[st.block], ntbs_[st.index], n, s, cnt) : launch_tower(st.index, n, s, cnt)) return -1;
     }
     __half* xfinal = d_x[1];
-    ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, hdr.wdl_mode};
+    ValueHeadW vw{vh_wv, vh_bv, vh_w1t, vh_b1, vh_w2, vh_b2, vh_wdl_w, vh_wdl_b, vh_plys_w, vh_plys_b, vh_mlp, hdr.wdl_mode};
     // value head on the side stream (a second branch of the captured graph), policy head on s
     ARA_CUDA_OK(cudaEventRecord(ev_fork, s));
     ARA_CUDA_OK(cudaStreamWaitEvent(head_stream, ev_fork, 0));

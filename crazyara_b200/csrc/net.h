@@ -25,6 +25,9 @@ struct BlockDesc {
 // ARAB2002 block flags: the shortcut adds the block input before the squeeze-excitation; the ca_se fully-connected layers
 // have biases
 constexpr int kBlobShortcutPreSe = 1, kBlobSeBias = 2;
+// the base header's WDL word: the value head's kind (net_kernels.cuh value_head_kernel, weights.py VALUE_HEADS)
+constexpr int kValueHeadStandard = 0, kValueHeadWdl = 1, kValueHeadWdlMlp = 2, kValueHeadMxWdl = 3, kValueHeadMxWdlMlp = 4;
+constexpr int kValueMlp = 8;  // the hidden width of the trainers' value MLP on (WDL, plies)
 
 struct NetHeader {
     int in_channels;
@@ -33,7 +36,7 @@ struct NetHeader {
     int channels;        // 256 (ARAB2003: 64..256, zero padded to 256 at load)
     int value_channels;  // 8
     int value_fc;        // 256 (ARAB2003: <= 256, zero padded to 256 at load)
-    int wdl_mode;        // 1: value head with WDL + plys-to-end auxiliary outputs
+    int wdl_mode;        // the value head's kind (kValueHead*): WDL + plies-to-end auxiliary outputs from 1 on
     int input_version;   // e.g. 10 = v1.0, 30 = v3.0
     int stem_act;        // 1: ReLU behind the stem convolution (ARAB2001: always)
     int policy_bias;     // 1: the last policy convolution has a bias (ARAB2001: never)
@@ -65,6 +68,8 @@ struct HostWeights {
     std::vector<float> stem_w, stem_b;
     std::vector<HostBlock> blocks;
     std::vector<float> vh_wv, vh_bv, vh_a, vh_ab, vh_b, vh_bb;  // standard: fc1 / b1 / fc2 / b2; WDL: wdl w / b, plys w / b
+    std::vector<float> vh_hid_w, vh_hid_b;  // MXNet WDL heads: value_fc0 [value_fc][512], [value_fc]
+    std::vector<float> vh_mlp;              // value MLP: w0 [8][4] | b0 [8] | w1 [8] | b1 [1]
     std::vector<float> pol_w1, pol_b1, pol_w2, pol_b2;  // pol_b2: [policy_channels] when hdr.policy_bias or hdr.n_classic
     std::vector<float> fc_w, fc_b;                      // ARAB2004: [L][policy_channels * 64] (NCHW flatten), [L]
 };
@@ -185,7 +190,7 @@ class Net {
     float *d_yf = nullptr, *d_qkvf = nullptr, *d_zf = nullptr, *d_x2f = nullptr;
     __half *d_ys = nullptr, *d_atts = nullptr, *d_zs = nullptr, *d_gs = nullptr, *d_x2s = nullptr, *d_hs = nullptr;
     float *vh_wv = nullptr, *vh_bv = nullptr, *vh_w1t = nullptr, *vh_b1 = nullptr, *vh_w2 = nullptr, *vh_b2 = nullptr;
-    float *vh_wdl_w = nullptr, *vh_wdl_b = nullptr, *vh_plys_w = nullptr, *vh_plys_b = nullptr;
+    float *vh_wdl_w = nullptr, *vh_wdl_b = nullptr, *vh_plys_w = nullptr, *vh_plys_b = nullptr, *vh_mlp = nullptr;
     ConvLayer pol_conv1, pol_conv2;
     // fully-connected policy head (policy_fc.cuh): relu(conv2) as fp16 (float32: split) rows, one board per row, weights
     // [lp][K] with their tensor maps, bias, split-K partial sums.  Like d_logits, shared by both input / output sets: their

@@ -152,11 +152,16 @@ __global__ void __launch_bounds__(256) se_f32_kernel(float* __restrict__ x, __ha
 }
 
 // ---------------------------------------------------------------------------------------------
-// Value head.  One CTA (256 threads) per board.
+// Value head.  One CTA (256 threads) per board.  The kinds (wdl_mode, net.h kValueHead*):
 //   f[j*64+sq] = relu(sum_c x[sq][c] * wv[j][c] + bv[j])            (conv1x1 256->8 + BN folded, NCHW flatten)
-//   standard:  value = tanh(w2 . relu(W1 f + b1) + b2)               W1t: [512][256] (transposed)
-//   wdl+plys:  wdl = Ww f + bw (3), plys = sigmoid(wp . f + bp); value = -softmax(wdl)[0] + softmax(wdl)[2];
-//              aux = [wdl0, wdl1, wdl2, plys]
+//   0 standard:  value = tanh(w2 . relu(W1 f + b1) + b2)             W1t: [512][256] (transposed)
+//   1 wdl+plys:  wdl = Ww f + bw (3), plys = sigmoid(wp . f + bp); value = -softmax(wdl)[0] + softmax(wdl)[2];
+//                aux = [wdl0, wdl1, wdl2, plys] (the logits, as the PyTorch network outputs them)
+//   2 as 1, value = tanh(m1 . relu(M0 [wdl logits, plys] + c0) + c1)  (use_mlp_wdl_ply: M0 [8][4], m1 [8]); aux as 1
+//   3 MXNet:     g = relu(W1 f + b1) (value_fc0, zero-padded to 256 units, W1t as the standard head's), then 1 on g
+//                (Ww [3][256], wp [256]); aux = [softmax(wdl), plys] (the probabilities SoftmaxOutput outputs)
+//   4 as 3, value = the MLP of 2 on [softmax(wdl), plys]; aux as 3
+// Every kind's arithmetic after the convolution is fp32 and per board.
 struct ValueHeadW {
     const float* wv;   // [8][256]
     const float* bv;   // [8]
@@ -164,15 +169,67 @@ struct ValueHeadW {
     const float* b1;   // [256]
     const float* w2;   // [256]
     const float* b2;   // [1]
-    const float* wdl_w;   // [3][512]
+    const float* wdl_w;   // [3][512] (kinds 3 / 4: [3][256])
     const float* wdl_b;   // [3]
-    const float* plys_w;  // [512]
+    const float* plys_w;  // [512] (kinds 3 / 4: [256])
     const float* plys_b;  // [1]
+    const float* mlp;     // kinds 2 / 4: M0 [8][4] | c0 [8] | m1 [8] | c1 [1]
     int wdl_mode;
 };
 
 __device__ __forceinline__ float act_to_float(__half v) { return __half2float(v); }
 __device__ __forceinline__ float act_to_float(float v) { return v; }
+
+// relu(W1 f + b1) of thread t's unit: 512 L2-resident weight loads per thread, four independent chains, 16 loads in flight
+__device__ __forceinline__ float value_hidden_unit(const float* __restrict__ w1t, const float* __restrict__ b1, const float* f,
+                                                   int t) {
+    float h0 = __ldg(b1 + t), h1 = 0.0f, h2 = 0.0f, h3 = 0.0f;
+    const float* wp = w1t + t;
+#pragma unroll 4
+    for (int i = 0; i < 512; i += 4) {
+        h0 = fmaf(__ldg(wp + (i + 0) * 256), f[i + 0], h0);
+        h1 = fmaf(__ldg(wp + (i + 1) * 256), f[i + 1], h1);
+        h2 = fmaf(__ldg(wp + (i + 2) * 256), f[i + 2], h2);
+        h3 = fmaf(__ldg(wp + (i + 3) * 256), f[i + 3], h3);
+    }
+    const float h = (h0 + h1) + (h2 + h3);
+    return fmaxf(h, 0.0f);
+}
+
+// Kinds 2, 3 and 4 from the four outputs s_red (WDL logits, plies logit): *value and aux[0 .. 4).  Not inlined, so that
+// kind 1's code in the kernel, and with it its floating-point contractions, stays as it was.
+__device__ __noinline__ void value_wdl_finish(const float* s_red, int mode, const float* __restrict__ mlp, float* value,
+                                              float* aux) {
+    const float l0 = s_red[0], l1 = s_red[1], l2 = s_red[2];
+    const float m = fmaxf(l0, fmaxf(l1, l2));
+    const float e0 = expf(l0 - m), e1 = expf(l1 - m), e2 = expf(l2 - m);
+    const float inv = 1.0f / (e0 + e1 + e2);
+    const float plys = 1.0f / (1.0f + expf(-s_red[3]));
+    // what the network outputs as its WDL: PyTorch the logits, MXNet the SoftmaxOutput's probabilities
+    const bool mx = mode >= 3;
+    const float o0 = mx ? e0 * inv : l0, o1 = mx ? e1 * inv : l1, o2 = mx ? e2 * inv : l2;
+    if (mode == 3) {
+        *value = -e0 * inv + e2 * inv;
+    } else {  // the value MLP on (WDL, plies): 4 -> 8, ReLU, 8 -> 1, tanh
+        float v = __ldg(mlp + 48);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            float h = __ldg(mlp + 32 + j);
+            h = fmaf(__ldg(mlp + j * 4 + 0), o0, h);
+            h = fmaf(__ldg(mlp + j * 4 + 1), o1, h);
+            h = fmaf(__ldg(mlp + j * 4 + 2), o2, h);
+            h = fmaf(__ldg(mlp + j * 4 + 3), plys, h);
+            v = fmaf(__ldg(mlp + 40 + j), fmaxf(h, 0.0f), v);
+        }
+        *value = tanhf(v);
+    }
+    if (aux != nullptr) {
+        aux[0] = o0;
+        aux[1] = o1;
+        aux[2] = o2;
+        aux[3] = plys;
+    }
+}
 
 template <typename T>  // T = __half (Precision float16) or float (Precision float32)
 __global__ void __launch_bounds__(256) value_head_kernel(const T* __restrict__ x, ValueHeadW w,
@@ -182,7 +239,7 @@ __global__ void __launch_bounds__(256) value_head_kernel(const T* __restrict__ x
     constexpr int kPitch = 256 + 16 / static_cast<int>(sizeof(T));  // padded rows
     extern __shared__ __align__(16) uint8_t s_x_raw[];
     T* s_x = reinterpret_cast<T*>(s_x_raw);
-    __shared__ float s_wv[8 * 256];
+    __shared__ float s_wv[8 * 256];  // (kinds 3 / 4: then the hidden units g)
     __shared__ float s_f[512];
     __shared__ float s_red[8];
     pdl_wait();
@@ -209,19 +266,9 @@ __global__ void __launch_bounds__(256) value_head_kernel(const T* __restrict__ x
     }
     __syncthreads();
     const int warp = t >> 5, lane = t & 31;
-    if (!w.wdl_mode) {
-        // 512 L2-resident weight loads per thread: four independent chains, 16 loads in flight
-        float h0 = __ldg(w.b1 + t), h1 = 0.0f, h2 = 0.0f, h3 = 0.0f;
-        const float* wp = w.w1t + t;
-#pragma unroll 4
-        for (int i = 0; i < 512; i += 4) {
-            h0 = fmaf(__ldg(wp + (i + 0) * 256), s_f[i + 0], h0);
-            h1 = fmaf(__ldg(wp + (i + 1) * 256), s_f[i + 1], h1);
-            h2 = fmaf(__ldg(wp + (i + 2) * 256), s_f[i + 2], h2);
-            h3 = fmaf(__ldg(wp + (i + 3) * 256), s_f[i + 3], h3);
-        }
-        float h = (h0 + h1) + (h2 + h3);
-        h = fmaxf(h, 0.0f) * __ldg(w.w2 + t);
+    const int mode = w.wdl_mode;
+    if (!mode) {
+        float h = value_hidden_unit(w.w1t, w.b1, s_f, t) * __ldg(w.w2 + t);
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
         if (lane == 0) s_red[warp] = h;
@@ -232,27 +279,40 @@ __global__ void __launch_bounds__(256) value_head_kernel(const T* __restrict__ x
             value[b] = tanhf(s);
         }
     } else {
-        // warps 0..3 each reduce one 512-long dot product
+        const bool mx = mode >= 3;
+        const float* feat = s_f;
+        int nf = 512;
+        if (mx) {  // s_wv is free: every thread is past the convolution
+            s_wv[t] = value_hidden_unit(w.w1t, w.b1, s_f, t);
+            __syncthreads();
+            feat = s_wv;
+            nf = 256;
+        }
+        // warps 0..3 each reduce one dot product over the features
         if (warp < 4) {
-            const float* wr = (warp < 3) ? (w.wdl_w + warp * 512) : w.plys_w;
+            const float* wr = (warp < 3) ? (w.wdl_w + warp * nf) : w.plys_w;
             float s = 0.0f;
-            for (int i = lane; i < 512; i += 32) s = fmaf(__ldg(wr + i), s_f[i], s);
+            for (int i = lane; i < nf; i += 32) s = fmaf(__ldg(wr + i), feat[i], s);
 #pragma unroll
             for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
             if (lane == 0) s_red[warp] = s + ((warp < 3) ? __ldg(w.wdl_b + warp) : __ldg(w.plys_b));
         }
         __syncthreads();
         if (t == 0) {
-            const float l0 = s_red[0], l1 = s_red[1], l2 = s_red[2];
-            const float m = fmaxf(l0, fmaxf(l1, l2));
-            const float e0 = expf(l0 - m), e1 = expf(l1 - m), e2 = expf(l2 - m);
-            const float inv = 1.0f / (e0 + e1 + e2);
-            value[b] = -e0 * inv + e2 * inv;
-            if (aux != nullptr) {
-                aux[b * 4 + 0] = l0;
-                aux[b * 4 + 1] = l1;
-                aux[b * 4 + 2] = l2;
-                aux[b * 4 + 3] = 1.0f / (1.0f + expf(-s_red[3]));
+            if (mode == 1) {
+                const float l0 = s_red[0], l1 = s_red[1], l2 = s_red[2];
+                const float m = fmaxf(l0, fmaxf(l1, l2));
+                const float e0 = expf(l0 - m), e1 = expf(l1 - m), e2 = expf(l2 - m);
+                const float inv = 1.0f / (e0 + e1 + e2);
+                value[b] = -e0 * inv + e2 * inv;
+                if (aux != nullptr) {
+                    aux[b * 4 + 0] = l0;
+                    aux[b * 4 + 1] = l1;
+                    aux[b * 4 + 2] = l2;
+                    aux[b * 4 + 3] = 1.0f / (1.0f + expf(-s_red[3]));
+                }
+            } else {
+                value_wdl_finish(s_red, mode, w.mlp, value + b, aux != nullptr ? aux + b * 4 : nullptr);
             }
         }
     }

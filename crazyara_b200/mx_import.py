@@ -20,8 +20,10 @@ onnx_import._import_mxnet_graph reads an MXNet ONNX export, and shares its edge 
 reads -- per block the 1x1 expansion, the 3x3 / 5x5 depthwise kernel, ca_se or eca_se on the block input with the
 shortcut taken before it; the value head; a policy map or policy_bn1, activation, Flatten and FullyConnected onto a
 classic label list; every BatchNorm's eps and fix_gamma -- becomes the MXNet-named parameters and arch that
-export_mx_blob converts.  Refused by name, as no blob format holds them: sa_se / sm_se / cm_se / cbam blocks,
-use_extra_variant_input, the WDL and plies-to-end value head, and a fully-connected policy layer of another width.
+export_mx_blob converts.  The value head is the standard one or, with use_wdl and use_plys_to_end, the WDL and plies
+outputs behind value_fc0 with value = win - loss or the value MLP (use_mlp_wdl_ply).  Refused by name, as no blob format
+holds them: sa_se / sm_se / cm_se / cbam blocks, use_extra_variant_input, a value head with only one of the WDL and
+plies-to-end outputs, and a fully-connected policy layer of another width.
 """
 import ast
 import json
@@ -222,14 +224,12 @@ def _import_symbol(g, variables, arrays, blob_path, input_version, channels):
     vbn = g.one(vconv[0][2][0], "BatchNorm")
     take(vconv[0], "value_conv0"), take_bn(vbn, "value_bn0")
     fc0 = g.one(relu_out(vbn), "FullyConnected")
-    fcs = g.fwd(relu_out(fc0), "FullyConnected")
-    if len(fcs) != 1 or attr(fcs[0], "num_hidden") != 1:
-        g.fail("value head: WDL and plies-to-end outputs (use_wdl, use_plys_to_end) behind value_fc0; no blob format "
-               "holds that head (ARAB's WDL head has no hidden layer)")
-    take(fc0, "value_fc0"), take(fcs[0], "value_fc1")
+    take(fc0, "value_fc0")
+    value_head = _value_outputs(g, g.fwd(relu_out(fc0), "FullyConnected"), take, relu_out)
     vc, fc = int(params["value_conv0_weight"].shape[0]), int(params["value_fc0_weight"].shape[0])
-    if (vc, fc) != (8, 256):
-        g.fail(f"value head: {vc} channels and {fc} hidden units (ARAB2002 holds 8 and 256)")
+    if vc != 8 or (fc != 256 if value_head is None else not 1 <= fc <= 256):
+        g.fail(f"value head: {vc} channels and {fc} hidden units (the blob formats hold 8 and 256, or with WDL and "
+               f"plies-to-end outputs 1 .. 256 hidden units)")
     pbn = g.one(pconv[0][2][0], "BatchNorm")
     take(pconv[0], "policy_conv0"), take_bn(pbn, "policy_bn0")
     pc1 = g.one(relu_out(pbn), "Convolution")
@@ -237,7 +237,10 @@ def _import_symbol(g, variables, arrays, blob_path, input_version, channels):
     P = int(params["policy_conv1_weight"].shape[0])
     arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(params["stem_conv0_weight"].shape[1]),
                 policy_channels=P, channels=channels, kernels=kernels, se_types=se_types, se_gates=se_gates, c_ops=c_ops,
-                wdl=False, value_channels=vc, value_fc=fc, stem_act=stem_act, policy_bias="policy_conv1_bias" in params)
+                wdl=value_head is not None, value_channels=vc, value_fc=fc, stem_act=stem_act,
+                policy_bias="policy_conv1_bias" in params)
+    if value_head is not None:
+        arch["value_head"] = value_head
     # select_policy_from_plane=False (builder_util_symbol.py policy_head): policy_bn1, the activation, Flatten, policy_out
     bn1 = g.first(pc1[2][0], "BatchNorm")
     if bn1 is None and g.downstream(pc1[2][0], ("FullyConnected",)) is not None:
@@ -257,6 +260,43 @@ def _import_symbol(g, variables, arrays, blob_path, input_version, channels):
         arch.update(policy_bias=False, n_labels=int(L))  # (the convolution's bias is folded with policy_bn1)
     export_mx_blob(params, arch, blob_path, input_version_of(arch, input_version), eps=eps, fix_gamma=False)
     return arch
+
+
+def _value_outputs(g, fcs, take, relu_out):
+    """the value head's layers behind value_fc0 and its activation (builder_util_symbol.py value_head), the FullyConnected
+    nodes fcs there -> None for value_fc1 and tanh; with use_wdl and use_plys_to_end, the WDL layer (3 units) into its
+    SoftmaxOutput and value_plys_to_end_fc (1 unit) into a sigmoid, then "mx_wdl" for value = win - loss or "mx_wdl_mlp"
+    for the MLP (use_mlp_wdl_ply) value_wdl_ply_fc (8 units), activation, value_fc1, tanh on Concat(probabilities, plies)"""
+    attr = lambda nd, k, d=None: nd[3].get(k, d)
+    if len(fcs) == 1 and attr(fcs[0], "num_hidden") == 1:
+        take(fcs[0], "value_fc1")
+        return None
+    widths = sorted(attr(nd, "num_hidden") for nd in fcs)
+    if widths != [1, 3]:
+        g.fail(f"value head: fully-connected layers of {widths} units behind value_fc0 (value_fc1, or the WDL and "
+               f"plies-to-end layers)")
+    wdl, plys = sorted(fcs, key=lambda nd: -attr(nd, "num_hidden"))
+    sm = g.first(wdl[2][0], "SoftmaxOutput")
+    sig = g.first(plys[2][0], "Activation")
+    if sm is None or sig is None or attr(sig, "act_type") != "sigmoid":
+        g.fail("value head: WDL and plies-to-end layers behind value_fc0 without a SoftmaxOutput behind the first or a "
+               "sigmoid behind the second")
+    take(wdl, "wdl_out"), take(plys, "value_plys_to_end_fc")
+    m0 = g.downstream(sm[2][0], ("FullyConnected",))
+    if m0 is None:  # value = broadcast_add(-loss, win) of the split probabilities
+        if g.downstream(sm[2][0], ("SliceChannel", "split")) is None:
+            g.fail("value head: neither win - loss nor a value MLP behind the WDL output")
+        return "mx_wdl"
+    cat = g.back(m0[1][0], "Concat")
+    plys_out = lambda t: t == sig[2][0] or (g.prod.get(t, ("",))[0] == "LinearRegressionOutput" and g.prod[t][1][0] == sig[2][0])
+    if len(cat[1]) != 2 or cat[1][0] != sm[2][0] or not plys_out(cat[1][1]):
+        g.fail("value head: the value MLP does not take Concat(WDL probabilities, plies)")
+    m1 = g.one(relu_out(m0), "FullyConnected")
+    tanh = g.first(m1[2][0], "Activation")
+    if attr(m1, "num_hidden") != 1 or tanh is None or attr(tanh, "act_type") != "tanh":
+        g.fail("value head: the value MLP does not end in one unit and tanh")
+    take(m0, "value_wdl_ply_fc"), take(m1, "value_fc1")
+    return "mx_wdl_mlp"
 
 
 def _se(g, mul, x, i, take, p, n_eca):

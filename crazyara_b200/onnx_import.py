@@ -22,10 +22,15 @@ a classic label list; it is written as ARAB2004 around the base format.  Such a 
 ReLU, has another label count or another width is refused, as are a bias or a Relu behind a folded policy-map
 convolution and a policy_bn1 with no such layer behind it: no blob format holds them, and dropping them would change
 the network.
+The value head is the standard one, the WDL and plies-to-end layers (a torch export's WDL `Gemm` may feed the value MLP
+of use_mlp_wdl_ply: Concat(WDL logits, Sigmoid(plies)) -> Gemm -> Relu -> Gemm -> Tanh), or, in an MXNet export, every
+Gemm behind value_fc0's Relu: value_fc1, or the WDL layer into its Softmax and the plies layer into its Sigmoid, then
+win - loss (Split) or the value MLP on Concat(probabilities, plies) (crazyara_b200/weights.py VALUE_HEADS).
 
 PARITY UNPINNED: the reference tree holds no .onnx file and no `onnx` / `onnxsim` package is installed, so the readers are
 checked against files written by tests/onnx_writer.py, tests/onnx_mx_writer.py and tests/onnx_alphavile_writer.py
-(tests/onnx_classic_writer.py adds the fully-connected policy head to them).
+(tests/onnx_classic_writer.py adds the fully-connected policy head to them, tests/onnx_wdl_writer.py the value heads
+above).
 """
 import struct
 from collections import defaultdict
@@ -334,10 +339,15 @@ def _import_mxnet_graph(g, blob_path, input_version, channels):
     take(vconv[0], "value_conv0")
     take_bn(g.first(vconv[0][2][0], "BatchNormalization"), "value_bn0")
     g0 = g.downstream(vconv[0][2][0], ("Gemm", "MatMul"))
-    g1 = g0 and g.downstream(g0[2][0], ("Gemm", "MatMul"))
-    if g1 is None:
+    act = g0 and g.first(g0[2][0], "Relu")
+    behind = (g.fwd(act[2][0], "Gemm", True) or g.fwd(act[2][0], "MatMul", True)) if act is not None else []
+    if not behind:
         g.fail("value head: two fully-connected layers not found")
-    take(g0, "value_fc0"), take(g1, "value_fc1")
+    take(g0, "value_fc0")
+    value_head = _mx_value_outputs(g, behind, take)
+    fc = int(params["value_fc0_weight"].shape[0])
+    if value_head is not None and not 1 <= fc <= 256:
+        g.fail(f"value head: {fc} hidden units in front of the WDL and plies-to-end outputs (1 .. 256)")
     take(pconv[0], "policy_conv0")
     take_bn(g.first(pconv[0][2][0], "BatchNormalization"), "policy_bn0")
     pc1 = g.downstream(pconv[0][2][0], ("Conv",))
@@ -352,14 +362,71 @@ def _import_mxnet_graph(g, blob_path, input_version, channels):
         g.fail("policy head: a BatchNormalization behind the last policy convolution but no fully-connected layer")
     arch = dict(name=f"rise_{len(kernels)}b", semantics="mxnet", in_channels=int(g.weight(stem).shape[1]),
                 policy_channels=P, channels=channels, kernels=kernels,
-                se_types=se_types, se_gates=se_gates, c_ops=c_ops, wdl=False, value_channels=int(params["value_conv0_weight"].shape[0]),
-                value_fc=256, stem_act=stem_act, policy_bias="policy_conv1_bias" in params)
+                se_types=se_types, se_gates=se_gates, c_ops=c_ops, wdl=value_head is not None,
+                value_channels=int(params["value_conv0_weight"].shape[0]), value_fc=256, stem_act=stem_act,
+                policy_bias="policy_conv1_bias" in params)
+    if value_head is not None:
+        arch.update(value_head=value_head, value_fc=fc)
     if head is not None:  # the convolution's bias is folded with policy_bn1 into the head (ARAB2004)
         take_bn(bn1, "policy_bn1")
         params["policy_out_weight"], params["policy_out_bias"] = head
         arch.update(policy_bias=False, n_labels=int(head[0].shape[0]))
     export_mx_blob(params, arch, blob_path, input_version_of(arch, input_version), eps=eps, fix_gamma=False)
     return arch
+
+
+def _mx_value_outputs(g, fcs, take):
+    """the value head of an MXNet export behind value_fc0's Relu, whose Gemm nodes are fcs (builder_util_symbol.py
+    value_head) -> None for value_fc1 and Tanh; with use_wdl and use_plys_to_end, the WDL layer (3 units) into the
+    Softmax of its SoftmaxOutput and value_plys_to_end_fc (1 unit) into a Sigmoid, then "mx_wdl" for value = win - loss
+    (Split, Neg, Add) or "mx_wdl_mlp" for the MLP value_wdl_ply_fc (8 units), Relu, value_fc1, Tanh on
+    Concat(probabilities, plies).  All the Gemm nodes behind the Relu are read, so the node order does not matter."""
+    widths = sorted(int(g.weight(nd).shape[0]) for nd in fcs)
+    if widths == [1]:
+        take(fcs[0], "value_fc1")
+        return None
+    if widths != [1, 3]:
+        g.fail(f"value head: fully-connected layers of {widths} units behind value_fc0 (value_fc1, or the WDL and "
+               f"plies-to-end layers)")
+    wdl, plys = sorted(fcs, key=lambda nd: -int(g.weight(nd).shape[0]))
+    sm, sig = g.first(wdl[2][0], "Softmax"), g.first(plys[2][0], "Sigmoid")
+    if sm is None or sig is None:
+        g.fail("value head: WDL and plies-to-end layers behind value_fc0 without a Softmax behind the first or a Sigmoid "
+               "behind the second")
+    take(wdl, "wdl_out"), take(plys, "value_plys_to_end_fc")
+    m0 = g.downstream(sm[2][0], ("Gemm", "MatMul"))
+    if m0 is None:  # value = broadcast_add(-loss, win) of the split probabilities
+        if g.downstream(sm[2][0], ("Split",)) is None:
+            g.fail("value head: neither win - loss nor a value MLP behind the WDL output")
+        return "mx_wdl"
+    cat = g.back(m0[1][0], "Concat")
+    if len(cat[1]) != 2 or cat[1][0] != sm[2][0] or cat[1][1] != sig[2][0]:
+        g.fail("value head: the value MLP does not take Concat(WDL probabilities, plies)")
+    m1 = g.one(g.one(m0[2][0], "Relu")[2][0], "Gemm", True)
+    if g.weight(m1).shape[0] != 1 or g.first(m1[2][0], "Tanh") is None:
+        g.fail("value head: the value MLP does not end in one unit and Tanh")
+    take(m0, "value_wdl_ply_fc"), take(m1, "value_fc1")
+    return "mx_wdl_mlp"
+
+
+def _torch_value_mlp(g, wdl, plys):
+    """use_mlp_wdl_ply in a torch export (builder_util.py _ValueHead :315-320): behind the WDL Gemm and the plies Gemm's
+    Sigmoid, Concat(wdl, plies) -> Gemm (8) -> Relu -> Gemm (1) -> Tanh -> its two layers as [W0, b0, W1, b1]; None for
+    the WDL head without it"""
+    m0 = g.downstream(wdl[2][0], ("Gemm", "MatMul"))
+    if m0 is None:
+        return None
+    sig = g.first(plys[2][0], "Sigmoid")
+    cat = g.back(m0[1][0], "Concat")
+    if sig is None or len(cat[1]) != 2 or cat[1][0] != wdl[2][0] or cat[1][1] != sig[2][0]:
+        g.fail("value head: a fully-connected layer behind the WDL output that does not take Concat(WDL logits, "
+               "sigmoid(plies)), the value MLP's input")
+    if m0[0] != "Gemm":
+        g.fail("value head: the value MLP's first layer is not a Gemm")
+    m1 = g.one(g.one(m0[2][0], "Relu")[2][0], "Gemm", True)
+    if g.weight(m1).shape[0] != 1 or g.first(m1[2][0], "Tanh") is None:
+        g.fail("value head: the value MLP does not end in one unit and Tanh")
+    return [g.weight(m0), g.bias(m0), g.weight(m1), g.bias(m1)]
 
 
 def _import_folded_graph(g, blob_path, input_version, channels):
@@ -470,6 +537,7 @@ def _import_folded_graph(g, blob_path, input_version, channels):
     wdl = len(fc) == 2
     if wdl:
         fc = sorted(fc, key=lambda nd: -W(nd).shape[0])  # WDL (3 outputs), then plies (1)
+        mlp = _torch_value_mlp(g, *fc)
     elif len(fc) == 1:
         fc = [fc[0], g.downstream(fc[0][2][0], ("Gemm", "MatMul"))]
         if fc[1] is None:
@@ -478,6 +546,8 @@ def _import_folded_graph(g, blob_path, input_version, channels):
         g.fail(f"value head: {len(fc)} fully-connected layers behind the convolution")
     for nd in fc:
         tensors += [W(nd), bias(nd)]
+    if wdl and mlp is not None:
+        tensors += mlp
     p2 = g.downstream(pconv[0][2][0], ("Conv",))
     if p2 is None:
         g.fail("policy head: second convolution not found")
@@ -485,6 +555,8 @@ def _import_folded_graph(g, blob_path, input_version, channels):
     arch = dict(name=f"rise_{len(kernels)}b", in_channels=int(W(stem).shape[1]), policy_channels=int(W(p2).shape[0]),
                 channels=C, kernels=kernels, se_types=se_types, c_ops=c_ops, wdl=wdl, value_channels=int(W(vconv[0]).shape[0]),
                 value_fc=256)
+    if wdl and mlp is not None:
+        arch["value_head"] = "wdl_mlp"
     if widths:
         (M, Ca, H), = widths
         arch.update(name=f"alphavile_{len(kernels)}b", ntb=ntb, mhsa=M, mhca=Ca, mlp=H,

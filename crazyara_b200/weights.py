@@ -21,6 +21,12 @@ folded into q / k / v and mlp.conv1 the way the reference's merge_pre_bn does be
 A network with a fully-connected policy head (the trainer's select_policy_from_plane=False: policy_head.body2 BatchNorm
 + ReLU and policy_head.body3 Linear onto the classic labels; in the MXNet symbols policy_bn1, the activation and
 FullyConnected policy_out) is written as ARAB2004 around one of the three (write_blob).
+
+The base header's WDL word is the value head's kind (VALUE_HEADS, arch["value_head"]): 0 the standard head, 1 WDL and
+plies-to-end outputs with value = P(win) - P(loss), 2 the same outputs feeding the trainer's value MLP (use_mlp_wdl_ply:
+the WDL logits and the plies, 4 -> 8 -> 1, tanh), 3 and 4 the MXNet symbols' head with use_wdl and use_plys_to_end
+(builder_util_symbol.py value_head): a hidden layer value_fc0 of value_fc units in front of the WDL and plies outputs,
+then win - loss, or the MLP on the WDL probabilities.
 """
 import struct
 
@@ -32,6 +38,35 @@ MX_BN_EPS = 1e-3  # mx.sym.BatchNorm's default
 # squeeze-excitation gates: torch Hardsigmoid clamp(x / 6 + 0.5), MXNet hard_sigmoid clamp(0.2 x + 0.5), sigmoid
 GATE_CODE = {None: 0, "torch_hard_sigmoid": 0, "hard_sigmoid": 1, "sigmoid": 2}
 SHORTCUT_PRE_SE, SE_BIAS = 1, 2  # ARAB2002 block flags
+# the base header's WDL word: the value head's kind, by arch["value_head"] (absent: 0 or 1 by arch["wdl"])
+VALUE_HEADS = {"wdl_mlp": 2, "mx_wdl": 3, "mx_wdl_mlp": 4}
+VALUE_MLP = 8  # the hidden width of the trainers' value MLP (builder_util.py _ValueHead, builder_util_symbol.py value_head)
+
+
+def value_kind(arch):
+    """the value head's kind as the blob header holds it"""
+    return VALUE_HEADS[arch["value_head"]] if arch.get("value_head") else int(bool(arch["wdl"]))
+
+
+def check_value_head(kind, fc, n_policy, sizes):
+    """Checks a value head of kind `kind` with header word value_fc = fc against the element counts `sizes` of a blob's
+    tensors in order; the value head's tensors sit in front of the policy head's n_policy.  Raises ValueError naming what
+    is malformed: an unknown kind, a hidden layer outside 1 .. 256 units, an MLP whose width is not 8, other sizes."""
+    if kind not in (0, 1, *VALUE_HEADS.values()):
+        raise ValueError(f"value head of unknown kind {kind}")
+    if kind < 2:
+        return
+    if kind in (3, 4) and not 1 <= fc <= 256:
+        raise ValueError(f"value head: hidden layer of {fc} units (1 .. 256)")
+    hidden = 512 if kind == 2 else fc
+    head = ([fc * 512, fc] if kind in (3, 4) else []) + [3 * hidden, 3, hidden, 1]
+    if kind in (2, 4):
+        head += [4 * VALUE_MLP, VALUE_MLP, VALUE_MLP, 1]
+    got = list(sizes[max(len(sizes) - n_policy - len(head), 0):len(sizes) - n_policy])
+    if kind in (2, 4) and len(got) == len(head) and got[-4] != 4 * VALUE_MLP:
+        raise ValueError(f"value head: MLP of width {got[-4] / 4:g} (the trainers' MLP has {VALUE_MLP})")
+    if got != head:
+        raise ValueError(f"value head of kind {kind}: tensor sizes {got}, expected {head}")
 
 
 def _np(t):
@@ -94,6 +129,9 @@ def export_blob(sd, arch, path, input_version=10):
     if arch["wdl"]:
         put(_np(sd["value_head.body_wdl.0.weight"])), put(_np(sd["value_head.body_wdl.0.bias"]))
         put(_np(sd["value_head.body_plys.0.weight"])), put(_np(sd["value_head.body_plys.0.bias"]))
+        if arch.get("value_head") == "wdl_mlp":  # use_mlp_wdl_ply: body_final is the MLP on cat(wdl logits, plies)
+            for n in ("value_head.body_final.0", "value_head.body_final.2"):
+                put(_np(sd[n + ".weight"])), put(_np(sd[n + ".bias"]))
     else:
         put(_np(sd["value_head.body_final.0.weight"])), put(_np(sd["value_head.body_final.0.bias"]))
         put(_np(sd["value_head.body_final.2.weight"])), put(_np(sd["value_head.body_final.2.bias"]))
@@ -155,13 +193,16 @@ def write_blob(path, arch, tensors, input_version):
     n_labels = arch.get("n_labels")
     if n_labels and arch.get("policy_bias"):
         raise ValueError("ARAB2004 carries the policy convolution's bias with its head (policy_bias must be False)")
+    kind = value_kind(arch)
+    fc = arch.get("value_fc", 256) if v3 or kind in (3, 4) else 256
+    check_value_head(kind, fc, 6 if n_labels else 3 + bool(arch.get("policy_bias")), [np.size(t) for t in tensors])
     with open(path, "wb") as f:
         if n_labels:
             f.write(b"ARAB2004" + struct.pack("<2i", 3 if v3 else 2 if mx else 1, n_labels))
         else:
             f.write(b"ARAB2003" if v3 else b"ARAB2002" if mx else b"ARAB2001")
         f.write(struct.pack("<8i", arch["in_channels"], arch["policy_channels"], len(arch["kernels"]), C, 8,
-                            arch.get("value_fc", 256) if v3 else 256, 1 if arch["wdl"] else 0, input_version))
+                            fc, kind, input_version))
         if mx or v3:
             f.write(struct.pack("<2i", int(arch.get("stem_act", True)), int(arch.get("policy_bias", False))))
         for i, (k, se, cop) in enumerate(zip(arch["kernels"], arch["se_types"], arch["c_ops"])):
@@ -184,7 +225,7 @@ def read_blob(path):
     """The inverse of write_blob: an ARAB2001 / 2002 / 2003 / 2004 blob -> (arch, tensors [flat float32], input_version).  arch
     holds what the header and block table say, under write_blob's keys; write_blob(path2, *read_blob(path)) rewrites the
     file byte for byte.  A blob write_blob cannot have written (ARAB2002 block flags other than the ones it sets, an unknown
-    block type, a tensor past the end of the file) is refused."""
+    block type, a tensor past the end of the file, a malformed value head: check_value_head) is refused."""
     buf = open(path, "rb").read()
     magic = buf[:8]
     if magic not in (b"ARAB2001", b"ARAB2002", b"ARAB2003", b"ARAB2004"):
@@ -198,9 +239,11 @@ def read_blob(path):
             raise ValueError(f"{path}: {n_labels} policy labels (the classic label lists have {CLASSIC_LABELS})")
         magic, off = b"ARAB200%d" % base, 16
     mx, v3 = magic == b"ARAB2002", magic == b"ARAB2003"
-    cin, pch, n, C, vc, fc, wdl, version = struct.unpack_from("<8i", buf, off)
-    arch = dict(in_channels=cin, policy_channels=pch, channels=C, value_channels=vc, value_fc=fc, wdl=bool(wdl),
+    cin, pch, n, C, vc, fc, kind, version = struct.unpack_from("<8i", buf, off)
+    arch = dict(in_channels=cin, policy_channels=pch, channels=C, value_channels=vc, value_fc=fc, wdl=bool(kind),
                 kernels=[], se_types=[], c_ops=[])
+    if kind >= 2:
+        arch["value_head"] = {v: k for k, v in VALUE_HEADS.items()}.get(kind, kind)
     if n_labels:
         arch["n_labels"] = n_labels
     off += 32
@@ -236,6 +279,10 @@ def read_blob(path):
         size, = struct.unpack_from("<q", buf, off)
         tensors.append(np.frombuffer(buf, "<f4", size, off + 8).copy())
         off += 8 + 4 * size
+    try:
+        check_value_head(kind, fc, 6 if n_labels else 3 + arch.get("policy_bias", False), [t.size for t in tensors])
+    except ValueError as e:
+        raise ValueError(f"{path}: {e}") from None
     return arch, tensors, version
 
 
@@ -277,6 +324,13 @@ def eca_band(w, channels=256):
     return m
 
 
+# the FullyConnected layers of the symbols' value heads in blob order (builder_util_symbol.py value_head; the WDL layer
+# is named main_config["wdl_output"])
+MX_VALUE_LAYERS = {None: ("value_fc0", "value_fc1"),
+                   "mx_wdl": ("value_fc0", "wdl_out", "value_plys_to_end_fc"),
+                   "mx_wdl_mlp": ("value_fc0", "wdl_out", "value_plys_to_end_fc", "value_wdl_ply_fc", "value_fc1")}
+
+
 def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamma=True):
     """MXNet-named parameters (arg and aux params as the reference's symbol code names them) -> ARAB2002 blob.
     arch: as oracle.net_mx.arch_mx_risev2 / arch_mx_risev33 (semantics "mxnet", se_gates, stem_act, policy_bias).
@@ -285,7 +339,9 @@ def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamm
     widths below 128 are zero-padded to 128; the eca_se convolution becomes its banded 256 x 256 matrix.
     arch["n_labels"] set (select_policy_from_plane=False, builder_util_symbol.py policy_head): policy_conv1 is folded with
     policy_bn1, its bias included, and FullyConnected policy_out follows; the blob is ARAB2004 around ARAB2002, and
-    arch["policy_bias"] has to be False (the bias goes with the head)."""
+    arch["policy_bias"] has to be False (the bias goes with the head).  arch["value_head"] "mx_wdl" / "mx_wdl_mlp"
+    (use_wdl and use_plys_to_end, without or with use_mlp_wdl_ply): the layers MX_VALUE_LAYERS names, value_fc0 of
+    arch["value_fc"] units."""
     assert arch.get("semantics") == "mxnet"
     tensors = []
     put = tensors.append
@@ -316,7 +372,7 @@ def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamm
         put(w), put(b)
     w, b = fold("value_conv0", "value_bn0")
     put(w), put(b)
-    for n in ("value_fc0", "value_fc1"):
+    for n in MX_VALUE_LAYERS[arch.get("value_head")]:
         put(_np(params[n + "_weight"])), put(_np(params[n + "_bias"]))
     w, b = fold("policy_conv0", "policy_bn0")
     put(w), put(b)
@@ -334,7 +390,8 @@ def export_mx_blob(params, arch, path, input_version=10, eps=MX_BN_EPS, fix_gamm
 def arch_from_state_dict(sd):
     """Reads the architecture off a RiseV3 state_dict (rise_mobile_v3.py:81-183): block count, operating channels,
     depthwise kernel sizes, SE flavour per block, WDL head, input / policy channels; for AlphaVile (alpha_vile.py) also
-    the trunk width, the NTB positions and widths and the value head's hidden width."""
+    the trunk width, the NTB positions and widths and the value head's hidden width.  A WDL head whose body_final takes
+    4 inputs is the value MLP of use_mlp_wdl_ply (arch["value_head"] = "wdl_mlp")."""
     keys = set(sd.keys())
     is_ntb = lambda i: f"body_spatial.{i}.patch_embed.conv.weight" in keys
     n_blocks = 0
@@ -368,11 +425,15 @@ def arch_from_state_dict(sd):
                 value_fc=256)
     if "policy_head.body3.0.weight" in keys:  # select_policy_from_plane=False (builder_util.py _PolicyHead body2 / body3)
         arch["n_labels"] = int(sd["policy_head.body3.0.weight"].shape[0])
+    fc = sd.get("value_head.body_final.0.weight")
+    if arch["wdl"] and fc is not None and tuple(fc.shape)[1:] == (4,):
+        # use_mlp_wdl_ply: body_final is the MLP on cat(WDL logits, plies) (builder_util.py:292-296), not a layer of fc0 units
+        arch["value_head"] = "wdl_mlp"
+        fc = None
     if any(ntb) or C != 256:
         if len(widths) > 1:
             raise ValueError(f"NTB blocks of different widths {sorted(widths)}")
         (M, Ca, H), = widths or {(0, 0, 0)}
-        fc = sd.get("value_head.body_final.0.weight")
         arch.update(name=f"alphavile_{n_blocks}b", ntb=ntb, mhsa=M, mhca=Ca, mlp=H,
                     value_fc=C if fc is None else int(fc.shape[0]))
     return arch
