@@ -42,7 +42,7 @@ clean:
 
 # C++ host: UCI front-end over the C-ABI (no CUDA in this translation unit)
 UCI := crazyara_b200/ara_uci
-$(UCI): crazyara_b200/host/uci_main.cpp crazyara_b200/host/ara_host.h crazyara_b200/host/benchmark_positions.h include/ara_b200.h $(LIB)
-	g++ -O2 -std=c++17 -Wall -pthread -Iinclude -Icrazyara_b200/host $< -o $@ -Lcrazyara_b200 -lara_b200 -Wl,-rpath,'$$ORIGIN' -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64
+$(UCI): crazyara_b200/host/uci_main.cpp $(wildcard crazyara_b200/host/*.h) $(CSRC)/chess_dev.cuh include/ara_b200.h $(LIB)
+	g++ -O2 -std=c++17 -Wall -pthread -Iinclude -Icrazyara_b200/host -I$(CSRC) $< -o $@ -Lcrazyara_b200 -lara_b200 -Wl,-rpath,'$$ORIGIN' -L/usr/local/cuda/lib64 -Wl,-rpath,/usr/local/cuda/lib64
 
 all: $(UCI)

@@ -599,4 +599,70 @@ ARA_HD int policy_map_index(Move m, int stm, int chess960) {
     return (dir * 7 + len) * 64 + from;
 }
 
+// ------------------------------------------------------------------ classic-label index of a move
+// Index of the (rank-mirrored for black) UCI string in the classic label list of `mode` (0 crazyhouse 2272 labels,
+// 1 chess 1968, 2 lichess 2316; generate_uci_labels / generate_dropping_moves, outputrepresentation.cpp:108-163), what
+// a fully-connected policy head and the training data's y_policy are indexed by.  The list is computed arithmetically
+// in its generation order:
+//   1. per origin square, file-major (a1, a2, ..., h8): the rank destinations, the file destinations, both diagonals,
+//      the eight knight jumps -- 1792 labels;
+//   2. per origin file: the promotions to q, r, b, n (and k in mode 2), each as 2->1 and 7->8 straight, then to the
+//      left file, then to the right file;
+//   3. the drops P, N, B, R, Q per square, file-major, pawns not on the first and last rank (modes 0 and 2).
+// Castling is spelt as the policy map spells it: e1g1 / e1c1 outside chess960, king to rook square in chess960.
+ARA_HD int classic_moves_from(int f, int r) {  // labels of part 1 with origin file f, rank r
+    const int d1 = (f < r ? 7 - r + f : 7 - f + r), d2 = (f + r < 7 ? f + r : 14 - f - r);
+    int kn = 0;
+    const int kdx[8] = {-2, -1, -2, 1, 2, -1, 2, 1}, kdy[8] = {-1, -2, 1, -2, -1, 2, 1, 2};
+    for (int k = 0; k < 8; ++k) kn += (f + kdx[k] >= 0 && f + kdx[k] < 8 && r + kdy[k] >= 0 && r + kdy[k] < 8);
+    return 14 + d1 + d2 + kn;
+}
+ARA_HD int classic_label_index(Move m, int stm, int chess960, int mode) {
+    int from = mv_from(m), to = mv_to(m);
+    const int flag = mv_flag(m);
+    if (flag == MF_CASTLE && !chess960) to = (from & 56) | ((to & 7) > (from & 7) ? 6 : 2);
+    if (stm) {
+        from ^= 56;
+        to ^= 56;
+    }
+    constexpr int kQueenKnight = 1792;
+    const int n_promo = mode == 2 ? 5 : 4;
+    const int tf = to & 7, tr = to >> 3;
+    if (flag >= MF_DROP) {  // 5 labels per square, 4 on the first and last rank (no pawn)
+        if (mode == 1) return -1;
+        const int pt = flag - MF_DROP, sq = tf * 8 + tr;
+        const int before = 5 * sq - 2 * tf - (tr > 0 ? 1 : 0);  // pawnless squares (rank 1 and 8) of earlier files and this one
+        return kQueenKnight + n_promo * 44 + before + (tr == 0 || tr == 7 ? pt - 1 : pt);
+    }
+    const int ff = from & 7, fr = from >> 3;
+    if (flag >= MF_PROMO_N && flag <= MF_PROMO_Q) {
+        int start = kQueenKnight;
+        for (int f = 0; f < ff; ++f) start += n_promo * (2 + 2 * (f > 0) + 2 * (f < 7));
+        const int per = 2 + 2 * (ff > 0) + 2 * (ff < 7);
+        const int side = tf == ff ? 1 : (tf == ff - 1 ? 3 : (ff > 0 ? 5 : 3));
+        return start + (MF_PROMO_Q - flag) * per + side;
+    }
+    int idx = 0;
+    for (int s = 0; s < ff * 8 + fr; ++s) idx += classic_moves_from(s >> 3, s & 7);
+    const int dx = tf - ff, dy = tr - fr;
+    if (dy == 0) return idx + (tf < ff ? tf : tf - 1);
+    idx += 7;
+    if (dx == 0) return idx + (tr < fr ? tr : tr - 1);
+    idx += 7;
+    const int lo1 = -(ff < fr ? ff : fr), n1 = (ff < fr ? 7 - fr + ff : 7 - ff + fr);
+    if (dx == dy) return idx + dx - lo1 - (dx > 0 ? 1 : 0);
+    idx += n1;
+    const int lo2 = -(ff < 7 - fr ? ff : 7 - fr), n2 = (ff + fr < 7 ? ff + fr : 14 - ff - fr);
+    if (dx == -dy) return idx + dx - lo2 - (dx > 0 ? 1 : 0);
+    idx += n2;
+    const int kdx[8] = {-2, -1, -2, 1, 2, -1, 2, 1}, kdy[8] = {-1, -2, 1, -2, -1, 2, 1, 2};
+    for (int k = 0; k < 8; ++k) {
+        const int x = ff + kdx[k], y = fr + kdy[k];
+        if (x < 0 || x >= 8 || y < 0 || y >= 8) continue;
+        if (x == tf && y == tr) return idx;
+        ++idx;
+    }
+    return -1;
+}
+
 }  // namespace ara

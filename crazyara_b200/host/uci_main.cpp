@@ -1,7 +1,7 @@
 // Minimal UCI front-end over the C++ host classes (engine/src/uci/crazyara.cpp:76-143 command loop, option names of
 // uci/optionsuci.cpp:66-220).  Supported: uci, isready, setoption, ucinewgame, position [startpos|fen] [moves ...],
 // go [nodes N | movetime T | wtime W btime B [winc I] [binc I] [movestogo M]] (or the Simulations / Nodes options),
-// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], root, quit.  With Use_Raw_Network a `go`
+// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], selfplay N, root, quit.  With Use_Raw_Network a `go`
 // is answered by RawNetAgent (the network's policy alone) instead of a search.  The move time follows TimeManager::get_time_for_move (manager/timemanager.cpp:51-100) without its
 // random factor; the search then also stops after that much wall time (ara_search_set_movetime), and in clock games
 // the ThreadManager's early stopping / prolongation rules run on top (ara_search_set_time_control).
@@ -19,6 +19,7 @@
 
 #include "ara_host.h"
 #include "benchmark_positions.h"
+#include "selfplay.h"
 
 using namespace crazyara;
 
@@ -39,7 +40,30 @@ struct Options {
                                              // the reference's defaults (optionsuci.cpp:89-90, :182); Threads 1 and both epsilons 0
                                              // give the deterministic single-threaded search
                                              {"Threads", "2"},              {"Centi_Epsilon_Greedy", "5"},
-                                             {"Centi_Epsilon_Checks", "1"}};
+                                             {"Centi_Epsilon_Checks", "1"},
+                                             // self-play (the reference's USE_RL options, optionsuci.cpp:198-218, and the
+                                             // play settings `selfplay` samples its moves with, :102-154)
+                                             {"Centi_Node_Random_Factor", "10"}, {"Centi_Quick_Dirichlet_Epsilon", "0"},
+                                             {"Centi_Quick_Probability", "0"}, {"Centi_Quick_Q_Value_Weight", "70"},
+                                             {"Quick_Nodes", "100"},        {"Centi_Raw_Prob_Temperature", "25"},
+                                             {"MaxInitPly", "30"},          {"MeanInitPly", "15"},     {"EPD_File_Path", "<empty>"},
+                                             {"Centi_Resign_Probability", "90"}, {"Centi_Resign_Threshold", "-90"},
+                                             {"Milli_Policy_Clip_Thresh", "0"}, {"Selfplay_Number_Chunks", "640"},
+                                             {"Selfplay_Chunk_Size", "128"}, {"Centi_Temperature", "80"},
+                                             {"Temperature_Moves", "15"},   {"Centi_Temperature_Decay", "92"},
+                                             {"Centi_Quantile_Clipping", "0"},
+                                             // not in the reference: concurrent games of `selfplay` (one search tree each,
+                                             // sharing every network batch) and the seed of its move sampling
+                                             {"Selfplay_Games", "64"},      {"Selfplay_Seed", "0"}};
+    // the self-play options are spin options with the reference's ranges
+    std::map<std::string, std::pair<long, long>> range = {
+        {"Centi_Node_Random_Factor", {0, 100}}, {"Centi_Quick_Dirichlet_Epsilon", {0, 99999}}, {"Centi_Quick_Probability", {0, 100}},
+        {"Centi_Quick_Q_Value_Weight", {0, 99999}}, {"Quick_Nodes", {0, 99999}}, {"Centi_Raw_Prob_Temperature", {0, 100}},
+        {"MaxInitPly", {0, 99999}}, {"MeanInitPly", {0, 99999}}, {"Centi_Resign_Probability", {0, 100}},
+        {"Centi_Resign_Threshold", {-100, 100}}, {"Milli_Policy_Clip_Thresh", {0, 100}}, {"Selfplay_Number_Chunks", {1, 99999}},
+        {"Selfplay_Chunk_Size", {1, 99999}}, {"Centi_Temperature", {0, 99999}}, {"Temperature_Moves", {0, 99999}},
+        {"Centi_Temperature_Decay", {0, 100}}, {"Centi_Quantile_Clipping", {0, 100}}, {"Selfplay_Games", {1, 4096}},
+        {"Selfplay_Seed", {0, 2147483647}}};
     int i(const std::string& k) const { return std::stoi(kv.at(k)); }
     bool b(const std::string& k) const { return kv.at(k) == "true"; }
 };
@@ -82,9 +106,8 @@ int main() {
     bool searched = false;
     auto variant = [&]() { return variant_id(opt.kv["UCI_Variant"]); };
     auto new_game = [&]() { state.init(variant(), opt.b("UCI_Chess960")); };
-    auto prepare = [&]() {  // CrazyAra::is_ready (crazyara.cpp:597): build net + agent from the options
-        const int mode = mode_of_variant(variant());
-        SearchSettings s(mode);
+    auto search_settings = [&]() {  // CrazyAra::prepare_search_config_structs (crazyara.cpp:729-770)
+        SearchSettings s(mode_of_variant(variant()));
         s.batch_size = opt.i("Batch_Size");
         s.simulations = static_cast<unsigned>(opt.i("Simulations"));
         s.nodes = static_cast<unsigned>(opt.i("Nodes"));
@@ -105,6 +128,11 @@ int main() {
         s.epsilon_greedy_counter = opt.i("Centi_Epsilon_Greedy") > 0 ? static_cast<int>(std::lround(100.0 / opt.i("Centi_Epsilon_Greedy"))) : 0;
         s.epsilon_checks_counter = opt.i("Centi_Epsilon_Checks") > 0 ? static_cast<int>(std::lround(100.0 / opt.i("Centi_Epsilon_Checks"))) : 0;
         if (opt.i("Input_Version") > 0) s.input_version = opt.i("Input_Version");
+        return s;
+    };
+    auto prepare = [&]() {  // CrazyAra::is_ready (crazyara.cpp:597): build net + agent from the options
+        const int mode = mode_of_variant(variant());
+        SearchSettings s = search_settings();
         agent.reset();
         rawAgent.reset();
         net.reset();
@@ -166,7 +194,12 @@ int main() {
         try {
             if (cmd == "uci") {
                 std::cout << "id name CrazyAra-B200\nid author crazyara_b200 (hot path of QueensGambit/CrazyAra on sm_90a)\n";
-                for (const auto& kv : opt.kv) std::cout << "option name " << kv.first << " type string default " << kv.second << "\n";
+                for (const auto& kv : opt.kv) {
+                    std::cout << "option name " << kv.first;
+                    const auto r = opt.range.find(kv.first);
+                    if (r == opt.range.end()) std::cout << " type string default " << kv.second << "\n";
+                    else std::cout << " type spin default " << kv.second << " min " << r->second.first << " max " << r->second.second << "\n";
+                }
                 std::cout << "uciok" << std::endl;
             } else if (cmd == "isready") {
                 if (!ready) prepare();
@@ -176,8 +209,16 @@ int main() {
                 ss >> tok;  // "name"
                 while (ss >> tok && tok != "value") name += (name.empty() ? "" : " ") + tok;
                 while (ss >> tok) value += (value.empty() ? "" : " ") + tok;
+                const auto r = opt.range.find(name);
+                long v = 0;
+                size_t used = 0;
                 if (opt.kv.count(name) == 0) {
                     std::cout << "info string unknown option " << name << std::endl;
+                } else if (r != opt.range.end() &&
+                           ((void)(v = value.empty() ? 0 : std::stol(value, &used)), used == 0 || used != value.size() ||
+                            v < r->second.first || v > r->second.second)) {
+                    std::cout << "info string " << name << " takes an integer in [" << r->second.first << ", " << r->second.second
+                              << "]" << std::endl;
                 } else {
                     opt.kv[name] = value;
                     ready = false;
@@ -368,6 +409,48 @@ int main() {
                 const double elapsedMS = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
                 std::cout << "info string Inference results\ninfo string -----------------\ninfo string Elapsed time: " << elapsedMS / 1000.0
                           << " s\ninfo string Evaluations per second: " << (iterations / elapsedMS) * 1000.0 * B << " nps" << std::endl;
+            } else if (cmd == "selfplay") {  // CrazyAra::selfplay (crazyara.cpp:356-364): `selfplay N`, N = 0: until the data file is full
+                long numberOfGames = 0;
+                ss >> numberOfGames;
+                if (opt.kv["Model_Path"].empty()) {
+                    std::cout << "info string selfplay needs a network (setoption name Model_Path)" << std::endl;
+                    continue;
+                }
+                RLSettings rl;
+                rl.nodeRandomFactor = opt.i("Centi_Node_Random_Factor") / 100.0;
+                rl.quickDirichletEpsilon = opt.i("Centi_Quick_Dirichlet_Epsilon") / 100.0;
+                rl.quickProbability = opt.i("Centi_Quick_Probability") / 100.0;
+                rl.quickQValueWeight = opt.i("Centi_Quick_Q_Value_Weight") / 100.0;
+                rl.quickNodes = opt.i("Quick_Nodes");
+                rl.rawProbTemperature = opt.i("Centi_Raw_Prob_Temperature") / 100.0;
+                rl.maxInitPly = opt.i("MaxInitPly");
+                rl.meanInitPly = opt.i("MeanInitPly");
+                rl.epdFilePath = opt.kv["EPD_File_Path"];
+                rl.resignProbability = opt.i("Centi_Resign_Probability") / 100.0;
+                rl.resignThreshold = opt.i("Centi_Resign_Threshold") / 100.0;
+                rl.policyClipThresh = opt.i("Milli_Policy_Clip_Thresh") / 1000.0;
+                rl.numberChunks = opt.i("Selfplay_Number_Chunks");
+                rl.chunkSize = opt.i("Selfplay_Chunk_Size");
+                rl.temperature = opt.i("Centi_Temperature") / 100.0;
+                rl.temperatureMoves = opt.i("Temperature_Moves");
+                rl.temperatureDecay = opt.i("Centi_Temperature_Decay") / 100.0;
+                rl.quantileClipping = opt.i("Centi_Quantile_Clipping") / 100.0;
+                rl.reuseTree = opt.b("Reuse_Tree");
+                rl.games = opt.i("Selfplay_Games");
+                rl.seed = static_cast<uint64_t>(opt.i("Selfplay_Seed"));
+                const SearchSettings s = search_settings();
+                // the session's agent and network (`isready`) are released: self-play builds its own, whose batch holds
+                // the leaves of every game's tree (Selfplay_Games x Batch_Size rows); the next search rebuilds them
+                agent.reset();
+                rawAgent.reset();
+                net.reset();
+                ready = false;
+                searched = false;
+                NeuralNetAPI spNet("gpu", opt.i("First_Device_ID"), static_cast<unsigned>(rl.games * s.batch_size), opt.kv["Model_Path"],
+                                   opt.kv["Precision"]);
+                SelfPlay sp(&spNet, s, rl, variant(), opt.b("UCI_Chess960"), opt.i("First_Device_ID"));
+                sp.go(numberOfGames);
+                std::cout << "readyok" << std::endl;
             } else if (cmd == "root") {  // Node::print_node_statistics (node.cpp:1248-1301): the parity dump format
                 std::cout << "  #  | Move  |    Visits    |  Policy   |  Q-values  |  CP   \n";
                 std::cout << std::fixed << std::setprecision(7);
