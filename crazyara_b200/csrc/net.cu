@@ -546,20 +546,17 @@ int Net::build_ntb_precise(const BlockDesc& bd, const HostBlock& hb, int in, int
     return 0;
 }
 
-// The fully-connected policy head: W_fc [L][P * 64] (the trainer's NCHW flatten c * 64 + sq) -> fp16 [lp][K] with the
-// columns in the order of a board's row of d_pol_x: float16 sq * ldp + c (K = 64 ldp); float32 per square hi | lo | hi
-// parts cs wide (K = 64 * 3 cs) against the activations' hi | hi | lo.  Padding rows and columns are zero.
-int Net::build_policy_fc(const HostWeights& hw) {
-    const int L = hdr.n_classic, P = hdr.policy_channels;
-    const int lp = round_up(L, 64);
+int policy_fc_square_cols(int P, int precision) { return precision == 0 ? round_up(P, 32) : 3 * round_up(P, 64); }
+
+std::vector<__half> policy_fc_weight_image(const float* w_fc, int L, int P, int precision) {
     const int parts = precision == 0 ? 1 : 3;
-    const int cs = precision == 0 ? ldp : round_up(P, 64);
+    const int cs = policy_fc_square_cols(P, precision) / parts;
     const int K = 64 * parts * cs;
-    std::vector<__half> h(static_cast<size_t>(lp) * K, __float2half(0.0f));
+    std::vector<__half> h(static_cast<size_t>(round_up(L, 64)) * K, __float2half(0.0f));
     for (int l = 0; l < L; ++l)
         for (int c = 0; c < P; ++c)
             for (int sq = 0; sq < 64; ++sq) {
-                const float v = hw.fc_w[(static_cast<size_t>(l) * P + c) * 64 + sq];
+                const float v = w_fc[(static_cast<size_t>(l) * P + c) * 64 + sq];
                 const __half hi = __float2half_rn(v);
                 __half* col = &h[static_cast<size_t>(l) * K + static_cast<size_t>(sq) * parts * cs];
                 col[c] = hi;
@@ -568,24 +565,62 @@ int Net::build_policy_fc(const HostWeights& hw) {
                     col[2 * cs + c] = hi;
                 }
             }
+    return h;
+}
+
+void policy_fc_split(int L, int K, int* kb_per_split, int* splits) {
+    const int m_tiles = round_up(L, 64) / 64, num_kb = K / 64;
+    const int want = (kFcTargetCtas + m_tiles - 1) / m_tiles;
+    *kb_per_split = (num_kb + want - 1) / want;
+    *splits = (num_kb + *kb_per_split - 1) / *kb_per_split;
+}
+
+int policy_fc_choose_bn(int batch) { return batch <= 32 ? 32 : batch <= 64 ? 64 : 128; }
+
+int policy_fc_build(PolicyFcLayer* F, const __half* w, const float* bias, const __half* x, float* part, int L, int P,
+                    int precision, int rows_cap, int bn) {
+    const int lp = round_up(L, 64);
+    const int K = 64 * policy_fc_square_cols(P, precision);
+    int kb_per = 0;
+    policy_fc_split(L, K, &kb_per, &F->splits);
+    F->args = PolicyFcArgs{kb_per, K / 64, lp, rows_cap, part, nullptr};
+    F->bias = bias;
+    F->L = L;
+    F->bn = bn;
+    if (make_weight_tensor_map(&F->tm_w, w, K, lp, 64) || make_weight_tensor_map(&F->tm_x, x, K, rows_cap, bn)) return -1;
+    switch (bn) {
+        case 32: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<32>::kSmemBytes)); break;
+        case 64: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<64>::kSmemBytes)); break;
+        case 128: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<128>::kSmemBytes)); break;
+        default: return set_error("policy_fc_build: N tile %d (32, 64 or 128)", bn);
+    }
+    ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L * 4));
+    return 0;
+}
+
+int policy_fc_launch(const PolicyFcLayer& F, int n, float* prob, cudaStream_t s, const int* boards_dev) {
+    PolicyFcArgs a = F.args;
+    a.boards_dev = boards_dev;
+    const dim3 grid(a.lp / 64, F.splits, (n + F.bn - 1) / F.bn);
+    ARA_CUDA_OK(F.bn == 32 ? launch_pdl(policy_fc_kernel<32>, grid, dim3(kFcThreads), PolicyFcCfg<32>::kSmemBytes, s, F.tm_w, F.tm_x, a)
+                : F.bn == 64 ? launch_pdl(policy_fc_kernel<64>, grid, dim3(kFcThreads), PolicyFcCfg<64>::kSmemBytes, s, F.tm_w, F.tm_x, a)
+                             : launch_pdl(policy_fc_kernel<128>, grid, dim3(kFcThreads), PolicyFcCfg<128>::kSmemBytes, s, F.tm_w, F.tm_x, a));
+    ARA_CUDA_OK(launch_pdl(policy_fc_softmax_kernel, dim3(n), dim3(256), F.L * 4, s, static_cast<const float*>(a.part), F.bias, prob,
+                           F.L, a.lp, F.splits, a.rows_cap, boards_dev));
+    return 0;
+}
+
+// The fully-connected policy head on d_pol_x: float16 rows [batch_cap][64 ldp], float32 the split rows
+int Net::build_policy_fc(const HostWeights& hw) {
+    const int L = hdr.n_classic, P = hdr.policy_channels, lp = round_up(L, 64);
+    const std::vector<__half> h = policy_fc_weight_image(hw.fc_w.data(), L, P, precision);
     if (mem_.dalloc(&fc_w, h.size())) return -1;
     ARA_CUDA_OK(cudaMemcpy(fc_w, h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice));
     if (upload_f32(hw.fc_b.data(), L, lp, &fc_b)) return -1;
-    // the split count depends on L and K only, never on the batch: the partial sums of a board are the same in any batch
-    const int m_tiles = lp / 64, num_kb = K / 64;
-    const int want = (kFcTargetCtas + m_tiles - 1) / m_tiles;
-    const int kb_per = (num_kb + want - 1) / want;
-    fc_splits_ = (num_kb + kb_per - 1) / kb_per;
-    fc_bn_ = batch <= 32 ? 32 : batch <= 64 ? 64 : 128;
-    if (mem_.dalloc(&d_fc_part, static_cast<size_t>(fc_splits_) * batch_cap * lp)) return -1;
-    fc_args = PolicyFcArgs{kb_per, num_kb, lp, batch_cap, d_fc_part, nullptr};
-    if (make_weight_tensor_map(&fc_tm_w, fc_w, K, lp, 64) || make_weight_tensor_map(&fc_tm_x, d_pol_x, K, batch_cap, fc_bn_)) return -1;
-    switch (fc_bn_) {
-        case 32: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<32>::kSmemBytes)); break;
-        case 64: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<64>::kSmemBytes)); break;
-        default: ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, PolicyFcCfg<128>::kSmemBytes));
-    }
-    return 0;
+    int kb_per = 0, splits = 0;
+    policy_fc_split(L, 64 * policy_fc_square_cols(P, precision), &kb_per, &splits);
+    if (mem_.dalloc(&d_fc_part, static_cast<size_t>(splits) * batch_cap * lp)) return -1;
+    return policy_fc_build(&fc_, fc_w, fc_b, d_pol_x, d_fc_part, L, P, precision, batch_cap, policy_fc_choose_bn(batch));
 }
 
 // The policy head after the first convolution: the second convolution, then the softmax over its P * 64 logits, or the
@@ -594,15 +629,9 @@ int Net::launch_policy_head(int n, cudaStream_t s, const int* cnt, int io) {
     if (launch_conv(pol_conv2, n, s, cnt)) return -1;
     if (is_policy_map())
         return launch(policy_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_logits, io_prob[io], hdr.policy_channels, ldp, cnt);
-    PolicyFcArgs a = fc_args;
-    a.boards_dev = cnt;
-    const dim3 grid(a.lp / 64, fc_splits_, (n + fc_bn_ - 1) / fc_bn_);
-    const int rc = fc_bn_ == 32 ? launch(policy_fc_kernel<32>, grid, dim3(kFcThreads), PolicyFcCfg<32>::kSmemBytes, s, fc_tm_w, fc_tm_x, a)
-                 : fc_bn_ == 64 ? launch(policy_fc_kernel<64>, grid, dim3(kFcThreads), PolicyFcCfg<64>::kSmemBytes, s, fc_tm_w, fc_tm_x, a)
-                                : launch(policy_fc_kernel<128>, grid, dim3(kFcThreads), PolicyFcCfg<128>::kSmemBytes, s, fc_tm_w, fc_tm_x, a);
-    if (rc) return -1;
-    return launch(policy_fc_softmax_kernel, dim3(n), dim3(256), n_labels() * 4, s, d_fc_part, fc_b, io_prob[io], n_labels(), a.lp,
-                  fc_splits_, batch_cap, cnt);
+    if (policy_fc_launch(fc_, n, io_prob[io], s, cnt)) return -1;
+    launches += 2;
+    return 0;
 }
 
 int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
@@ -641,10 +670,8 @@ int Net::init(const char* blob_path, int dev, int batch_size, int prec) {
     io_in_h[0] = d_in_h, io_prob[0] = d_prob, io_value[0] = d_value, io_aux[0] = d_aux;
     ARA_CUDA_OK(cudaFuncSetAttribute(value_head_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      value_head_smem<__half>()));
-    if (is_policy_map())
+    if (is_policy_map())  // (the fully-connected head's softmax: policy_fc_build)
         ARA_CUDA_OK(cudaFuncSetAttribute(policy_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n_labels() * 4));
-    else
-        ARA_CUDA_OK(cudaFuncSetAttribute(policy_fc_softmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n_labels() * 4));
     ARA_CUDA_OK(cudaFuncSetAttribute(nchw_f32_to_nhwc_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      hdr.in_channels * 65 * 4));
     ARA_CUDA_OK(cudaDeviceSynchronize());
@@ -702,11 +729,26 @@ int Net::enqueue_precise(int n, cudaStream_t s, bool from_f32, const int* cnt, i
     return 0;
 }
 
+// The attention of an NTB of width M over n boards: grid (boards, heads).  float16: qkv [n * 64][3M] fp16 -> out
+// [n * 64][M] fp16; float32: qkv fp32 -> out the split [n * 64][3 * ceil64(M)] (hi | hi | lo).
+static cudaError_t ntb_attention_launch(int precision, const void* qkv, __half* out, int M, int n, cudaStream_t s, const int* cnt) {
+    if (precision == 0)
+        return launch_pdl(ntb_attention_kernel, dim3(n, M / kNtbHeadDim), dim3(128), 0, s, static_cast<const __half*>(qkv), out, M, cnt);
+    return launch_pdl(ntb_attention_f32_kernel, dim3(n, M / kNtbHeadDim), dim3(64), 0, s, static_cast<const float*>(qkv), out, M,
+                      round_up(M, 64), cnt);
+}
+
+int Net::launch_attention(const void* qkv, __half* out, int M, int n, cudaStream_t s, const int* cnt) {
+    ARA_CUDA_OK(ntb_attention_launch(precision, qkv, out, M, n, s, cnt));
+    ++launches;
+    return 0;
+}
+
 // y = patch_embed(x); q|k|v; attention; y1 = y + proj(attention); z = projection(y1); z2 = z + conv1x1(relu(group
 // conv(z))); x' = x2 + mlp2(relu(mlp1(x2))) with x2 = y1 | z2 -- 9 launches, next_vit_official_modules.py:321-335
 int Net::enqueue_ntb_half(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* cnt) {
     if (launch_conv(L.pe, n, s, cnt) || launch_conv(L.qkv, n, s, cnt) ||
-        launch(ntb_attention_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(128), 0, s, d_qkv, d_att, bd.ntb_m, cnt) ||
+        launch_attention(d_qkv, d_att, bd.ntb_m, n, s, cnt) ||
         launch_conv(L.proj, n, s, cnt) || launch_conv(L.prj, n, s, cnt) || launch_conv(L.gc, n, s, cnt) || launch_conv(L.mh, n, s, cnt) ||
         launch_conv(L.mlp1, n, s, cnt) || launch_conv(L.mlp2, n, s, cnt))
         return -1;
@@ -717,8 +759,7 @@ int Net::enqueue_ntb_half(const BlockDesc& bd, const NtbLayers& L, int n, cudaSt
 // conversion of x2 -- 10 launches
 int Net::enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* cnt) {
     if (launch_conv(L.pe, n, s, cnt) || launch_conv(L.qkv, n, s, cnt) ||
-        launch(ntb_attention_f32_kernel, dim3(n, bd.ntb_m / kNtbHeadDim), dim3(64), 0, s, d_qkvf, d_atts, bd.ntb_m, round_up(bd.ntb_m, 64),
-               cnt) ||
+        launch_attention(d_qkvf, d_atts, bd.ntb_m, n, s, cnt) ||
         launch_conv(L.proj, n, s, cnt) || launch_conv(L.prj, n, s, cnt) || launch_conv(L.gc, n, s, cnt) || launch_conv(L.mh, n, s, cnt) ||
         launch(f32_to_split256_kernel, dim3(n * 64), dim3(256), 0, s, d_x2f, d_x2s, cnt) || launch_conv(L.mlp1, n, s, cnt) ||
         launch_conv(L.mlp2, n, s, cnt))
@@ -939,4 +980,77 @@ extern "C" long long ara_net_launch_count(ara_net_t h) { return h ? reinterpret_
 extern "C" int ara_net_debug_trunk_cycles(ara_net_t h, unsigned long long* out32) {
     if (h == nullptr || out32 == nullptr) return ara::set_error("ara_net_debug_trunk_cycles: null argument");
     return reinterpret_cast<Net*>(h)->trunk_cycles(out32);
+}
+
+namespace {
+// the device-side board count of the debug entries: count >= 0 in a fresh device int, -1 none
+int debug_count(ara::DeviceBuffers* mem, int count, int** dev) {
+    *dev = nullptr;
+    if (count < 0) return 0;
+    if (mem->dalloc(dev, 1)) return -1;
+    ARA_CUDA_OK(cudaMemcpy(*dev, &count, sizeof(int), cudaMemcpyHostToDevice));
+    return 0;
+}
+}  // namespace
+
+extern "C" int ara_debug_ntb_attention(const void* qkv, int n, int M, int precision, int count, void* out) {
+    if (M < 32 || M % 32 != 0 || M > 224) return ara::set_error("ara_debug_ntb_attention: M %d (32 .. 224 in steps of 32)", M);
+    if (n < 1) return ara::set_error("ara_debug_ntb_attention: %d boards", n);
+    if (precision != ARA_PRECISION_FLOAT16 && precision != ARA_PRECISION_FLOAT32)
+        return ara::set_error("ara_debug_ntb_attention: precision %d (0 = float16, 1 = float32)", precision);
+    if (count < -1 || count > n) return ara::set_error("ara_debug_ntb_attention: board count %d of %d boards", count, n);
+    if (qkv == nullptr || out == nullptr) return ara::set_error("ara_debug_ntb_attention: null buffer");
+    const size_t rows = static_cast<size_t>(n) * 64;
+    const size_t in_bytes = rows * 3 * M * (precision == 0 ? 2 : 4);
+    const size_t out_bytes = rows * (precision == 0 ? M : 3 * ara::round_up(M, 64)) * 2;
+    ara::DeviceBuffers mem;
+    uint8_t *d_in = nullptr, *d_out = nullptr;
+    int* d_cnt = nullptr;
+    if (mem.dalloc(&d_in, in_bytes) || mem.dalloc(&d_out, out_bytes) || debug_count(&mem, count, &d_cnt)) return -1;
+    ARA_CUDA_OK(cudaMemcpy(d_in, qkv, in_bytes, cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(cudaMemcpy(d_out, out, out_bytes, cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(ara::ntb_attention_launch(precision, d_in, reinterpret_cast<__half*>(d_out), M, n, nullptr, d_cnt));
+    ARA_CUDA_OK(cudaMemcpy(out, d_out, out_bytes, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+extern "C" int ara_debug_policy_fc(int precision, int P, int L, int boards, int batch, int bn, int count, const float* w_fc,
+                                   const float* b_fc, const void* x, float* part, float* prob, int* splits_out, int* kb_per_split_out) {
+    if (precision != ARA_PRECISION_FLOAT16 && precision != ARA_PRECISION_FLOAT32)
+        return ara::set_error("ara_debug_policy_fc: precision %d (0 = float16, 1 = float32)", precision);
+    if (P < 1 || P > 256) return ara::set_error("ara_debug_policy_fc: %d policy planes (1 .. 256)", P);
+    if (L != 1968 && L != 2272 && L != 2316) return ara::set_error("ara_debug_policy_fc: %d labels (1968, 2272 or 2316)", L);
+    if (batch < 1 || boards < 1 || boards > batch) return ara::set_error("ara_debug_policy_fc: %d boards of a batch of %d", boards, batch);
+    if (bn != 0 && bn != 32 && bn != 64 && bn != 128) return ara::set_error("ara_debug_policy_fc: N tile %d (0, 32, 64 or 128)", bn);
+    if (count < -1 || count > boards) return ara::set_error("ara_debug_policy_fc: board count %d of %d boards", count, boards);
+    const int K = 64 * ara::policy_fc_square_cols(P, precision);
+    int kb_per = 0, splits = 0;
+    ara::policy_fc_split(L, K, &kb_per, &splits);
+    if (splits_out) *splits_out = splits;
+    if (kb_per_split_out) *kb_per_split_out = kb_per;
+    if (x == nullptr && part == nullptr && prob == nullptr) return 0;
+    if (w_fc == nullptr || b_fc == nullptr || x == nullptr || part == nullptr || prob == nullptr)
+        return ara::set_error("ara_debug_policy_fc: null buffer");
+    const int rows_cap = ara::round_up(batch < 2 ? 2 : batch, 2), lp = ara::round_up(L, 64);  // Net::batch_cap
+    const size_t part_bytes = static_cast<size_t>(splits) * rows_cap * lp * 4, prob_bytes = static_cast<size_t>(boards) * L * 4;
+    const std::vector<__half> img = ara::policy_fc_weight_image(w_fc, L, P, precision);
+    ara::DeviceBuffers mem;
+    __half *d_w = nullptr, *d_x = nullptr;
+    float *d_b = nullptr, *d_part = nullptr, *d_prob = nullptr;
+    int* d_cnt = nullptr;
+    if (mem.dalloc(&d_w, img.size()) || mem.dalloc(&d_x, static_cast<size_t>(rows_cap) * K) || mem.dalloc(&d_b, lp) ||
+        mem.dalloc(&d_part, part_bytes / 4) || mem.dalloc(&d_prob, prob_bytes / 4) || debug_count(&mem, count, &d_cnt))
+        return -1;
+    ARA_CUDA_OK(cudaMemcpy(d_w, img.data(), img.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(cudaMemcpy(d_x, x, static_cast<size_t>(rows_cap) * K * sizeof(__half), cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(cudaMemcpy(d_b, b_fc, static_cast<size_t>(L) * 4, cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(cudaMemcpy(d_part, part, part_bytes, cudaMemcpyHostToDevice));
+    ARA_CUDA_OK(cudaMemcpy(d_prob, prob, prob_bytes, cudaMemcpyHostToDevice));
+    ara::PolicyFcLayer F;
+    if (ara::policy_fc_build(&F, d_w, d_b, d_x, d_part, L, P, precision, rows_cap, bn ? bn : ara::policy_fc_choose_bn(batch)) ||
+        ara::policy_fc_launch(F, boards, d_prob, nullptr, d_cnt))
+        return -1;
+    ARA_CUDA_OK(cudaMemcpy(part, d_part, part_bytes, cudaMemcpyDeviceToHost));
+    ARA_CUDA_OK(cudaMemcpy(prob, d_prob, prob_bytes, cudaMemcpyDeviceToHost));
+    return 0;
 }

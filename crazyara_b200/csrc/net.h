@@ -29,6 +29,33 @@ constexpr int kBlobShortcutPreSe = 1, kBlobSeBias = 2;
 constexpr int kValueHeadStandard = 0, kValueHeadWdl = 1, kValueHeadWdlMlp = 2, kValueHeadMxWdl = 3, kValueHeadMxWdlMlp = 4;
 constexpr int kValueMlp = 8;  // the hidden width of the trainers' value MLP on (WDL, plies)
 
+// The fully-connected policy layer as a network builds and launches it: policy_fc_kernel<bn> over `splits` K ranges,
+// then policy_fc_softmax_kernel.  Net::build_policy_fc and ara_debug_policy_fc both build through policy_fc_build.
+struct PolicyFcLayer {
+    CUtensorMap tm_w, tm_x;
+    PolicyFcArgs args;
+    const float* bias;  // [lp] zero padded
+    int L, bn, splits;
+};
+// the columns of one square in a board's row of the layer's input: float16 ceil32(P) (the policy convolution's row
+// pitch), float32 3 * ceil64(P) (its split output hi | hi | lo); K = 64 times this
+int policy_fc_square_cols(int P, int precision);
+// W_fc [L][P * 64] (the trainer's NCHW flatten c * 64 + sq) -> the fp16 image [ceil64(L)][K] with the columns in the
+// order of the input rows: float16 sq * ceil32(P) + c, float32 per square hi | lo | hi parts ceil64(P) wide against the
+// activations' hi | hi | lo.  Padding rows and columns are zero.
+std::vector<__half> policy_fc_weight_image(const float* w_fc, int L, int P, int precision);
+// 64-wide K blocks per split and the split count: from L and K only, never from the batch, so that a board's partial
+// sums are the same in any batch
+void policy_fc_split(int L, int K, int* kb_per_split, int* splits);
+// the N tile (boards per CTA) for a layer built for `batch` boards
+int policy_fc_choose_bn(int batch);
+// w: the image of policy_fc_weight_image, bias [ceil64(L)], x: the input rows [rows_cap][K], part: [splits][rows_cap]
+// [ceil64(L)] fp32 partial sums
+int policy_fc_build(PolicyFcLayer* F, const __half* w, const float* bias, const __half* x, float* part, int L, int P,
+                    int precision, int rows_cap, int bn);
+// the two launches of the layer for n boards: prob [n][L]; boards_dev as in PolicyFcArgs
+int policy_fc_launch(const PolicyFcLayer& F, int n, float* prob, cudaStream_t s, const int* boards_dev);
+
 struct NetHeader {
     int in_channels;
     int policy_channels;
@@ -167,6 +194,7 @@ class Net {
     int build_ntb_precise(const BlockDesc& bd, const HostBlock& hb, int in, int out, NtbLayers* L);
     int enqueue_ntb_half(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* boards_dev);
     int enqueue_ntb_precise(const BlockDesc& bd, const NtbLayers& L, int n, cudaStream_t s, const int* boards_dev);
+    int launch_attention(const void* qkv, __half* out, int M, int n, cudaStream_t s, const int* boards_dev);
     DeviceBuffers mem_;
     int max_cop_ = 0;
     ConvLayer stem_conv;
@@ -199,9 +227,7 @@ class Net {
     __half* fc_w = nullptr;
     float* fc_b = nullptr;
     float* d_fc_part = nullptr;
-    CUtensorMap fc_tm_w, fc_tm_x;
-    PolicyFcArgs fc_args{};
-    int fc_bn_ = 0, fc_splits_ = 0;
+    PolicyFcLayer fc_{};
     int build_policy_fc(const HostWeights& hw);
     int launch_policy_head(int n, cudaStream_t s, const int* boards_dev, int io);
     struct Captured {

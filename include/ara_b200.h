@@ -374,6 +374,30 @@ typedef struct ara_debug_conv_s {
 } ara_debug_conv_t;
 int ara_debug_conv(const ara_debug_conv_t* args, void* stream);
 int ara_debug_choose_bn(int boards, int n_out);
+/* ara_debug_ntb_attention: the attention of one NTB of width M (M / 32 heads) on host buffers, launched as the network
+ * launches it (Net::enqueue_ntb_half / enqueue_ntb_precise); synchronous.
+ *   qkv   [n * 64][3M] q | k | v: fp16 for precision 0, fp32 for precision 1
+ *   count >= 0: a device-side board count of that value (<= n), as a search passes; -1: none
+ *   out   in: the initial contents, out: the result; fp16 [n * 64][M], or for precision 1 the split [n * 64][3 * ceil64(M)]
+ *         (hi | hi | lo)
+ * M outside 32 .. 224 or not a multiple of 32, n < 1 and other precisions are refused before any device call. */
+int ara_debug_ntb_attention(const void* qkv, int n, int M, int precision, int count, void* out);
+/* ara_debug_policy_fc: the fully-connected policy layer (policy_fc_kernel, then policy_fc_softmax_kernel) on host
+ * buffers, built and launched as the network builds and launches it (Net::build_policy_fc, launch_policy_head);
+ * synchronous.
+ *   P, L      policy planes (1 .. 256) and labels (1968, 2272 or 2316)
+ *   boards    boards launched, 1 .. batch; batch: the batch the layer is built for, which fixes the N tile and rows_cap
+ *             (batch rounded up to even, at least 2); bn 32, 64 or 128 forces the N tile, 0 takes the network's
+ *   count     >= 0: a device-side board count of that value (<= boards); -1: none
+ *   w_fc      [L][P * 64] (the trainer's NCHW flatten), b_fc [L]
+ *   x         the policy convolution's output as the layer reads it: fp16 [rows_cap][64 * ceil32(P)], or for precision 1
+ *             the split [rows_cap][64 * 3 * ceil64(P)] (per square hi | hi | lo)
+ *   part      in: initial contents, out: the fp32 partial sums [splits][rows_cap][ceil64(L)]
+ *   prob      in: initial contents, out: the probabilities [boards][L]
+ *   splits, kb_per_split   out (or NULL): the split count and the 64-wide K blocks per split of the layer
+ * With x, part and prob all NULL only splits and kb_per_split are reported, and no device is touched. */
+int ara_debug_policy_fc(int precision, int P, int L, int boards, int batch, int bn, int count, const float* w_fc,
+                        const float* b_fc, const void* x, float* part, float* prob, int* splits, int* kb_per_split);
 /* the residual tower kernel alone on host buffers, on the shape ARA_TRUNK_ROWS selects: x_half, out_half [n][64][256]
  * fp16; per block (no squeeze-excitation), one after the other: w1 [c_op][256], b1 [c_op], wd [c_op][k*k], bd [c_op],
  * w2 [256][c_op], b2 [256] (BN folded) */
