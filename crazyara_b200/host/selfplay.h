@@ -78,6 +78,64 @@ inline std::vector<double> normalised_power(const std::vector<double>& p, double
     return q;
 }
 
+// load_random_fen (selfplay.cpp:58-79): a uniformly drawn line of the EPD file without its trailing ';'; "" (the
+// variant's start position) without a file ("" or "<empty>")
+inline std::string load_random_fen(const std::string& path, NumpyRandom& rng) {
+    if (path.empty() || path == "<empty>") return "";
+    std::ifstream in(path);
+    if (!in) throw std::runtime_error(path + ": cannot open");
+    std::vector<std::string> lines;
+    for (std::string l; std::getline(in, l);) lines.push_back(l);
+    if (lines.empty()) throw std::runtime_error(path + ": no positions");
+    std::string line = lines[rng.integers(static_cast<int64_t>(lines.size()))];
+    if (!line.empty() && line.back() == ';') line.pop_back();
+    return line;
+}
+
+inline std::string chess960_fen(NumpyRandom& rng) {  // chess960fen (chess960position.h:36-80) on the driver's generator
+    char p[8] = {0};
+    p[2 * rng.integers(4)] = 'B';
+    p[2 * rng.integers(4) + 1] = 'B';
+    for (char c : std::string("QNN"))
+        while (true) {
+            const long loc = rng.integers(8);
+            if (!p[loc]) {
+                p[loc] = c;
+                break;
+            }
+        }
+    for (char c : std::string("RKR")) *std::find(p, p + 8, 0) = c;
+    std::string first(p, 8), lower = first;
+    for (char& c : lower) c = static_cast<char>(std::tolower(c));
+    return lower + "/pppppppp/8/8/8/8/PPPPPPPP/" + first + " w KQkq - 0 1";
+}
+
+// the FEN of a new game: a random EPD line, else a random chess960 set-up (chess only), else "" (the start position)
+inline std::string start_fen(NumpyRandom& rng, int variant, bool is960, const std::string& epdFilePath) {
+    std::string fen = load_random_fen(epdFilePath, rng);
+    if (fen.empty() && is960 && variant == 0) fen = chess960_fen(rng);
+    return fen;
+}
+
+// Agent::set_best_move (agents/agent.cpp:38-53) with get_current_temperature (playsettings.cpp:31-34): the index of the
+// move to play at game ply `ply`, sampled from the search's policy while the temperature lasts, else the best move
+inline size_t set_best_move(const std::vector<double>& pol, int bestIdx, int ply, NumpyRandom& rng, const RLSettings& rl) {
+    if (ply < rl.temperatureMoves && rl.temperature > 0.01 && pairwise_sum(pol) > 0) {
+        const double temp = rl.temperature * std::pow(rl.temperatureDecay, ply);
+        std::vector<double> p = normalised_power(pol, 1.0 / temp);
+        if (rl.quantileClipping != 0) p = quantile_clip(p, rl.quantileClipping);
+        return rng.choice(p);
+    }
+    return static_cast<size_t>(bestIdx);
+}
+
+// WHITE_WIN / BLACK_WIN / DRAWN of a game that ended with `term`, `stmAtEnd` (0 white) to move: that side lost (mate,
+// variant loss) or won (variant win); everything else is a draw
+inline Result game_result(TerminalType term, int stmAtEnd) {
+    return term == TERMINAL_LOSS ? (stmAtEnd == 0 ? BLACK_WIN : WHITE_WIN)
+                                 : (term == TERMINAL_WIN ? (stmAtEnd == 0 ? WHITE_WIN : BLACK_WIN) : DRAWN);
+}
+
 class SelfPlay {
    public:
     // net: batch size >= rl.games * settings.batch_size; files go to the working directory, named after `device`
@@ -142,38 +200,7 @@ class SelfPlay {
             if (ply > rl_.maxInitPly) ply = rng_.integers(int64_t{1} << 31) % rl_.maxInitPly;
             initPlies_[t] = static_cast<int>(ply);
         }
-        std::string fen = load_random_fen();
-        if (fen.empty() && is960_ && variant_ == 0) fen = chess960_fen();
-        states_[t].set(fen, is960_, variant_);
-    }
-    std::string load_random_fen() {  // load_random_fen (selfplay.cpp:58-79)
-        const std::string& path = rl_.epdFilePath;
-        if (path.empty() || path == "<empty>") return "";
-        std::ifstream in(path);
-        if (!in) throw std::runtime_error(path + ": cannot open");
-        std::vector<std::string> lines;
-        for (std::string l; std::getline(in, l);) lines.push_back(l);
-        if (lines.empty()) throw std::runtime_error(path + ": no positions");
-        std::string line = lines[rng_.integers(static_cast<int64_t>(lines.size()))];
-        if (!line.empty() && line.back() == ';') line.pop_back();
-        return line;
-    }
-    std::string chess960_fen() {  // chess960fen (chess960position.h:36-80) on the arena's generator
-        char p[8] = {0};
-        p[2 * rng_.integers(4)] = 'B';
-        p[2 * rng_.integers(4) + 1] = 'B';
-        for (char c : std::string("QNN"))
-            while (true) {
-                const long loc = rng_.integers(8);
-                if (!p[loc]) {
-                    p[loc] = c;
-                    break;
-                }
-            }
-        for (char c : std::string("RKR")) *std::find(p, p + 8, 0) = c;
-        std::string first(p, 8), lower = first;
-        for (char& c : lower) c = static_cast<char>(std::tolower(c));
-        return lower + "/pppppppp/8/8/8/8/PPPPPPPP/" + first + " w KQkq - 0 1";
+        states_[t].set(start_fen(rng_, variant_, is960_, rl_.epdFilePath), is960_, variant_);
     }
     bool draw_resign() { return rl_.resignProbability >= 0.01 && rng_.random() < rl_.resignProbability; }
 
@@ -252,8 +279,7 @@ class SelfPlay {
     }
 
     void game_over(int t, TerminalType term, int stmAtEnd) {
-        const Result result = term == TERMINAL_LOSS ? (stmAtEnd == 0 ? BLACK_WIN : WHITE_WIN)
-                                                    : (term == TERMINAL_WIN ? (stmAtEnd == 0 ? WHITE_WIN : BLACK_WIN) : DRAWN);
+        const Result result = game_result(term, stmAtEnd);
         if (!exporter_->is_file_full()) ++gameIdx_;
         const long samples = exporter_->export_game_samples(records_[t], result);
         records_[t] = TrainDataExporter::Game();
@@ -309,7 +335,7 @@ class SelfPlay {
                 continue;
             }
             const std::vector<double> policy(r.policy, r.policy + r.n_moves);
-            const size_t idx = pick(policy, r.best_idx, plies_[t]);
+            const size_t idx = set_best_move(policy, r.best_idx, plies_[t], rng_, rl_);
             if (!quick_[t]) {  // a quick search exports nothing (selfplay.cpp:228); the policy is sharpened after the pick
                 const std::vector<double> sharp = sharpen_distribution(policy, rl_.policyClipThresh);
                 exporter_->save_sample(records_[t], &planes[static_cast<size_t>(t) * channels_ * 64], r.moves, sharp.data(), r.n_moves,
@@ -326,16 +352,6 @@ class SelfPlay {
         play_openings();
     }
 
-    // Agent::set_best_move (agents/agent.cpp:38-53) with get_current_temperature (playsettings.cpp:31-34)
-    size_t pick(const std::vector<double>& pol, int bestIdx, int ply) {
-        if (ply < rl_.temperatureMoves && rl_.temperature > 0.01 && pairwise_sum(pol) > 0) {
-            const double temp = rl_.temperature * std::pow(rl_.temperatureDecay, ply);
-            std::vector<double> p = normalised_power(pol, 1.0 / temp);
-            if (rl_.quantileClipping != 0) p = quantile_clip(p, rl_.quantileClipping);
-            return rng_.choice(p);
-        }
-        return static_cast<size_t>(bestIdx);
-    }
     static void check(int rc) {
         if (rc != 0) throw std::runtime_error(ara_last_error());
     }

@@ -4,6 +4,8 @@
 //   TrainDataExporter  crazyara_b200.export.TrainDataExporter (rl/traindataexporter.cpp): the uncompressed zarr v2 store
 //   GamePGN          crazyara_b200.pgn.GamePGN (rl/gamepgn.cpp): the PGN stream of the self-play games
 //   write_game_idx   SelfPlay::export_number_generated_games (rl/selfplay.cpp:353-359): gameIdx_<device>.txt
+//   TournamentResult crazyara_b200.match.TournamentResult (rl/tournamentresult.{h,cpp}): an arena's score, its text and
+//                    CSV line, and the verdict
 // Header-only; no CUDA in this file (the classic-label index is the __host__ __device__ one of chess_dev.cuh).
 #pragma once
 #include <sys/stat.h>
@@ -15,6 +17,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <fstream>
+#include <iomanip>
 #include <sstream>
 #include <stdexcept>
 #include <string>
@@ -351,5 +354,29 @@ class GamePGN {
 };
 
 inline void write_game_idx(const std::string& path, long games) { std::ofstream(path, std::ios::binary | std::ios::trunc) << games; }
+
+// ---------------------------------------------------------------------------------------------------- arena result
+// The result of a match from the view of player A (the contender).
+struct TournamentResult {
+    std::string playerA, playerB;
+    long wins = 0, draws = 0, losses = 0;
+
+    long games() const { return wins + draws + losses; }
+    float score() const {  // (W + 0.5 D) / games in float32, as score() computes it
+        return (static_cast<float>(wins) + static_cast<float>(draws) * 0.5f) / static_cast<float>(games());
+    }
+    // what the arena prints after its summary: the contender replaces the producer if it scored above 0.5
+    const char* verdict() const { return score() > 0.5f ? "replace" : "keep"; }
+    std::string str() const {  // operator<<: "<A>-<B>: W - D - L [score]", the score at precision 2
+        std::ostringstream o;
+        o << playerA << "-" << playerB << ": " << wins << " - " << draws << " - " << losses << " [" << std::setprecision(2) << score() << "]";
+        return o.str();
+    }
+    std::string csv_line() const {
+        return playerA + "," + playerB + "," + std::to_string(wins) + "," + std::to_string(draws) + "," + std::to_string(losses) + "\n";
+    }
+    // write_tournament_result_to_csv: appends "A,B,W,D,L"
+    void write_csv(const std::string& path) const { std::ofstream(path, std::ios::app | std::ios::binary) << csv_line(); }
+};
 
 }  // namespace crazyara

@@ -1,8 +1,11 @@
 // Minimal UCI front-end over the C++ host classes (engine/src/uci/crazyara.cpp:76-143 command loop, option names of
 // uci/optionsuci.cpp:66-220).  Supported: uci, isready, setoption, ucinewgame, position [startpos|fen] [moves ...],
 // go [nodes N | movetime T | wtime W btime B [winc I] [binc I] [movestogo M]] (or the Simulations / Nodes options),
-// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], selfplay N, root, quit.  With Use_Raw_Network a `go`
-// is answered by RawNetAgent (the network's policy alone) instead of a search.  The move time follows TimeManager::get_time_for_move (manager/timemanager.cpp:51-100) without its
+// go infinite + stop, benchmark <movetime>, inference [warmup N] [iterations N], selfplay N, arena N, activeuci, root, quit.
+// With Use_Raw_Network a `go` is answered by RawNetAgent (the network's policy alone) instead of a search.  `arena N`
+// plays N games of the network of Model_Path_Contender against the one of Model_Path (CrazyAra::arena,
+// crazyara.cpp:366-385) and ends with `replace` or `keep`; `activeuci` prints every option's current value
+// (CrazyAra::activeuci, :348-353).  The move time follows TimeManager::get_time_for_move (manager/timemanager.cpp:51-100) without its
 // random factor; the search then also stops after that much wall time (ara_search_set_movetime), and in clock games
 // the ThreadManager's early stopping / prolongation rules run on top (ara_search_set_time_control).
 #include <algorithm>
@@ -19,7 +22,7 @@
 
 #include "ara_host.h"
 #include "benchmark_positions.h"
-#include "selfplay.h"
+#include "match.h"
 
 using namespace crazyara;
 
@@ -27,6 +30,9 @@ namespace {
 
 struct Options {
     std::map<std::string, std::string> kv = {{"UCI_Variant", "crazyhouse"}, {"Model_Path", ""},        {"Batch_Size", "16"},
+                                             // the network `arena` plays against Model_Path's (the reference's
+                                             // Model_Directory_Contender, a weight blob here as Model_Path is)
+                                             {"Model_Path_Contender", ""},
                                              {"Simulations", "800"},        {"Nodes", "0"},            {"Centi_CPuct_Init", "250"},
                                              {"CPuct_Base", "19652"},       {"Centi_Node_Temperature", "170"},
                                              {"Centi_Dirichlet_Epsilon", "0"}, {"Centi_Dirichlet_Alpha", "20"},
@@ -129,6 +135,40 @@ int main() {
         s.epsilon_checks_counter = opt.i("Centi_Epsilon_Checks") > 0 ? static_cast<int>(std::lround(100.0 / opt.i("Centi_Epsilon_Checks"))) : 0;
         if (opt.i("Input_Version") > 0) s.input_version = opt.i("Input_Version");
         return s;
+    };
+    auto rl_settings = [&]() {  // the RL options of `selfplay` and `arena` (OptionsUCI::init_rl_settings, optionsuci.cpp)
+        RLSettings rl;
+        rl.nodeRandomFactor = opt.i("Centi_Node_Random_Factor") / 100.0;
+        rl.quickDirichletEpsilon = opt.i("Centi_Quick_Dirichlet_Epsilon") / 100.0;
+        rl.quickProbability = opt.i("Centi_Quick_Probability") / 100.0;
+        rl.quickQValueWeight = opt.i("Centi_Quick_Q_Value_Weight") / 100.0;
+        rl.quickNodes = opt.i("Quick_Nodes");
+        rl.rawProbTemperature = opt.i("Centi_Raw_Prob_Temperature") / 100.0;
+        rl.maxInitPly = opt.i("MaxInitPly");
+        rl.meanInitPly = opt.i("MeanInitPly");
+        rl.epdFilePath = opt.kv["EPD_File_Path"];
+        rl.resignProbability = opt.i("Centi_Resign_Probability") / 100.0;
+        rl.resignThreshold = opt.i("Centi_Resign_Threshold") / 100.0;
+        rl.policyClipThresh = opt.i("Milli_Policy_Clip_Thresh") / 1000.0;
+        rl.numberChunks = opt.i("Selfplay_Number_Chunks");
+        rl.chunkSize = opt.i("Selfplay_Chunk_Size");
+        rl.temperature = opt.i("Centi_Temperature") / 100.0;
+        rl.temperatureMoves = opt.i("Temperature_Moves");
+        rl.temperatureDecay = opt.i("Centi_Temperature_Decay") / 100.0;
+        rl.quantileClipping = opt.i("Centi_Quantile_Clipping") / 100.0;
+        rl.reuseTree = opt.b("Reuse_Tree");
+        rl.games = opt.i("Selfplay_Games");
+        rl.seed = static_cast<uint64_t>(opt.i("Selfplay_Seed"));
+        return rl;
+    };
+    // the session's agent and network (`isready`) are released before `selfplay` and `arena` build their own; the next
+    // search rebuilds them
+    auto release_session = [&]() {
+        agent.reset();
+        rawAgent.reset();
+        net.reset();
+        ready = false;
+        searched = false;
     };
     auto prepare = [&]() {  // CrazyAra::is_ready (crazyara.cpp:597): build net + agent from the options
         const int mode = mode_of_variant(variant());
@@ -416,40 +456,54 @@ int main() {
                     std::cout << "info string selfplay needs a network (setoption name Model_Path)" << std::endl;
                     continue;
                 }
-                RLSettings rl;
-                rl.nodeRandomFactor = opt.i("Centi_Node_Random_Factor") / 100.0;
-                rl.quickDirichletEpsilon = opt.i("Centi_Quick_Dirichlet_Epsilon") / 100.0;
-                rl.quickProbability = opt.i("Centi_Quick_Probability") / 100.0;
-                rl.quickQValueWeight = opt.i("Centi_Quick_Q_Value_Weight") / 100.0;
-                rl.quickNodes = opt.i("Quick_Nodes");
-                rl.rawProbTemperature = opt.i("Centi_Raw_Prob_Temperature") / 100.0;
-                rl.maxInitPly = opt.i("MaxInitPly");
-                rl.meanInitPly = opt.i("MeanInitPly");
-                rl.epdFilePath = opt.kv["EPD_File_Path"];
-                rl.resignProbability = opt.i("Centi_Resign_Probability") / 100.0;
-                rl.resignThreshold = opt.i("Centi_Resign_Threshold") / 100.0;
-                rl.policyClipThresh = opt.i("Milli_Policy_Clip_Thresh") / 1000.0;
-                rl.numberChunks = opt.i("Selfplay_Number_Chunks");
-                rl.chunkSize = opt.i("Selfplay_Chunk_Size");
-                rl.temperature = opt.i("Centi_Temperature") / 100.0;
-                rl.temperatureMoves = opt.i("Temperature_Moves");
-                rl.temperatureDecay = opt.i("Centi_Temperature_Decay") / 100.0;
-                rl.quantileClipping = opt.i("Centi_Quantile_Clipping") / 100.0;
-                rl.reuseTree = opt.b("Reuse_Tree");
-                rl.games = opt.i("Selfplay_Games");
-                rl.seed = static_cast<uint64_t>(opt.i("Selfplay_Seed"));
+                const RLSettings rl = rl_settings();
                 const SearchSettings s = search_settings();
-                // the session's agent and network (`isready`) are released: self-play builds its own, whose batch holds
-                // the leaves of every game's tree (Selfplay_Games x Batch_Size rows); the next search rebuilds them
-                agent.reset();
-                rawAgent.reset();
-                net.reset();
-                ready = false;
-                searched = false;
+                // self-play's network batch holds the leaves of every game's tree (Selfplay_Games x Batch_Size rows)
+                release_session();
                 NeuralNetAPI spNet("gpu", opt.i("First_Device_ID"), static_cast<unsigned>(rl.games * s.batch_size), opt.kv["Model_Path"],
                                    opt.kv["Precision"]);
                 SelfPlay sp(&spNet, s, rl, variant(), opt.b("UCI_Chess960"), opt.i("First_Device_ID"));
                 sp.go(numberOfGames);
+                std::cout << "readyok" << std::endl;
+            } else if (cmd == "arena") {  // CrazyAra::arena (crazyara.cpp:366-385): `arena N`, contender against producer
+                std::string tok;
+                ss >> tok;
+                long numberOfGames = 0;
+                size_t used = 0;
+                try {
+                    numberOfGames = std::stol(tok, &used);
+                } catch (const std::exception&) {
+                    used = 0;
+                }
+                const std::string producerPath = opt.kv["Model_Path"], contenderPath = opt.kv["Model_Path_Contender"];
+                if (producerPath.empty()) {
+                    std::cout << "info string arena needs the producer's network (setoption name Model_Path)" << std::endl;
+                    continue;
+                }
+                if (contenderPath.empty()) {
+                    std::cout << "info string arena needs the contender's network (setoption name Model_Path_Contender)" << std::endl;
+                    continue;
+                }
+                if (used == 0 || used != tok.size() || numberOfGames < 1) {
+                    std::cout << "info string arena takes a number of games of at least 1" << std::endl;
+                    continue;
+                }
+                const RLSettings rl = rl_settings();
+                const SearchSettings s = search_settings();
+                release_session();
+                // every network's batch holds the leaves of all of its handle's trees; one network for equal paths
+                const unsigned batch = static_cast<unsigned>(std::min<long>(rl.games, numberOfGames) * s.batch_size);
+                const int device = opt.i("First_Device_ID");
+                std::unique_ptr<NeuralNetAPI> producer(new NeuralNetAPI("gpu", device, batch, producerPath, opt.kv["Precision"])), contender;
+                if (contenderPath != producerPath) contender.reset(new NeuralNetAPI("gpu", device, batch, contenderPath, opt.kv["Precision"]));
+                Match match(producer.get(), contender ? contender.get() : producer.get(), player_name(producerPath), player_name(contenderPath),
+                            s, rl, numberOfGames, variant(), opt.b("UCI_Chess960"), device, "arena_games_gpu_" + std::to_string(device) + ".pgn",
+                            true);
+                const TournamentResult& result = match.run();
+                std::cout << "Arena summary\nScore of Contender vs Producer: " << result.str() << "\n" << result.verdict() << std::endl;
+                result.write_csv("arena_results.csv");
+            } else if (cmd == "activeuci") {  // CrazyAra::activeuci (crazyara.cpp:348-353)
+                for (const auto& kv : opt.kv) std::cout << "option name " << kv.first << " value " << kv.second << "\n";
                 std::cout << "readyok" << std::endl;
             } else if (cmd == "root") {  // Node::print_node_statistics (node.cpp:1248-1301): the parity dump format
                 std::cout << "  #  | Move  |    Visits    |  Policy   |  Q-values  |  CP   \n";
